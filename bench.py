@@ -1,22 +1,27 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native Fish-Speech hot path.
+"""bench.py — headline benchmark of the H100-native (sm_90a) Fish-Speech hot path.
 
 Workload (BASELINE.json configs[2]): batch-32 text->codec->wav, 64-token prompts, 256 codec frames per
 utterance, bf16, greedy (top_k=1), synthetic seeded weights at the assumed S2-Pro geometry
 (SURVEY.md §8) — one "step" = the whole batch: prefill + 255 decode frames (+ codec decode to waveform
 once the codec stage is present in this build; `config.stages` says which stages were timed).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Prints ONE JSON line.  `value` = audio-seconds generated per second (whole job, all GPUs) with the prompts
 resident in HBM; `e2e` = the same through the public API (`generate_batch`) from pinned host memory,
 including H2D of the prompts and D2H of the generated codes; `roofline` = measured HBM stream of the
-dominant kernel (the tcgen05 weight-streaming step GEMM) against MEASURED_PEAKS.json, in the frame and as a
-GEMM-only replay; `cpu_baseline` = the reference's CPU path (oracle/cpu_baseline.py) timed on this box's host
+dominant kernel (the wgmma weight-streaming step GEMM) against MEASURED_PEAKS.json (else the H100 SXM data sheet), in
+the frame and as a GEMM-only replay; `cpu_baseline` = the reference's CPU path (oracle/cpu_baseline.py) timed on this box's host
 cores on a bounded sample.
 
 Under torchrun (N > 1) every rank runs a full replica on its own shard of utterances (32 per GPU, weak
 scaling, no collective on the data path); times are device-side, max over ranks.
+
+--dump-outputs DIR writes what the last timed step computed (rank 0), as float32 .npy files: `codes.npy` = the
+generated tokens [batch, codebooks + 1, frames] and `wav.npy` = every 4th sample of the decoded waveforms
+(flattened [batch, 1, frames * 2048]; 16 MB at the default size).  Prompts, weights and sampling seeds are fixed,
+so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -83,7 +88,7 @@ def make_prompts(cfg, n, first_seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -118,26 +123,17 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(self.rows)}
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed
-    `ncu --set full` capture (profiles/r02_step_gemm_ncu_full.json); None if no capture is committed."""
-    try:
-        d = json.loads((ROOT / "profiles" / "r02_step_gemm_ncu_full.json").read_text())
-        return d["avg_dram_bytes_per_launch"]
-    except Exception:
-        return None
-
-
 def peaks():
     try:
         return json.loads((ROOT / "MEASURED_PEAKS.json").read_text()), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # H100 SXM data sheet (700 W): dense BF16, HBM3
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "datasheet"
 
 
 def cpu_reference(steps: int, warmup: int):
-    """The reference's own CPU implementation of the path on this box's host cores (oracle/cpu_baseline.py:
-    the unmodified reference modules when /root/reference exists, else the pinned oracle port)."""
+    """The reference's CPU implementation of the path on the host cores (oracle/cpu_baseline.py: the oracle port
+    pinned to the reference)."""
     from oracle import cpu_baseline
 
     return cpu_baseline.measure(steps, warmup)
@@ -313,7 +309,7 @@ def roundtrip_bench(args):
         codes, lens = dac.encode(wav_host.to(dev, non_blocking=True))
         return dac.from_indices(codes).cpu(), codes
 
-    ms, (wav, codes) = _timed_events(step, max(args.steps, 10), 3)
+    ms, (wav, codes) = _timed_events(step, args.steps, 3)
     enc_ms, _ = _timed_events(lambda: dac.encode(wav_host.to(dev)), 10, 2)
     dec_ms, _ = _timed_events(lambda: dac.from_indices(codes), 10, 2)
     cpu = None
@@ -337,7 +333,7 @@ def roundtrip_bench(args):
                "sample": f"the same 1 s clip, fp32: encode {1e3 * (t1 - t0):.0f} ms + decode {1e3 * (t2 - t1):.0f} ms"}
     v = (codes.shape[-1] * FRAME / SR) / (ms / 1e3)
     print(json.dumps({
-        "metric": "audio-sec/s", "value": v, "unit": "audio-s/s", "n_gpus": 1, "steps": max(args.steps, 10), "warmup": 3,
+        "metric": "audio-sec/s", "value": v, "unit": "audio-s/s", "n_gpus": 1, "steps": args.steps, "warmup": 3,
         "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
         "data": "synthetic",
         "config": {"workload": "Firefly VQ-GAN (391 M DAC) encode -> decode roundtrip, 1 s 44.1 kHz mono, batch 1",
@@ -495,6 +491,8 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's generated codes and waveform as .npy files")
     ap.add_argument("--frames", type=int, default=N_FRAMES)
     ap.add_argument("--batch", type=int, default=B_PER_GPU)
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -601,12 +599,14 @@ def main():
         codes = eng.buffer("out_tokens")[:B, 1:, :NF].contiguous()
         return dac.from_indices(codes)
 
+    last = {}
+
     def step_resident():
         eng.reset()
         eng.prefill(prompts_dev, list(range(B)), sp, do_sample=True)
         eng.decode(B, NF - 1, sp, use_graph=True)
         if not args.no_codec:
-            codec_stage()
+            last["wav"] = codec_stage()
 
     def barrier():
         torch.cuda.synchronize()
@@ -642,6 +642,14 @@ def main():
     ms = timed(step_resident, args.steps)
     launches = _lib.launch_count() - launches0
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        np.save(out_dir / "codes.npy", eng.buffer("out_tokens")[:B, :, :NF].float().cpu().numpy())
+        if "wav" in last:
+            np.save(out_dir / "wav.npy", last["wav"].float().flatten()[::4].cpu().numpy())
     ms_per_step = ms / args.steps
     audio_s = B * world * NF * FRAME / SR
     value = audio_s / (ms_per_step / 1e3)
@@ -710,7 +718,7 @@ def main():
                 "codec_tokens_per_s": B * world * NF * cfg.num_codebooks / (ms_per_step / 1e3),
                 "ms_per_frame": frame_ms, "ms_per_decode_frame": decode_ms, "prefill_ms": prefill_ms,
                 "codec_ms": codec["ms"] if codec else None, "sampling": "greedy top_k=1 T=0.7 top_p=0.7",
-                "l2_note": "inputs larger than L2: 9.1 GB of weights streamed per frame (126 MB L2)",
+                "l2_note": "inputs larger than L2: 9.1 GB of weights streamed per frame (50 MB L2)",
                 "parallelism": f"replica x{world}, utts[rank::world]", "weights": weights_from,
                 "step_hbm_frac": frame_bytes / (frame_ms / 1e3) / 1e9 / pk["hbm_gbs"],
             },
@@ -719,8 +727,8 @@ def main():
             "gpu_launches": int(launches),
             "roofline": {
                 "bound": "hbm", "achieved": dec_gbs, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                "frac": dec_gbs / pk["hbm_gbs"], "traffic": ncu_traffic(), "peak_kind": pk_kind,
-                "kernel": "step_gemm_kernel (tcgen05 + TMA weight streaming, host-scheduled stream-K, RMSNorm applied on "
+                "frac": dec_gbs / pk["hbm_gbs"], "traffic": None, "peak_kind": pk_kind,
+                "kernel": "step_gemm_kernel (wgmma + TMA weight streaming, host-scheduled stream-K, RMSNorm applied on "
                           "operand load; partials finished by the consuming kernels), in-frame: bytes of one decode frame "
                           "(weights + KV) / device time of one frame",
                 "bytes_per_launch": dec_bytes / nl.value, "launches_per_frame": nl.value,
@@ -735,7 +743,7 @@ def main():
             pkv = pk.get("bf16_tflops_sustained", 1400.0)
             out["roofline_codec"] = {"bound": "tensor", "achieved": codec["tflops"], "peak": pkv, "unit": "TFLOP/s",
                                      "frac": codec["tflops"] / pkv, "traffic": None, "ms_per_step": codec["ms"],
-                                     "kernel": "gemm_tc_kernel<BN,1> implicit-im2col conv GEMMs (tcgen05) + glue",
+                                     "kernel": "gemm_tc_kernel<BN,1> implicit-im2col conv GEMMs (wgmma) + glue",
                                      "flop_per_step": codec["flop_per_step"]}
     if world > 1:
         dist.barrier()

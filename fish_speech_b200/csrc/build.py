@@ -1,4 +1,4 @@
-"""Build libfishb200.so in-tree with nvcc for sm_100a (no other architecture, no JIT cache)."""
+"""Build libfishb200.so in-tree with nvcc for sm_90a (H100; no other architecture, no JIT cache)."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ HERE = Path(__file__).resolve().parent
 LIB = HERE.parent / "libfishb200.so"
 SOURCES = ["error.cu", "gemm_tc.cu", "lm_gemm.cu", "lm_kernels.cu", "attn_tile.cu", "lm_engine.cu", "codec_kernels.cu", "codec_resunit.cu", "api.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -58,7 +58,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed")
-    cmd = [nvcc, "-shared", "-o", str(LIB), *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", str(LIB), *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     subprocess.check_call(cmd)
     return LIB
 

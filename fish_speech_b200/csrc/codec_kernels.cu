@@ -1,7 +1,7 @@
 // Codec (modified Descript-DAC) kernels that are not GEMM-shaped, plus the op-level C-ABI of the codec.
 //
 // Activations are channels-last bf16 [B][T][C]; every Conv1d / ConvTranspose1d / Linear runs on the
-// tcgen05 multi-tap GEMM (gemm_tc.cu) with the causal left pad supplied by TMA zero fill; this file
+// wgmma multi-tap GEMM (gemm_tc.cu) with the causal left pad supplied by TMA zero fill; this file
 // holds the small memory-bound pieces around it:
 //   codebook_sum   rvq.py:361-363 + dac/nn/quantize.py from_codes (tables = out_proj(codebook), folded at load)
 //   dwconv_ln      rvq.py:176-179 (ConvNeXt: causal depthwise conv k=7, LayerNorm eps 1e-6)
@@ -301,9 +301,9 @@ int fsb_conv_gemm(const void* d_x, int B, int T_in, int C_in, int row_stride, lo
     FSB_CHECK(taps >= 1 && taps <= kMaxTaps, "conv_gemm: taps=%d out of range", taps);
     FSB_CHECK(kpad % 64 == 0, "conv_gemm: kpad must be a multiple of 64");
     FSB_CHECK(d_out0 || d_out1, "conv_gemm: no output");
-    // tile width along the output channels: no padding waste for the 192- and 384-channel blocks (UMMA N = 192)
+    // tile width along the output channels: no padding waste for the 192- and 384-channel blocks (wgmma N = 192)
     const int bn = C_out <= 32 ? 32 : (C_out <= 64 ? 64 : (C_out <= 128 ? 128 : ((C_out % 256 != 0 && C_out % 192 == 0) ? 192 : 256)));
-    const int two = bn <= 128 ? 2 : 1;  // CTAs per SM (shared memory: 3 x 32 KB stages each; TMEM: 2 x 256 columns)
+    const int two = bn <= 128 ? 2 : 1;  // CTAs per SM (shared memory: 3 x 32 KB stages each; registers: BN / 2 accumulators)
     ConvKey key;
     memset(&key, 0, sizeof(key));
     key.x = d_x; key.w = d_w; key.B = B; key.T_in = T_in; key.T_out = T_out; key.C_in = C_in;

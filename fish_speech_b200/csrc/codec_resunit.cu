@@ -6,24 +6,25 @@
 // a = snake_0(x) (channels-last bf16 [B][T][C]).  Outputs: the new raw stream y (in place over x, optional) and
 // snake_next(y) for the consumer, in a different buffer than `a` (neighbouring tiles still read their halo from `a`).
 //
-// Per tile of 128 time steps (one CTA per SM, persistent over the tiles):
+// Per tile of BM time steps (128; 64 for C = 384, whose accumulators take two warpgroups per 64 rows) -- one CTA per
+// SM, persistent over the tiles:
 //   phase 1  acc[128 x C]  = sum over 7 taps, C/64 k-blocks of  A(tap) W7(tap)^T : implicit im2col, the A tile of a
 //            tap is fetched by TMA at a shifted time coordinate, rows before t = 0 are zero-filled by the TMA unit
-//            (the causal left pad, modded_dac.py:546-552); tcgen05.mma, accumulator in TMEM.
+//            (the causal left pad, modded_dac.py:546-552); wgmma, accumulator in registers.
 //   epi 1    h = snake_1(acc + b7) -> bf16, written straight into shared memory in the K-major SWIZZLE_128B layout
 //            the tensor core reads operand A in (fence.proxy.async): the intermediate never leaves the SM.
 //   phase 2  acc[128 x C]  = h W1^T  (operand A from shared memory, W1 tiles through the same TMA ring).
 //   epi 2    y = acc + b1 + x;  y and snake_next(y) are staged in shared memory (swizzled 64-channel blocks; the h buffer
 //            is free again by then) and leave by TMA bulk tensor stores: whole 128-byte lines, issued asynchronously,
-//            overlapping the next tile's first phase.  Per-thread 16-byte global stores of a [time][channel] tile are
-//            partial-sector writes (one 384-byte row per thread): measured 2.4-2.7 TB/s, the bound of the unfused
-//            1x1 conv (profiles/r01_codec_layers.md).  (C = 384: both staging buffers do not fit next to the ring;
-//            that size keeps the register stores.)
+//            overlapping the next tile's first phase.  (C = 384: both staging buffers do not fit next to the ring;
+//            that size stores from registers.)
 // Against two separate GEMM launches this saves the write + read of h and of the 1x1 conv's operand
 // (2 x 2 x N x C bytes of HBM traffic per unit) and one kernel's worth of residual-stream epilogue.
-// Warps 0-15 epilogues (four per TMEM lane quadrant), warp 16 TMA producer, warp 17 TMEM allocator + MMA issuer.
+// Warpgroup g computes rows [64 (g % MH), +64) x channels [NB (g / MH), +NB) of both products (MH = BM / 64) and runs
+// their epilogues;
+// the last warp is the TMA producer, which runs ahead into the next tile while the epilogues run.
 #include "gemm_tc.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 #include <cstring>
 #include <map>
@@ -33,8 +34,6 @@ namespace fsb {
 
 namespace {
 
-constexpr int kRuEpiWarps = 16;  // four per TMEM lane quadrant: the epilogues are latency-bound instruction streams
-constexpr int kRuThreads = (kRuEpiWarps + 2) * 32;
 constexpr int kRuTaps = 7;
 
 struct ResUnitParams {
@@ -51,7 +50,7 @@ struct ResUnitParams {
     __nv_bfloat16* out1;      // snake_next(y)
     const float* alpha_n;
     const float* inv_n;
-    unsigned long long* trace;  // diagnostics: CTA 0, per tile 6 globaltimer stamps of epilogue thread 0 (or null)
+    unsigned long long* trace;  // diagnostics: CTA 0, per tile 6 globaltimer stamps of thread 0 (or null)
 };
 
 __device__ __forceinline__ float ru_snake(float v, float a, float ia) {
@@ -63,27 +62,33 @@ template <int C>
 struct RuShape {
     static constexpr int CP = (C + 63) / 64 * 64;   // K of both convolutions per tap, padded to the 64-wide k-block
     static constexpr int KB = CP / 64;
-    static constexpr int NB = C <= 256 ? C : C / 2; // UMMA N (<= 256): wider outputs take two MMAs per k-step
+    static constexpr int NB = C <= 256 ? C : C / 2; // wgmma N (<= 256): wider outputs are split over warpgroups
     static constexpr int NS = C / NB;
+    static constexpr int BM = NS == 1 ? 128 : 64;   // time steps per tile: the accumulators must fit the registers
+    static constexpr int MH = BM / 64;
+    static constexpr int kWarpgroups = MH * NS;     // 64-row blocks of the tile x channel blocks
+    static constexpr int kABytes = BM * kBlockK * 2;
+    static constexpr int kMmaThreads = kWarpgroups * 128;
+    static constexpr int kThreads = kMmaThreads + 32;  // + the TMA producer warp
     static constexpr int kBBytes = C * kBlockK * 2;
-    static constexpr int kStageBytes = kATileBytes + kBBytes;
-    static constexpr int kHBytes = KB * kATileBytes;
-    static constexpr int kCols1 = 2 * C <= 512 && C <= 192 ? 2 * C : C;
-    static constexpr int kTmemCols = kCols1 <= 32 ? 32 : (kCols1 <= 64 ? 64 : (kCols1 <= 128 ? 128 : (kCols1 <= 256 ? 256 : 512)));
+    static constexpr int kStageBytes = kABytes + kBBytes;
+    static constexpr int kHBytes = KB * kABytes;
     static constexpr bool kStaged = C <= 192;  // outputs staged in shared memory and stored by TMA
-    static constexpr int kY0Bytes = kStaged ? KB * kATileBytes : 0;
-    // Two accumulator regions (tile parity) where TMEM holds them: the tensor core starts the next tile's conv7 while
-    // the epilogues of this tile run, and this tile's conv1 is slotted in after the first kSplit k-blocks of the next
-    // conv7 (by then epilogue 1 has written h).
-    static constexpr bool kPipe = 2 * C <= 512 && kStaged;
+    static constexpr int kY0Bytes = kStaged ? KB * kABytes : 0;
     static constexpr int kQ1 = 7 * KB;           // k-blocks of phase 1
-    static constexpr int kSplit = kPipe ? (kQ1 + 1) / 2 : 0;
-    static constexpr int kAccCols = kPipe ? 2 * C : C;
     static_assert(C % 32 == 0 && NB % 16 == 0 && NB <= 256 && C <= 512, "channel count not supported");
 };
 
+__device__ __forceinline__ void ru_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// byte offset of (row r, channel c) in a [KB][BM rows][128 B] SWIZZLE_128B staging buffer (c even: a bf16 pair)
+template <int BM>
+__device__ __forceinline__ int ru_swz(int r, int c) {
+    return (c >> 6) * (BM * 128) + r * 128 + (((((c & 63) >> 3) ^ (r & 7))) << 4) + (c & 7) * 2;
+}
+
 template <int C>
-__global__ void __launch_bounds__(kRuThreads, 1)
+__global__ void __launch_bounds__(RuShape<C>::kThreads, 1)
 res_unit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW7,
                 const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmY0,
                 const __grid_constant__ CUtensorMap tmY1, const __grid_constant__ ResUnitParams p) {
@@ -92,56 +97,45 @@ res_unit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t tiles = (raw + 1023u) & ~1023u;
     const int stages = p.stages;
-    const uint32_t h_smem = tiles + static_cast<uint32_t>(stages) * S::kStageBytes;  // [KB][128 rows][128 B]
+    const uint32_t h_smem = tiles + static_cast<uint32_t>(stages) * S::kStageBytes;  // [KB][BM rows][128 B]
     const uint32_t y0_smem = h_smem + S::kHBytes;  // staging of the raw output (kStaged)
     const uint32_t bars = y0_smem + S::kY0Bytes;
     const uint32_t full0 = bars, empty0 = bars + 8u * stages;
-    const uint32_t acc_full0 = empty0 + 8u * stages, acc_empty0 = acc_full0 + 16u, h_full = acc_empty0 + 16u;
-    const uint32_t tmem_slot = h_full + 8u;
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - raw));
     uint8_t* h_ptr = smem_raw + (h_smem - raw);
     uint8_t* y0_ptr = smem_raw + (y0_smem - raw);
+    constexpr int kProducerWarp = S::kMmaThreads / 32;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int item_begin = static_cast<int>(static_cast<long long>(p.total) * blockIdx.x / gridDim.x);
     const int item_end = static_cast<int>(static_cast<long long>(p.total) * (blockIdx.x + 1) / gridDim.x);
 
-    if (warp == kRuEpiWarps && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmW7);
         tma_prefetch_desc(&tmW1);
         for (int s = 0; s < stages; ++s) {
             mbar_init(full0 + 8u * s, 1);
-            mbar_init(empty0 + 8u * s, 1);
+            mbar_init(empty0 + 8u * s, kProducerWarp);  // one arrival per MMA warp
         }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(acc_full0 + 8u * a, 1);
-            mbar_init(acc_empty0 + 8u * a, kRuEpiWarps);
-        }
-        mbar_init(h_full, kRuEpiWarps);
         fence_mbar_init();
     }
-    if (warp == kRuEpiWarps + 1) tmem_alloc(tmem_slot, S::kTmemCols);
     if (S::CP != C) {
         // channels C..CP-1 of h are K padding: zero once (W1's padding columns are zero as well, but 0 x NaN is NaN)
-        for (int i = threadIdx.x; i < S::kHBytes / 16; i += kRuThreads) reinterpret_cast<uint4*>(h_ptr)[i] = make_uint4(0, 0, 0, 0);
+        for (int i = threadIdx.x; i < S::kHBytes / 16; i += S::kThreads) reinterpret_cast<uint4*>(h_ptr)[i] = make_uint4(0, 0, 0, 0);
         fence_proxy_async();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
     pdl_launch_dependents();
-    if (warp == kRuEpiWarps) {
-        // ===== TMA producer: feeds the ring in exactly the order the MMA issuer consumes it =====
+    if (warp == kProducerWarp) {
+        // ===== TMA producer: feeds the ring in exactly the order the MMA warpgroups consume it =====
         if (lane == 0) {
             pdl_wait();
             int it = 0;
-            auto load_p1 = [&](int n, int q0, int q1) {  // conv7 k-blocks [q0, q1) of tile n: activations of the tap + its weights
+            for (int n = item_begin; n < item_end; ++n) {
                 const int z = n / p.tiles_t;
-                const int t0 = (n - z * p.tiles_t) * kBlockM;
-                for (int q = q0; q < q1; ++q, ++it) {
+                const int t0 = (n - z * p.tiles_t) * S::BM;
+                for (int q = 0; q < S::kQ1; ++q, ++it) {  // conv7: activations of the tap + its weights
                     const int s = it % stages;
                     const uint32_t dst = tiles + static_cast<uint32_t>(s) * S::kStageBytes;
                     mbar_wait(empty0 + 8u * s, (static_cast<uint32_t>(it / stages) & 1u) ^ 1u);
@@ -150,222 +144,126 @@ res_unit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     tma_load_3d(dst, &tmA, full0 + 8u * s, kb * kBlockK, t0 + p.shift[tap], z, kEvictNormal);
 #pragma unroll
                     for (int hh = 0; hh < S::NS; ++hh)
-                        tma_load_3d(dst + kATileBytes + hh * S::NB * 128, &tmW7, full0 + 8u * s,
+                        tma_load_3d(dst + S::kABytes + hh * S::NB * 128, &tmW7, full0 + 8u * s,
                                     tap * S::CP + kb * kBlockK, hh * S::NB, 0, kEvictLast);
                 }
-            };
-            auto load_p2 = [&]() {  // conv1: its weights only (operand A is h in shared memory)
-                for (int kb = 0; kb < S::KB; ++kb, ++it) {
+                for (int kb = 0; kb < S::KB; ++kb, ++it) {  // conv1: its weights only (operand A is h in shared memory)
                     const int s = it % stages;
                     const uint32_t dst = tiles + static_cast<uint32_t>(s) * S::kStageBytes;
                     mbar_wait(empty0 + 8u * s, (static_cast<uint32_t>(it / stages) & 1u) ^ 1u);
                     mbar_expect_tx(full0 + 8u * s, S::kBBytes);
 #pragma unroll
                     for (int hh = 0; hh < S::NS; ++hh)
-                        tma_load_3d(dst + kATileBytes + hh * S::NB * 128, &tmW1, full0 + 8u * s, kb * kBlockK,
+                        tma_load_3d(dst + S::kABytes + hh * S::NB * 128, &tmW1, full0 + 8u * s, kb * kBlockK,
                                     hh * S::NB, 0, kEvictLast);
                 }
-            };
-            if (item_begin < item_end) load_p1(item_begin, 0, S::kQ1);
-            for (int n = item_begin; n < item_end; ++n) {
-                const bool more = n + 1 < item_end;
-                if (more && S::kSplit > 0) load_p1(n + 1, 0, S::kSplit);
-                load_p2();
-                if (more) load_p1(n + 1, S::kSplit, S::kQ1);
-            }
-        }
-    } else if (warp == kRuEpiWarps + 1) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc(S::NB);
-            int it = 0;
-            auto region = [&](int n) { return S::kPipe ? ((n - item_begin) & 1) : 0; };
-            auto use = [&](int n) { return S::kPipe ? ((n - item_begin) >> 1) : (n - item_begin); };  // uses of the region so far
-            auto block = [&](uint32_t d_tmem, uint64_t ad, uint32_t bsrc, uint32_t& acc) {
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k) {
-#pragma unroll
-                    for (int hh = 0; hh < S::NS; ++hh)
-                        umma_bf16(d_tmem + hh * S::NB, ad + 2u * k, make_sdesc(bsrc + hh * S::NB * 128) + 2u * k, idesc, acc);
-                    acc = 1;
-                }
-            };
-            auto mma_p1 = [&](int n, int q0, int q1) {
-                const int r = region(n);
-                const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(r * C);
-                if (q0 == 0) {  // the epilogues of the tile that used this region before have drained it
-                    mbar_wait(acc_empty0 + 8u * r, (static_cast<uint32_t>(use(n)) & 1u) ^ 1u);
-                    tc_fence_after();
-                }
-                uint32_t acc = q0 == 0 ? 0u : 1u;
-                for (int q = q0; q < q1; ++q, ++it) {
-                    const int s = it % stages;
-                    mbar_wait(full0 + 8u * s, static_cast<uint32_t>(it / stages) & 1u);
-                    tc_fence_after();
-                    const uint32_t src = tiles + static_cast<uint32_t>(s) * S::kStageBytes;
-                    block(d_tmem, make_sdesc(src), src + kATileBytes, acc);
-                    umma_commit(empty0 + 8u * s);
-                }
-                if (q1 == S::kQ1) umma_commit(acc_full0 + 8u * r);  // conv7 accumulator complete -> epilogue 1
-            };
-            auto mma_p2 = [&](int n) {
-                const int r = region(n);
-                const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(r * C);
-                mbar_wait(h_full, static_cast<uint32_t>(n - item_begin) & 1u);  // h written, conv7 accumulator read out
-                tc_fence_after();
-                uint32_t acc = 0;
-                for (int kb = 0; kb < S::KB; ++kb, ++it) {
-                    const int s = it % stages;
-                    mbar_wait(full0 + 8u * s, static_cast<uint32_t>(it / stages) & 1u);
-                    tc_fence_after();
-                    const uint32_t src = tiles + static_cast<uint32_t>(s) * S::kStageBytes;
-                    block(d_tmem, make_sdesc(h_smem + static_cast<uint32_t>(kb) * kATileBytes), src + kATileBytes, acc);
-                    umma_commit(empty0 + 8u * s);
-                }
-                umma_commit(acc_full0 + 8u * r);  // conv1 accumulator complete -> epilogue 2
-            };
-            if (item_begin < item_end) mma_p1(item_begin, 0, S::kQ1);
-            for (int n = item_begin; n < item_end; ++n) {
-                const bool more = n + 1 < item_end;
-                if (more && S::kSplit > 0) mma_p1(n + 1, 0, S::kSplit);
-                mma_p2(n);
-                if (more) mma_p1(n + 1, S::kSplit, S::kQ1);
             }
         }
     } else {
-        // ===== epilogues: the two warps of a TMEM lane quadrant take alternate 32-column chunks =====
-        const int quad = warp & 3, half = warp >> 2;  // `half`: which of the kCW warps of the lane quadrant
-        constexpr int kCW = kRuEpiWarps / 4;
-        constexpr int kCStride = 32 * kCW;
-        constexpr int NK = (C / 32 + kCW - 1) / kCW;  // 32-column chunks per warp (chunk k of warp h: columns h*32 + k*kCStride)
-        const int r = quad * 32 + lane;  // row of the tile = TMEM lane
+        // ===== MMA warpgroups =====
+        const int wg = warp >> 2, wq = warp & 3;
+        const int mh = wg % S::MH, cbase = (wg / S::MH) * S::NB;  // 64-row block of the tile, first channel
+        const int r0 = mh * 64 + wq * 16 + (lane >> 2);     // tile rows r0 and r0 + 8 of this thread
+        int it = 0;
+        // k-blocks [0, nkb) of one product into d; operand A at a_of(q) (+ this warpgroup's 64-row half)
+        auto run = [&](float* d, int nkb, auto a_of) {
+#pragma unroll 1
+            for (int q = 0; q < nkb; ++q, ++it) {
+                const int s = it % stages;
+                mbar_wait(full0 + 8u * s, static_cast<uint32_t>(it / stages) & 1u);
+                const uint32_t src = tiles + static_cast<uint32_t>(s) * S::kStageBytes;
+                const uint64_t ad = make_gdesc(a_of(q, src) + mh * kHalfATileBytes);
+                const uint64_t bd = make_gdesc(src + S::kABytes + cbase * 128);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBlockK / 16; ++k) wgmma_bf16<S::NB>(d, ad + 2u * k, bd + 2u * k, 1);
+                wgmma_commit();
+                wgmma_wait<1>();  // the previous k-block's MMAs have retired: release its ring slot
+                if (q > 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
+                }
+            }
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
+        };
         for (int n = item_begin; n < item_end; ++n) {
-            const int reg = S::kPipe ? ((n - item_begin) & 1) : 0;
-            const uint32_t acc_full = acc_full0 + 8u * reg, acc_empty = acc_empty0 + 8u * reg;
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + static_cast<uint32_t>(reg * C);
             const int z = n / p.tiles_t;
-            const int t = (n - z * p.tiles_t) * kBlockM + r;
-            const bool live = t < p.T;
-            const size_t rowoff = (static_cast<size_t>(z) * p.T + t) * C;
-            // ---- epilogue 1: h = snake_1(conv7 + b7) into the swizzled operand tile ----
+            const int t0 = (n - z * p.tiles_t) * S::BM;
             unsigned long long* tr = (p.trace && blockIdx.x == 0 && threadIdx.x == 0 && n - item_begin < 64)
                                          ? p.trace + (n - item_begin) * 6 : nullptr;
             if (tr) tr[0] = globaltimer_ns();
-            mbar_wait(acc_full, 0u);
-            tc_fence_after();
+            float d[S::NB / 2];
+            // ---- phase 1: conv7 ----
+#pragma unroll
+            for (int e = 0; e < S::NB / 2; ++e) d[e] = 0.f;
+            run(d, S::kQ1, [](int, uint32_t src) { return src; });
             if (tr) tr[1] = globaltimer_ns();
-            if (S::kStaged && n > item_begin) {
-                // the previous tile's bulk stores read the h / y0 buffers: they must have finished reading
-                if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                asm volatile("bar.sync 1, %0;" ::"n"(kRuEpiWarps * 32) : "memory");
-            }
-#pragma unroll 1
-            for (int k = 0; k < NK; ++k) {
-                const int c0 = half * 32 + k * kCStride;  // warp-uniform
-                if (c0 >= C) break;
-                uint32_t v[32];
-                tmem_ld32(taddr + c0, v);
-                tmem_ld_wait();
-                uint8_t* hrow = h_ptr + (c0 >> 6) * kATileBytes + r * 128;
+            // the previous tile's bulk stores read the h / y0 buffers: they must have finished reading
+            if (S::kStaged && n > item_begin && threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+            ru_bar(1, S::kMmaThreads);
+            // ---- epilogue 1: h = snake_1(conv7 + b7) into the swizzled operand tile ----
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int c = c0 + q * 8;
-                    float f[8];
+            for (int b = 0; b < S::NB / 8; ++b) {
+                const int c = cbase + 8 * b + 2 * (lane & 3);
+                const float2 bb = __ldg(reinterpret_cast<const float2*>(p.b7 + c));
+                const float2 al = __ldg(reinterpret_cast<const float2*>(p.alpha1 + c));
+                const float2 ia = __ldg(reinterpret_cast<const float2*>(p.inv1 + c));
 #pragma unroll
-                    for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[q * 8 + e]);
-                    const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.b7 + c));
-                    const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.b7 + c + 4));
-                    const float4 a0 = __ldg(reinterpret_cast<const float4*>(p.alpha1 + c));
-                    const float4 a1 = __ldg(reinterpret_cast<const float4*>(p.alpha1 + c + 4));
-                    const float4 i0 = __ldg(reinterpret_cast<const float4*>(p.inv1 + c));
-                    const float4 i1 = __ldg(reinterpret_cast<const float4*>(p.inv1 + c + 4));
-                    uint4 u;
+                for (int h = 0; h < 2; ++h) {
+                    const int r = r0 + 8 * h;
                     // the unfused path stores conv7's output as bf16 only after the Snake: same rounding point here
-                    u.x = pack_bf2(ru_snake(f[0] + b0.x, a0.x, i0.x), ru_snake(f[1] + b0.y, a0.y, i0.y));
-                    u.y = pack_bf2(ru_snake(f[2] + b0.z, a0.z, i0.z), ru_snake(f[3] + b0.w, a0.w, i0.w));
-                    u.z = pack_bf2(ru_snake(f[4] + b1.x, a1.x, i1.x), ru_snake(f[5] + b1.y, a1.y, i1.y));
-                    u.w = pack_bf2(ru_snake(f[6] + b1.z, a1.z, i1.z), ru_snake(f[7] + b1.w, a1.w, i1.w));
-                    const int cell = ((c & 63) >> 3) ^ (r & 7);  // SWIZZLE_128B: 16-byte cell index XOR row mod 8
-                    *reinterpret_cast<uint4*>(hrow + (cell << 4)) = u;
+                    *reinterpret_cast<uint32_t*>(h_ptr + ru_swz<S::BM>(r, c)) =
+                        pack_bf2(ru_snake(d[4 * b + 2 * h] + bb.x, al.x, ia.x), ru_snake(d[4 * b + 2 * h + 1] + bb.y, al.y, ia.y));
                 }
             }
             fence_proxy_async();  // generic-proxy writes of h -> visible to the tensor core's async proxy
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(h_full);
+            ru_bar(1, S::kMmaThreads);
             if (tr) tr[2] = globaltimer_ns();
-            // ---- epilogue 2: y = conv1 + b1 + x; store y and snake_next(y) ----
-            uint4 rr[NK * 4];  // the residual of this warp's chunks, requested before the accumulator is ready
+            // ---- phase 2: conv1 over h ----
 #pragma unroll
-            for (int k = 0; k < NK; ++k) {
-                const int c0 = half * 32 + k * kCStride;
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                    rr[k * 4 + q] = (live && c0 < C) ? *reinterpret_cast<const uint4*>(p.x + rowoff + c0 + q * 8)
-                                                     : make_uint4(0, 0, 0, 0);
-            }
-            mbar_wait(acc_full, 1u);
-            tc_fence_after();
+            for (int e = 0; e < S::NB / 2; ++e) d[e] = 0.f;
+            run(d, S::KB, [&](int q, uint32_t) { return h_smem + static_cast<uint32_t>(q) * S::kABytes; });
+            ru_bar(1, S::kMmaThreads);  // every warpgroup is done reading h before it takes snake_next(y)
             if (tr) tr[3] = globaltimer_ns();
-            {
+            // ---- epilogue 2: y = conv1 + b1 + x; store y and snake_next(y) ----
 #pragma unroll
-                for (int k = 0; k < NK; ++k) {
-                    const int c0 = half * 32 + k * kCStride;  // warp-uniform
-                    if (c0 >= C) break;
-                    uint32_t v[32];
-                    tmem_ld32(taddr + c0, v);
-                    tmem_ld_wait();
-                    if (!S::kStaged && !live) continue;
+            for (int b = 0; b < S::NB / 8; ++b) {
+                const int c = cbase + 8 * b + 2 * (lane & 3);
+                const float2 bb = __ldg(reinterpret_cast<const float2*>(p.b1 + c));
+                const float2 al = __ldg(reinterpret_cast<const float2*>(p.alpha_n + c));
+                const float2 ia = __ldg(reinterpret_cast<const float2*>(p.inv_n + c));
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const int c = c0 + q * 8;
-                        float f[8];
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[q * 8 + e]);
-                        const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.b1 + c));
-                        const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.b1 + c + 4));
-                        const uint4 xr = rr[k * 4 + q];
-                        // (acc + bias) + x, the association of the two-launch path: identical bits
-                        f[0] = (f[0] + b0.x) + bf_lo(xr.x); f[1] = (f[1] + b0.y) + bf_hi(xr.x);
-                        f[2] = (f[2] + b0.z) + bf_lo(xr.y); f[3] = (f[3] + b0.w) + bf_hi(xr.y);
-                        f[4] = (f[4] + b1.x) + bf_lo(xr.z); f[5] = (f[5] + b1.y) + bf_hi(xr.z);
-                        f[6] = (f[6] + b1.z) + bf_lo(xr.w); f[7] = (f[7] + b1.w) + bf_hi(xr.w);
-                        const int cell = ((c & 63) >> 3) ^ (r & 7);
-                        const int toff = (c >> 6) * kATileBytes + r * 128 + (cell << 4);
-                        if (p.out0) {
-                            uint4 u;
-                            u.x = pack_bf2(f[0], f[1]); u.y = pack_bf2(f[2], f[3]);
-                            u.z = pack_bf2(f[4], f[5]); u.w = pack_bf2(f[6], f[7]);
-                            if (S::kStaged) *reinterpret_cast<uint4*>(y0_ptr + toff) = u;
-                            else if (live) *reinterpret_cast<uint4*>(p.out0 + rowoff + c) = u;
-                        }
-                        const float4 a0 = __ldg(reinterpret_cast<const float4*>(p.alpha_n + c));
-                        const float4 a1 = __ldg(reinterpret_cast<const float4*>(p.alpha_n + c + 4));
-                        const float4 i0 = __ldg(reinterpret_cast<const float4*>(p.inv_n + c));
-                        const float4 i1 = __ldg(reinterpret_cast<const float4*>(p.inv_n + c + 4));
-                        uint4 u;
-                        u.x = pack_bf2(ru_snake(f[0], a0.x, i0.x), ru_snake(f[1], a0.y, i0.y));
-                        u.y = pack_bf2(ru_snake(f[2], a0.z, i0.z), ru_snake(f[3], a0.w, i0.w));
-                        u.z = pack_bf2(ru_snake(f[4], a1.x, i1.x), ru_snake(f[5], a1.y, i1.y));
-                        u.w = pack_bf2(ru_snake(f[6], a1.z, i1.z), ru_snake(f[7], a1.w, i1.w));
-                        if (S::kStaged) *reinterpret_cast<uint4*>(h_ptr + toff) = u;  // h has been consumed by phase 2
-                        else if (live) *reinterpret_cast<uint4*>(p.out1 + rowoff + c) = u;
+                for (int h = 0; h < 2; ++h) {
+                    const int r = r0 + 8 * h;
+                    const int t = t0 + r;
+                    const bool live = t < p.T;
+                    const size_t off = (static_cast<size_t>(z) * p.T + t) * C + c;
+                    const uint32_t xr = live ? *reinterpret_cast<const uint32_t*>(p.x + off) : 0u;
+                    // (acc + bias) + x, the association of the two-launch path: identical bits
+                    const float f0 = (d[4 * b + 2 * h] + bb.x) + bf_lo(xr);
+                    const float f1 = (d[4 * b + 2 * h + 1] + bb.y) + bf_hi(xr);
+                    const uint32_t y = pack_bf2(f0, f1);
+                    const uint32_t ys = pack_bf2(ru_snake(f0, al.x, ia.x), ru_snake(f1, al.y, ia.y));
+                    if (S::kStaged) {
+                        if (p.out0) *reinterpret_cast<uint32_t*>(y0_ptr + ru_swz<S::BM>(r, c)) = y;
+                        *reinterpret_cast<uint32_t*>(h_ptr + ru_swz<S::BM>(r, c)) = ys;  // h has been consumed by phase 2
+                    } else if (live) {
+                        if (p.out0) *reinterpret_cast<uint32_t*>(p.out0 + off) = y;
+                        *reinterpret_cast<uint32_t*>(p.out1 + off) = ys;
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc_empty);
             if (tr) tr[4] = globaltimer_ns();
             if (S::kStaged) {
                 fence_proxy_async();  // the staged tiles -> visible to the TMA engine
-                asm volatile("bar.sync 2, %0;" ::"n"(kRuEpiWarps * 32) : "memory");
+                ru_bar(1, S::kMmaThreads);
                 if (threadIdx.x == 0) {
-                    const int t0 = (n - z * p.tiles_t) * kBlockM;
 #pragma unroll
                     for (int kb = 0; kb < S::KB; ++kb) {
-                        if (p.out0) tma_store_3d(&tmY0, y0_smem + kb * kATileBytes, kb * kBlockK, t0, z);
-                        tma_store_3d(&tmY1, h_smem + kb * kATileBytes, kb * kBlockK, t0, z);
+                        if (p.out0) tma_store_3d(&tmY0, y0_smem + kb * S::kABytes, kb * kBlockK, t0, z);
+                        tma_store_3d(&tmY1, h_smem + kb * S::kABytes, kb * kBlockK, t0, z);
                     }
                     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
                 }
@@ -373,12 +271,6 @@ res_unit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             if (tr) tr[5] = globaltimer_ns();
         }
         if (S::kStaged && threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kRuEpiWarps + 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, S::kTmemCols);
     }
 }
 
@@ -413,7 +305,7 @@ int ru_setup() {
 template <int C>
 int ru_launch(const RuPlan& plan, const ResUnitParams& p, cudaStream_t st) {
     FSB_TRY(ru_setup<C>());
-    FSB_LAUNCH(res_unit_kernel<C>, plan.grid, dim3(kRuThreads), plan.smem, st, plan.tmA, plan.tmW7, plan.tmW1, plan.tmY0,
+    FSB_LAUNCH(res_unit_kernel<C>, plan.grid, dim3(RuShape<C>::kThreads), plan.smem, st, plan.tmA, plan.tmW7, plan.tmW1, plan.tmY0,
                plan.tmY1, p);
     return 0;
 }
@@ -425,25 +317,25 @@ int ru_plan(RuPlan* plan, const void* a, const void* w7, const void* w1, const v
     GemmOperand W7{reinterpret_cast<const __nv_bfloat16*>(w7), static_cast<long long>(kRuTaps) * S::CP, C, 1,
                    static_cast<long long>(kRuTaps) * S::CP, static_cast<long long>(C) * kRuTaps * S::CP};
     GemmOperand W1{reinterpret_cast<const __nv_bfloat16*>(w1), S::CP, C, 1, S::CP, static_cast<long long>(C) * S::CP};
-    FSB_TRY(gemm_make_tmap(&plan->tmA, A, kBlockM));
+    FSB_TRY(gemm_make_tmap(&plan->tmA, A, S::BM));
     FSB_TRY(gemm_make_tmap(&plan->tmW7, W7, S::NB));
     FSB_TRY(gemm_make_tmap(&plan->tmW1, W1, S::NB));
-    // outputs: the same {64 channels, 128 time steps} boxes, written by TMA from the staging tiles
+    // outputs: the same {64 channels, BM time steps} boxes, written by TMA from the staging tiles
     GemmOperand Y1 = A, Y0 = A;
     Y1.ptr = reinterpret_cast<const __nv_bfloat16*>(out1);
     Y0.ptr = reinterpret_cast<const __nv_bfloat16*>(out0 ? out0 : out1);
-    FSB_TRY(gemm_make_tmap(&plan->tmY1, Y1, kBlockM));
-    FSB_TRY(gemm_make_tmap(&plan->tmY0, Y0, kBlockM));
+    FSB_TRY(gemm_make_tmap(&plan->tmY1, Y1, S::BM));
+    FSB_TRY(gemm_make_tmap(&plan->tmY0, Y0, S::BM));
     const int budget = 227 * 1024 - 1024 - 256 - S::kHBytes - S::kY0Bytes;
     int stages = budget / S::kStageBytes;
     if (stages > 6) stages = 6;
     FSB_CHECK(stages >= 2, "res_unit: not enough shared memory for C=%d", C);
     plan->stages = stages;
     plan->smem = static_cast<size_t>(stages) * S::kStageBytes + S::kHBytes + S::kY0Bytes + 1024 + 16 * stages + 64;
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const long long total = static_cast<long long>(B) * cdiv(T, kBlockM);
+    int dev = 0, sms = 0;
+    FSB_CUDA(cudaGetDevice(&dev));
+    FSB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const long long total = static_cast<long long>(B) * cdiv(T, S::BM);
     plan->grid = dim3(static_cast<unsigned>(total < sms ? total : sms), 1, 1);
     return 0;
 }
@@ -484,7 +376,7 @@ int res_unit_run(const void* d_a, const void* d_x, int B, int T, int C, int dila
     ResUnitParams p;
     memset(&p, 0, sizeof(p));
     p.T = T; p.B = B;
-    p.tiles_t = cdiv(T, kBlockM);
+    p.tiles_t = cdiv(T, C == 384 ? RuShape<384>::BM : kBlockM);
     p.total = B * p.tiles_t;
     p.stages = plan.stages;
     for (int q = 0; q < kRuTaps; ++q) p.shift[q] = -(kRuTaps - 1 - q) * dilation;

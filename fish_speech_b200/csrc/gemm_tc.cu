@@ -1,12 +1,12 @@
-// tcgen05 / TMEM / TMA multi-tap GEMM — see gemm_tc.cuh for the contract.
+// wgmma / TMA multi-tap GEMM — see gemm_tc.cuh for the contract.
 //
-// CTA = 192 threads: warps 0-3 epilogue (TMEM lane quadrant = warp id), warp 4 TMA producer,
-// warp 5 TMEM allocator + single-thread MMA issuer.  smem ring of `stages` x {A 128x64 bf16 (16 KB),
-// B BNx64 bf16}, both written by TMA with SWIZZLE_128B and consumed through UMMA shared-memory
-// descriptors (K-major, SBO = 1024 B).  A CTA runs one output tile, or a stream-K range of segments
-// with two TMEM accumulators so the epilogue of segment n overlaps the MMAs of segment n+1.
+// CTA = 288 threads: warpgroups 0-1 (warps 0-7) issue wgmma for rows [0, 64) / [64, 128) of the 128-row tile and run
+// the epilogue from their registers, warp 8 is the TMA producer.  smem ring of `stages` x {A 128x64 bf16 (16 KB),
+// B BNx64 bf16}, both written by TMA with SWIZZLE_128B and read through wgmma shared-memory descriptors.  A CTA runs
+// one output tile, or a stream-K range of segments / a range of the persistent tiled schedule; the TMA ring keeps
+// flowing across item boundaries, so the next item's tiles land while this item's epilogue runs.
 #include "gemm_tc.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 #include <vector>
 
@@ -21,11 +21,13 @@ __device__ __forceinline__ float gelu_erf(float x) {
     return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f));
 }
 
-// Direct epilogue for one 32-column chunk of an accumulator row:
+// Direct epilogue for 8 consecutive columns of an accumulator row:
 //   bias -> GELU -> gamma -> +residual -> tanh -> store raw (out0) and/or Snake-activated (out1).
 // Fast path (channels on the columns, bf16 outputs contiguous along the columns, full chunk): per-column
-// parameters come in as float4 broadcast loads, 8 columns are processed at a time to keep the register
-// footprint small, sin() is the MUFU approximation (arguments are O(10), outputs are bf16).
+// parameters come in as float4 broadcast loads and leave as one 16-byte store; sin() is the MUFU approximation
+// (arguments are O(10), outputs are bf16).
+constexpr int kEpiCols = 8;
+
 __device__ __forceinline__ float snake_fast(float v, float a, float ia) {
     const float s = __sinf(a * v);
     return fmaf(ia * s, s, v);
@@ -33,86 +35,72 @@ __device__ __forceinline__ float snake_fast(float v, float a, float ia) {
 
 __device__ __forceinline__ bool epilogue_fast(const GemmParams& p, int jbase) {
     return !p.chan_on_i && (p.o_js == 1) && !p.out_f32 && ((p.o_is & 7) == 0) && ((p.o_zs & 7) == 0) &&
-           (jbase + 32 <= p.rows_j);
+           (jbase + kEpiCols <= p.rows_j);
 }
 
-// The residual of a chunk (4 x 16 bytes per thread) is requested BEFORE the accumulator is read from TMEM and
-// before any store of the chunk: the stores may alias the residual buffer (in-place residual stream), so the
-// compiler cannot hoist these loads itself, and one 16-byte load in flight per thread left the 1x1 convs of
-// the wide-time blocks latency-bound at ~2 TB/s.
-__device__ __forceinline__ void epilogue_preload(const GemmParams& p, int i, int jbase, int z, uint4 (&rr)[4]) {
-    if (p.resid == nullptr || !epilogue_fast(p, jbase)) return;
-    const size_t rowoff = static_cast<size_t>(z) * p.o_zs + static_cast<size_t>(i) * p.o_is;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) rr[q] = *reinterpret_cast<const uint4*>(p.resid + rowoff + jbase + q * 8);
-}
-
-template <int BN>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32_t* r, const uint4 (&rr)[4], int i,
-                                               int jbase, int z) {
+__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const float (&v0)[kEpiCols], int i, int jbase,
+                                               int z) {
     const size_t zoff = static_cast<size_t>(z) * p.o_zs;
     const size_t rowoff = zoff + static_cast<size_t>(i) * p.o_is;
-    const bool fast = epilogue_fast(p, jbase);
-    if (fast) {
+    if (epilogue_fast(p, jbase)) {
+        const int j = jbase;
+        float v[8];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const int j = jbase + q * 8;
-            float v[8];
+        for (int e = 0; e < 8; ++e) v[e] = v0[e];
+        // the residual may alias the outputs (in-place residual stream): load it before any store of the chunk
+        uint4 rr = make_uint4(0, 0, 0, 0);
+        if (p.resid) rr = *reinterpret_cast<const uint4*>(p.resid + rowoff + j);
+        if (p.bias) {
+            const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + j));
+            const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + j + 4));
+            v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
+            v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
+        }
+        if (p.act == ACT_GELU) {
 #pragma unroll
-            for (int e = 0; e < 8; ++e) v[e] = __uint_as_float(r[q * 8 + e]);
-            if (p.bias) {
-                const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + j));
-                const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + j + 4));
-                v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
-                v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
-            }
-            if (p.act == ACT_GELU) {
+            for (int e = 0; e < 8; ++e) v[e] = gelu_erf(v[e]);
+        }
+        if (p.gamma) {
+            const float4 g0 = __ldg(reinterpret_cast<const float4*>(p.gamma + j));
+            const float4 g1 = __ldg(reinterpret_cast<const float4*>(p.gamma + j + 4));
+            v[0] *= g0.x; v[1] *= g0.y; v[2] *= g0.z; v[3] *= g0.w;
+            v[4] *= g1.x; v[5] *= g1.y; v[6] *= g1.z; v[7] *= g1.w;
+        }
+        if (p.resid) {
+            v[0] += bf_lo(rr.x); v[1] += bf_hi(rr.x); v[2] += bf_lo(rr.y); v[3] += bf_hi(rr.y);
+            v[4] += bf_lo(rr.z); v[5] += bf_hi(rr.z); v[6] += bf_lo(rr.w); v[7] += bf_hi(rr.w);
+        }
+        if (p.act == ACT_TANH) {
 #pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] = gelu_erf(v[e]);
-            }
-            if (p.gamma) {
-                const float4 g0 = __ldg(reinterpret_cast<const float4*>(p.gamma + j));
-                const float4 g1 = __ldg(reinterpret_cast<const float4*>(p.gamma + j + 4));
-                v[0] *= g0.x; v[1] *= g0.y; v[2] *= g0.z; v[3] *= g0.w;
-                v[4] *= g1.x; v[5] *= g1.y; v[6] *= g1.z; v[7] *= g1.w;
-            }
-            if (p.resid) {
-                const uint4 u = rr[q];
-                v[0] += bf_lo(u.x); v[1] += bf_hi(u.x); v[2] += bf_lo(u.y); v[3] += bf_hi(u.y);
-                v[4] += bf_lo(u.z); v[5] += bf_hi(u.z); v[6] += bf_lo(u.w); v[7] += bf_hi(u.w);
-            }
-            if (p.act == ACT_TANH) {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] = tanhf(v[e]);
-            }
-            if (p.out0) {
-                uint4 u;
-                u.x = pack_bf2(v[0], v[1]); u.y = pack_bf2(v[2], v[3]);
-                u.z = pack_bf2(v[4], v[5]); u.w = pack_bf2(v[6], v[7]);
-                *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out0) + rowoff + j) = u;
-            }
-            if (p.out1) {
-                const float4 a0 = __ldg(reinterpret_cast<const float4*>(p.snake_alpha + j));
-                const float4 a1 = __ldg(reinterpret_cast<const float4*>(p.snake_alpha + j + 4));
-                const float4 i0 = __ldg(reinterpret_cast<const float4*>(p.snake_inv_alpha + j));
-                const float4 i1 = __ldg(reinterpret_cast<const float4*>(p.snake_inv_alpha + j + 4));
-                uint4 u;
-                u.x = pack_bf2(snake_fast(v[0], a0.x, i0.x), snake_fast(v[1], a0.y, i0.y));
-                u.y = pack_bf2(snake_fast(v[2], a0.z, i0.z), snake_fast(v[3], a0.w, i0.w));
-                u.z = pack_bf2(snake_fast(v[4], a1.x, i1.x), snake_fast(v[5], a1.y, i1.y));
-                u.w = pack_bf2(snake_fast(v[6], a1.z, i1.z), snake_fast(v[7], a1.w, i1.w));
-                *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out1) + rowoff + j) = u;
-            }
+            for (int e = 0; e < 8; ++e) v[e] = tanhf(v[e]);
+        }
+        if (p.out0) {
+            uint4 u;
+            u.x = pack_bf2(v[0], v[1]); u.y = pack_bf2(v[2], v[3]);
+            u.z = pack_bf2(v[4], v[5]); u.w = pack_bf2(v[6], v[7]);
+            *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out0) + rowoff + j) = u;
+        }
+        if (p.out1) {
+            const float4 a0 = __ldg(reinterpret_cast<const float4*>(p.snake_alpha + j));
+            const float4 a1 = __ldg(reinterpret_cast<const float4*>(p.snake_alpha + j + 4));
+            const float4 i0 = __ldg(reinterpret_cast<const float4*>(p.snake_inv_alpha + j));
+            const float4 i1 = __ldg(reinterpret_cast<const float4*>(p.snake_inv_alpha + j + 4));
+            uint4 u;
+            u.x = pack_bf2(snake_fast(v[0], a0.x, i0.x), snake_fast(v[1], a0.y, i0.y));
+            u.y = pack_bf2(snake_fast(v[2], a0.z, i0.z), snake_fast(v[3], a0.w, i0.w));
+            u.z = pack_bf2(snake_fast(v[4], a1.x, i1.x), snake_fast(v[5], a1.y, i1.y));
+            u.w = pack_bf2(snake_fast(v[6], a1.z, i1.z), snake_fast(v[7], a1.w, i1.w));
+            *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out1) + rowoff + j) = u;
         }
         return;
     }
-    // generic path (ragged chunks, fp32 outputs, channels on the lanes)
+    // generic path (ragged chunks, fp32 outputs, channels on the rows)
 #pragma unroll
-    for (int jj = 0; jj < 32; ++jj) {
+    for (int jj = 0; jj < kEpiCols; ++jj) {
         const int j = jbase + jj;
         if (j >= p.rows_j) continue;
         const int c = p.chan_on_i ? i : j;
-        float x = __uint_as_float(r[jj]);
+        float x = v0[jj];
         if (p.bias) x += p.bias[c];
         if (p.act == ACT_GELU) x = gelu_erf(x);
         if (p.gamma) x *= p.gamma[c];
@@ -131,38 +119,37 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32
     }
 }
 
-// MODE 0: fp32 partial sums to the workspace (decode / prefill of the LM). Lean in registers and shared
-//         memory so that TWO CTAs fit on an SM: the CTA of the next GEMM in the stream becomes resident
-//         (programmatic dependent launch) and prefetches its weight tiles while this one still runs.
+// Per-warp staging of 16 accumulator rows x 16 columns: the wgmma fragment (pairs of columns) is turned into
+// 8 consecutive columns of one row per thread for the vectorised epilogue.
+constexpr int kScratchLd = 20;  // floats per staged row (16 + 4: 16-byte aligned rows, fewer bank conflicts)
+constexpr int kScratchWarpFloats = 16 * kScratchLd;
+
+// MODE 0: fp32 partial sums to the workspace (decode / prefill of the LM).
 // MODE 1: direct fused epilogue (codec convolutions / linears).
 template <int MODE>
 struct GemmRoles {
-    static constexpr int kEpiWarps = MODE == 0 ? 4 : 8;  // MODE 1: two warps per TMEM lane quadrant
-    static constexpr int kThreads = (kEpiWarps + 2) * 32;
+    static constexpr int kMmaWarpgroups = 2;  // rows [0, 64) and [64, 128) of the tile
+    static constexpr int kProducerWarp = 4 * kMmaWarpgroups;
+    static constexpr int kThreads = (kProducerWarp + 1) * 32;
 };
+constexpr int kEpiScratchBytes = GemmRoles<1>::kProducerWarp * kScratchWarpFloats * 4;  // MODE 1 staging
 
 template <int BN, int MODE>
-__global__ void __launch_bounds__(GemmRoles<MODE>::kThreads, (MODE == 0 || BN <= 128) ? 2 : 1)
+__global__ void __launch_bounds__(GemmRoles<MODE>::kThreads, BN <= 128 ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ GemmParams p) {
     extern __shared__ uint8_t smem_raw[];
     constexpr int kBTileBytes = BN * kBlockK * 2;
     constexpr int kStageBytes = kATileBytes + kBTileBytes;
-    // two accumulators: epilogue of item n overlaps MMA of n+1 (allocation size must be a power of two)
-    constexpr int kTmemCols = BN == 192 ? 512 : 2 * BN;
-    constexpr int kEpiWarps = GemmRoles<MODE>::kEpiWarps;
-    constexpr int kProducerWarp = kEpiWarps, kMmaWarp = kEpiWarps + 1;
+    constexpr int kProducerWarp = GemmRoles<MODE>::kProducerWarp;
 
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t tiles = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
     const int stages = p.stages;
     const uint32_t bars = tiles + static_cast<uint32_t>(stages) * kStageBytes;
-    // barrier block: full[stages], empty[stages], tmem_full[2], tmem_empty[2], TMEM base word
-    const uint32_t full0 = bars, empty0 = bars + 8u * stages, tfull0 = bars + 16u * stages;
-    const uint32_t tempty0 = tfull0 + 16u;
-    const uint32_t tmem_slot = tempty0 + 16u;
-    uint32_t* tmem_slot_ptr =
-        reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - raw));
+    // barrier block: full[stages], empty[stages]; then the epilogue staging (kEpiScratchBytes, MODE 1)
+    const uint32_t full0 = bars, empty0 = bars + 8u * stages;
+    float* scratch = reinterpret_cast<float*>(smem_raw + (bars - raw) + 16 * stages);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -209,19 +196,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < stages; ++s) {
             mbar_init(full0 + 8u * s, 1);
-            mbar_init(empty0 + 8u * s, 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tfull0 + 8u * a, 1);
-            mbar_init(tempty0 + 8u * a, kEpiWarps);  // one arrival per epilogue warp
+            mbar_init(empty0 + 8u * s, kProducerWarp);  // one arrival per MMA warp
         }
         fence_mbar_init();
     }
-    if (warp == kMmaWarp) tmem_alloc(tmem_slot, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
     pdl_launch_dependents();  // let the consumer kernel get resident; it blocks in griddepcontrol.wait
     if (warp == kProducerWarp) {
@@ -289,92 +268,73 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == kMmaWarp) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc(BN);
-            int it = 0;
-            for (int n = item_begin; n < item_end; ++n) {
-                int i0, j0, kb0, kb1, slot;
-                get_item(n, i0, j0, kb0, kb1, slot);
-                const int a = (n - item_begin) & 1;
-                const uint32_t aph = static_cast<uint32_t>((n - item_begin) >> 1) & 1u;
-                mbar_wait(tempty0 + 8u * a, aph ^ 1u);  // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(a * BN);
-                uint32_t acc = 0;
-                for (int kb = kb0; kb < kb1; ++kb, ++it) {
-                    const int s = it % stages;
-                    const uint32_t ph = static_cast<uint32_t>(it / stages) & 1u;
-                    mbar_wait(full0 + 8u * s, ph);
-                    tc_fence_after();
-                    const uint32_t a_src = tiles + static_cast<uint32_t>(s) * kStageBytes;
-                    const uint64_t ad = make_sdesc(a_src), bd = make_sdesc(a_src + kATileBytes);
-#pragma unroll
-                    for (int k = 0; k < kBlockK / 16; ++k) {
-                        // advance 16 elements (32 B) along K inside the swizzle atom: +2 (16 B units)
-                        umma_bf16(d_tmem, ad + 2u * k, bd + 2u * k, idesc, acc);
-                        acc = 1;
-                    }
-                    umma_commit(empty0 + 8u * s);  // frees the smem slot once these MMAs retire
-                }
-                umma_commit(tfull0 + 8u * a);  // accumulator complete
-            }
-        }
     } else {
-        // ===== epilogue: TMEM -> registers -> global =====
+        // ===== MMA warpgroups: wgmma into registers, then the epilogue of the item =====
+        const int wg = warp >> 2, wq = warp & 3;  // warpgroup = 64-row half of the tile, warp inside it
+        int it = 0;
         for (int n = item_begin; n < item_end; ++n) {
             int i0, j0, kb0, kb1, slot;
             get_item(n, i0, j0, kb0, kb1, slot);
-            const int a = (n - item_begin) & 1;
-            const uint32_t aph = static_cast<uint32_t>((n - item_begin) >> 1) & 1u;
-            mbar_wait(tfull0 + 8u * a, aph);
-            tc_fence_after();
-            const int quad = warp & 3, half = warp >> 2;  // TMEM lane quadrant is fixed by warp id % 4
-            const int i = i0 + quad * 32 + lane;
-            const bool i_ok = i < p.rows_i;
-            const uint32_t taddr =
-                tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + static_cast<uint32_t>(a * BN);
-            if (MODE == 0) {
-                float* base = p.ws + static_cast<size_t>(slot) * p.ws_slot_stride;
-#pragma unroll 1
-                for (int c0 = 0; c0 < BN; c0 += 32) {
-                    uint32_t r[32];
-                    tmem_ld32(taddr + c0, r);
-                    tmem_ld_wait();
-                    if (i_ok) {
+            float d[BN / 2];
 #pragma unroll
-                        for (int jj = 0; jj < 32; ++jj) {
-                            const int j = j0 + c0 + jj;
-                            if (j < p.rows_j)
-                                base[static_cast<size_t>(j) * p.ws_ld + i] = __uint_as_float(r[jj]);
-                        }
-                    }
-                }
-            } else {
-                // the two warps of a lane quadrant take alternate 32-column chunks
-#pragma unroll 1
-                for (int c0 = half * 32; c0 < BN; c0 += 32 * (kEpiWarps / 4)) {
-                    uint32_t r[32];
-                    uint4 rr[4];
-                    const bool live = i_ok && j0 + c0 < p.rows_j;
-                    if (live) epilogue_preload(p, i, j0 + c0, z, rr);
-                    tmem_ld32(taddr + c0, r);
-                    tmem_ld_wait();
-                    if (live) epilogue_chunk<BN>(p, r, rr, i, j0 + c0, z);
+            for (int e = 0; e < BN / 2; ++e) d[e] = 0.f;
+            for (int kb = kb0; kb < kb1; ++kb, ++it) {
+                const int s = it % stages;
+                mbar_wait(full0 + 8u * s, static_cast<uint32_t>(it / stages) & 1u);
+                const uint32_t a_src = tiles + static_cast<uint32_t>(s) * kStageBytes;
+                const uint64_t ad = make_gdesc(a_src + wg * kHalfATileBytes), bd = make_gdesc(a_src + kATileBytes);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBlockK / 16; ++k) wgmma_bf16<BN>(d, ad + 2u * k, bd + 2u * k, 1);
+                wgmma_commit();
+                // the previous k-block's MMAs have retired: its ring slot goes back to the producer
+                wgmma_wait<1>();
+                if (kb > kb0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
                 }
             }
-            // release the accumulator to the MMA warp
-            tc_fence_before();
+            wgmma_wait<0>();
             __syncwarp();
-            if (lane == 0) mbar_arrive(tempty0 + 8u * a);
+            if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
+
+            const int rbase = i0 + wg * 64 + wq * 16;  // this warp's 16 rows
+            if (MODE == 0) {
+                float* base = p.ws + static_cast<size_t>(slot) * p.ws_slot_stride;
+#pragma unroll
+                for (int b = 0; b < BN / 8; ++b)
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) {
+                        const int i = rbase + (lane >> 2) + 8 * (r >> 1);
+                        const int j = j0 + 8 * b + 2 * (lane & 3) + (r & 1);
+                        if (i < p.rows_i && j < p.rows_j) base[static_cast<size_t>(j) * p.ws_ld + i] = d[4 * b + r];
+                    }
+            } else {
+                float* sw = scratch + warp * kScratchWarpFloats;
+                const int i = rbase + (lane & 15);
+#pragma unroll
+                for (int c0 = 0; c0 < BN; c0 += 16) {
+                    if (j0 + c0 >= p.rows_j) break;  // warp-uniform
+#pragma unroll
+                    for (int bb = 0; bb < 2; ++bb)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int e = 4 * (c0 / 8 + bb) + 2 * h;
+                            *reinterpret_cast<float2*>(sw + ((lane >> 2) + 8 * h) * kScratchLd + 8 * bb + 2 * (lane & 3)) =
+                                make_float2(d[e], d[e + 1]);
+                        }
+                    __syncwarp();
+                    float v[kEpiCols];
+                    const float4 q0 = *reinterpret_cast<const float4*>(sw + (lane & 15) * kScratchLd + (lane >> 4) * 8);
+                    const float4 q1 = *reinterpret_cast<const float4*>(sw + (lane & 15) * kScratchLd + (lane >> 4) * 8 + 4);
+                    __syncwarp();
+                    v[0] = q0.x; v[1] = q0.y; v[2] = q0.z; v[3] = q0.w;
+                    v[4] = q1.x; v[5] = q1.y; v[6] = q1.z; v[7] = q1.w;
+                    const int jb = j0 + c0 + (lane >> 4) * 8;
+                    if (i < p.rows_i && jb < p.rows_j) epilogue_chunk(p, v, i, jb, z);
+                }
+            }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kMmaWarp) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, kTmemCols);
     }
 }
 
@@ -453,13 +413,14 @@ int gemm_plan_init(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, i
     FSB_TRY(gemm_make_tmap(&plan->tmA, A, kBlockM));
     FSB_TRY(gemm_make_tmap(&plan->tmB, B, bn));
     const int stage_bytes = kATileBytes + bn * kBlockK * 2;
-    const int max_stages = (227 * 1024 - 1024 - 256) / stage_bytes;
+    const int scratch_bytes = kEpiScratchBytes;  // reserved whatever the mode
+    const int max_stages = (227 * 1024 - 1024 - 256 - scratch_bytes) / stage_bytes;
     if (stages > max_stages) stages = max_stages;
     if (stages > kMaxStages) stages = kMaxStages;
     FSB_CHECK(stages >= 2, "not enough shared memory for 2 stages");
     plan->bn = bn;
     plan->p.stages = stages;
-    plan->smem = static_cast<size_t>(stages) * stage_bytes + 1024 + 16 * stages + 64;
+    plan->smem = static_cast<size_t>(stages) * stage_bytes + 1024 + 16 * stages + scratch_bytes;
     plan->grid = dim3(tiles_i, tiles_j, batch);
     plan->p.sched = nullptr;
     plan->p.cta_items = nullptr;
@@ -520,10 +481,10 @@ int gemm_plan_streamk(GemmPlan* plan, int tiles_i, int kblocks, int num_ctas, bo
 int gemm_plan_tiled(GemmPlan* plan, int tiles_i, int tiles_j, int batch, int ctas_per_sm) {
     const long long total = static_cast<long long>(tiles_i) * tiles_j * batch;
     FSB_CHECK(total > 0 && total < (1ll << 31), "gemm_plan_tiled: bad tile count");
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // persistent CTAs: one per SM, or two where shared memory and TMEM allow (narrow tiles: more epilogue
+    int dev = 0, sms = 0;
+    FSB_CUDA(cudaGetDevice(&dev));
+    FSB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    // persistent CTAs: one per SM, or two where shared memory and registers allow (narrow tiles: more epilogue
     // warps in flight for the memory-bound layers)
     const long long slots = static_cast<long long>(sms) * (ctas_per_sm > 1 ? 2 : 1);
     const long long ctas = total < slots ? total : slots;

@@ -1,15 +1,14 @@
-// Generic multi-tap GEMM on the 5th-gen tensor cores (tcgen05.mma, accumulators in TMEM, operands
-// staged by TMA with the 128-byte swizzle).  One kernel serves
-//   * the Dual-AR decode step (weights = operand A on the TMEM lanes, the <=32 batch rows = operand B,
-//     host-scheduled stream-K work items, fp32 partial sums reduced by the consuming kernel),
-//   * LM prefill (same orientation, wide N tiles),
+// Generic multi-tap GEMM on the Hopper tensor cores (wgmma, accumulators in registers, operands staged by TMA with
+// the 128-byte swizzle).  One kernel serves
+//   * LM prefill (weights = operand A on the 128 tile rows, the token rows = operand B, fp32 results to a workspace),
+//   * stream-K scheduled skinny products (host-built work items, fp32 partial sums reduced by the consumer),
 //   * the codec's Conv1d / ConvTranspose1d / Linear layers as implicit-im2col GEMMs: each conv tap is
 //     a K-range whose activation tile is fetched by TMA at a shifted time coordinate; out-of-range
 //     rows (the causal left pad) are zero-filled by the TMA unit itself.
 //
 //   D[z][i][j] = sum_tap sum_k  A[zA][i + a_shift[tap]][a_tapk*tap + k] * B[zB][j + b_shift[tap]][b_tapk*tap + k]
 //
-// i indexes TMEM lanes (128 per tile), j indexes TMEM columns (BN per tile).
+// i indexes the 128 rows of a tile (two warpgroups of 64), j the BN columns (the wgmma N).
 #pragma once
 #include "common.cuh"
 

@@ -76,7 +76,7 @@ struct fsb_lm {
     unsigned long long* slot_seed = nullptr;
     bool graph_slot_control = false;
     fsb_lm_config cfg;
-    int num_sms = 148;
+    int num_sms = 0;
     int step_ctas = 0, step_stages = 4;
     Stack slow, fast;
     const bf16 *emb = nullptr, *cb_emb = nullptr, *norm_w = nullptr, *head_w = nullptr;
@@ -131,7 +131,7 @@ int dalloc(fsb_lm* h, T** p, size_t count, const char* name = nullptr) {
     return 0;
 }
 
-// Prefill plan: A = weight [n_out, k] on the TMEM lanes, B = activations [rows, k], fp32 result ws[row][n_out].
+// Prefill plan: A = weight [n_out, k] on the 128 tile rows, B = activations [rows, k], fp32 result ws[row][n_out].
 int make_prefill_plan(fsb_lm* h, GemmPlan* plan, const bf16* w, int n_out, int k, const bf16* act, int act_rows,
                       int bn = 128) {
     memset(plan, 0, sizeof(*plan));
@@ -166,8 +166,14 @@ int launch_rows_of(const GemmPlan& plan, int rows, cudaStream_t st) {
 
 int launch_rows_of(const GemmPlan& plan, const GemmPlan& wide, int rows, cudaStream_t st) {
     static const bool on = [] { const char* e = getenv("FSB_PREFILL_WIDE"); return !(e && e[0] == '0'); }();
+    static const int sms = [] {
+        int d = 0, n = 0;
+        cudaGetDevice(&d);
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
+        return n;
+    }();
     const long long tiles_wide = static_cast<long long>(wide.grid.x) * cdiv(rows, 256);
-    return (on && rows >= 512 && tiles_wide >= 296) ? launch_rows_of(wide, rows, st) : launch_rows_of(plan, rows, st);
+    return (on && rows >= 512 && tiles_wide >= 2 * sms) ? launch_rows_of(wide, rows, st) : launch_rows_of(plan, rows, st);
 }
 
 // Step GEMM over the weight `w` [n_out, K]. act != null: operand X = act, used as it is; act == null: operand X = the
@@ -471,8 +477,8 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
         delete h;
         return 1;
     }
-    if (prop.major != 10) {
-        set_error("fishb200 kernels are built for sm_100a only (device is sm_%d%d)", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("fishb200 kernels are built for sm_90a only (device is sm_%d%d)", prop.major, prop.minor);
         delete h;
         return 1;
     }

@@ -1,11 +1,10 @@
-// See lm_gemm.cuh.  CTA = 10 warps (6 when operand X needs no normalisation):
-//   warps 0-3  TMEM -> registers -> fp32 partial stores of this GEMM
+// See lm_gemm.cuh.  CTA = 5 warps (9 when operand X is normalised on load):
+//   warps 0-3  one warpgroup: wgmma over the ring, fp32 partial stores of this GEMM from the accumulator registers
 //   warp  4    TMA producer (weights and operand X)
-//   warp  5    TMEM allocator + single-thread tcgen05.mma issuer
-//   warps 6-9  operand-X normalisers (NORM == 1): RMSNorm of the TMA-delivered residual rows, in place in the ring
+//   warps 5-8  operand-X normalisers (NORM == 1): RMSNorm of the TMA-delivered residual rows, in place in the ring
 // step_finalize_kernel (the consumer-side finish of a GEMM: residual add / SwiGLU) lives here as well.
 #include "lm_gemm.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 #include <stdlib.h>
 
@@ -19,10 +18,12 @@ namespace {
 constexpr int kBN = kStepRows;
 constexpr int kBTileBytes = kBN * kBlockK * 2;  // 4 KB
 constexpr int kStageBytes = kATileBytes + kBTileBytes;
-constexpr int kTmemCols = 2 * kBN;  // two accumulators: the stores of item n overlap the MMAs of item n+1
 constexpr int kEpiThreads = 128;
+constexpr int kMmaThreads = 128;  // one warpgroup
+constexpr int kProducerWarp = kMmaThreads / 32;
+constexpr int kStepThreads = kMmaThreads + 32;  // + the TMA producer warp
 constexpr int kLoaderThreads = 128;  // four normaliser warps: two 16-byte cells per thread and k-block
-constexpr int kScratchBytes = 1024;  // r_s[32] | red[4][32]
+constexpr int kScratchBytes = 1024;  // r_s[32] | spare
 
 __device__ __forceinline__ void bar_sync(int id, int n) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
@@ -152,7 +153,7 @@ __global__ void __launch_bounds__(kEpiThreads) step_finalize_kernel(const __grid
 }
 
 template <int NORM>
-__global__ void __launch_bounds__(NORM ? 192 + kLoaderThreads : 192, 2)
+__global__ void __launch_bounds__(kStepThreads + (NORM ? kLoaderThreads : 0), 2)
 step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ StepGemmParams p) {
     extern __shared__ uint8_t smem_raw[];
@@ -160,52 +161,34 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const uint32_t tiles = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
     const int stages = p.stages;
     const uint32_t bars = tiles + static_cast<uint32_t>(stages) * kStageBytes;
-    // barrier block: full[stages] (tile ready for the MMA), empty[stages], rawx[stages] (un-normalised X landed),
-    // tmem_full[2], tmem_empty[2], TMEM base word
+    // barrier block: full[stages] (tile ready for the MMA), empty[stages], rawx[stages] (un-normalised X landed)
     const uint32_t full0 = bars, empty0 = bars + 8u * stages, rawx0 = bars + 16u * stages;
-    const uint32_t tfull0 = bars + 24u * stages, tempty0 = tfull0 + 16u;
-    const uint32_t tmem_slot = tempty0 + 16u + 8u;
-    const int scratch_off = ((24 * stages + 56 + 15) / 16) * 16;
+    const int scratch_off = ((24 * stages + 15) / 16) * 16;
     uint8_t* gen = smem_raw + (tiles - raw);
     uint8_t* bar_gen = gen + static_cast<size_t>(stages) * kStageBytes;
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(bar_gen + 24 * stages + 40);
     float* scratch = reinterpret_cast<float*>(bar_gen + scratch_off);
     float* r_s = scratch;       // [32] per-row rsqrt (normalisers)
-    float* red = scratch + 32;  // [4][32] spare
     uint4* normw_s = reinterpret_cast<uint4*>(bar_gen + scratch_off + kScratchBytes);  // [kblocks*8] norm weights
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int item_begin = p.cta_items[blockIdx.x], item_end = p.cta_items[blockIdx.x + 1];
     unsigned long long* trace = p.trace ? p.trace + static_cast<size_t>(blockIdx.x) * 8 : nullptr;
-    if (trace && threadIdx.x == 0) {
-        unsigned smid;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        trace[0] = globaltimer_ns();
-        (void)smid;
-    }
+    if (trace && threadIdx.x == 0) trace[0] = globaltimer_ns();
 
-    if (warp == 4 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < stages; ++s) {
             mbar_init(full0 + 8u * s, 1 + (NORM ? kLoaderThreads / 32 : 0));
-            mbar_init(empty0 + 8u * s, 1);
+            mbar_init(empty0 + 8u * s, kMmaThreads / 32);  // one arrival per MMA warp
             mbar_init(rawx0 + 8u * s, 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tfull0 + 8u * a, 1);
-            mbar_init(tempty0 + 8u * a, 4);  // one arrival per epilogue warp
         }
         fence_mbar_init();
     }
-    if (warp == 5) tmem_alloc(tmem_slot, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
     pdl_launch_dependents();
-    if (warp == 4) {
+    if (warp == kProducerWarp) {
         // ===== TMA producer. Weights do not depend on the upstream kernel: the first ring-full of weight
         // tiles is requested BEFORE griddepcontrol.wait, so this GEMM's HBM stream starts while the previous
         // kernel is still in its tail. Operand X follows once it is complete. =====
@@ -231,8 +214,7 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                         }
                     }
                 }
-                // ... optionally (FSB_L2_PREFETCH, default 0: measured no gain, profiles/r02_l2_prefetch.md) the weight
-                // tiles after those are requested into L2
+                // ... optionally (FSB_L2_PREFETCH, default 0) the weight tiles after those are requested into L2
                 for (int q = 0; q < p.l2_prefetch && n < item_end; ++q) {
                     tma_prefetch_l2_3d(&tmA, kb * kBlockK, w.x * kBlockM, 0);
                     if (++kb >= w.z) {
@@ -266,40 +248,10 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 5) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc(kBN);
-            int it = 0;
-            for (int n = item_begin; n < item_end; ++n) {
-                const int4 w = p.sched[n];
-                const int a = (n - item_begin) & 1;
-                const uint32_t aph = static_cast<uint32_t>((n - item_begin) >> 1) & 1u;
-                mbar_wait(tempty0 + 8u * a, aph ^ 1u);  // the stores of this accumulator's previous item are done
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(a * kBN);
-                uint32_t acc = 0;
-                for (int kb = w.y; kb < w.z; ++kb, ++it) {
-                    const int s = it % stages;
-                    const uint32_t ph = static_cast<uint32_t>(it / stages) & 1u;
-                    mbar_wait(full0 + 8u * s, ph);
-                    tc_fence_after();
-                    const uint32_t a_src = tiles + static_cast<uint32_t>(s) * kStageBytes;
-                    const uint64_t ad = make_sdesc(a_src), bd = make_sdesc(a_src + kATileBytes);
-#pragma unroll
-                    for (int k = 0; k < kBlockK / 16; ++k) {
-                        umma_bf16(d_tmem, ad + 2u * k, bd + 2u * k, idesc, acc);
-                        acc = 1;
-                    }
-                    umma_commit(empty0 + 8u * s);  // frees the ring slot once these MMAs retire
-                }
-                umma_commit(tfull0 + 8u * a);  // accumulator complete
-            }
-        }
-    } else if (warp >= 6) {
+    } else if (warp > kProducerWarp) {
         // ===== operand-X normalisers: rbf(rbf(x * r_row) * w) in place on the swizzled tile TMA delivered =====
         if (NORM) {
-            const int t = threadIdx.x - 192;  // 0..127
+            const int t = threadIdx.x - kStepThreads;  // 0..127
             // the norm weights are constants: stage them before waiting for the upstream kernel
             const int nchunks = ((p.K + kBlockK - 1) / kBlockK) * 8;
             for (int ch = t; ch < nchunks; ch += kLoaderThreads)
@@ -370,43 +322,65 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
         }
     } else {
-        // ===== warps 0-3: TMEM -> registers -> fp32 partial stores =====
-        const int tid = threadIdx.x;  // 0..127 = TMEM lane = feature inside the tile
+        // ===== warpgroup 0: wgmma over the ring (rows [0, 64) and [64, 128) of the weight tile), then the fp32
+        // partial stores straight from the accumulator registers =====
         pdl_wait();
+        int it = 0;
         for (int n = item_begin; n < item_end; ++n) {
             const int4 w = p.sched[n];
             const int tile = w.x, slot = w.w;
-            const int a = (n - item_begin) & 1;
-            const uint32_t aph = static_cast<uint32_t>((n - item_begin) >> 1) & 1u;
-            mbar_wait(tfull0 + 8u * a, aph);
-            tc_fence_after();
-            if (trace && tid == 0 && n == item_begin) trace[4] = globaltimer_ns();
-            uint32_t r[32];
-            tmem_ld32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + static_cast<uint32_t>(a * kBN), r);
-            tmem_ld_wait();
-            // the accumulator is in registers: hand it back to the MMA warp right away
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty0 + 8u * a);
-            float* dst = p.ws + ((static_cast<size_t>(slot) * p.tiles + tile) * 32) * 128 + tid;
+            float d0[kBN / 2], d1[kBN / 2];
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-                if (j < p.rows) __stcg(dst + j * 128, __uint_as_float(r[j]));
+            for (int e = 0; e < kBN / 2; ++e) d0[e] = d1[e] = 0.f;
+            for (int kb = w.y; kb < w.z; ++kb, ++it) {
+                const int s = it % stages;
+                mbar_wait(full0 + 8u * s, static_cast<uint32_t>(it / stages) & 1u);
+                const uint32_t a_src = tiles + static_cast<uint32_t>(s) * kStageBytes;
+                const uint64_t a0 = make_gdesc(a_src), a1 = make_gdesc(a_src + kHalfATileBytes);
+                const uint64_t bd = make_gdesc(a_src + kATileBytes);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBlockK / 16; ++k) {
+                    wgmma_bf16<kBN>(d0, a0 + 2u * k, bd + 2u * k, 1);
+                    wgmma_bf16<kBN>(d1, a1 + 2u * k, bd + 2u * k, 1);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();  // the previous k-block's MMAs have retired: release its ring slot
+                if (kb > w.y) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
+                }
+            }
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
+            if (trace && threadIdx.x == 0 && n == item_begin) trace[4] = globaltimer_ns();
+            // accumulator element (feature i, batch row j) -> ws[slot][tile][j][i]
+            float* dst = p.ws + ((static_cast<size_t>(slot) * p.tiles + tile) * 32) * 128;
+            const int i0 = warp * 16 + (lane >> 2);
+#pragma unroll
+            for (int b = 0; b < kBN / 8; ++b)
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    const int j = 8 * b + 2 * (lane & 3) + (r & 1);
+                    const int i = i0 + 8 * (r >> 1);
+                    if (j < p.rows) {
+                        __stcg(dst + j * 128 + i, d0[4 * b + r]);
+                        __stcg(dst + j * 128 + 64 + i, d1[4 * b + r]);
+                    }
+                }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (trace && threadIdx.x == 0) trace[5] = globaltimer_ns();
-    if (warp == 5) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, kTmemCols);
+    if (trace) {
+        __syncthreads();
+        if (threadIdx.x == 0) trace[5] = globaltimer_ns();
     }
 }
 
 template <int NORM>
 int launch_t(const StepGemmPlan& plan, cudaStream_t st) {
     auto k = step_gemm_kernel<NORM>;
-    FSB_LAUNCH(k, plan.grid, dim3(NORM ? 192 + kLoaderThreads : 192), plan.smem, st, plan.tmA, plan.tmB, plan.p);
+    FSB_LAUNCH(k, plan.grid, dim3(kStepThreads + (NORM ? kLoaderThreads : 0)), plan.smem, st, plan.tmA, plan.tmB, plan.p);
     return 0;
 }
 
@@ -444,26 +418,18 @@ int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K,
     const int tiles = cdiv(n_out, kBlockM), kblocks = cdiv(K, kBlockK);
     const int normw_bytes = norm ? kblocks * 128 : 0;
     auto smem_of = [&](int st) {
-        return static_cast<size_t>(1024) + static_cast<size_t>(st) * kStageBytes + ((24 * st + 56 + 15) / 16) * 16 +
+        return static_cast<size_t>(1024) + static_cast<size_t>(st) * kStageBytes + ((24 * st + 15) / 16) * 16 +
                kScratchBytes + normw_bytes;
     };
     while (stages > 2 && 2 * (smem_of(stages) + 1024) > 228 * 1024) --stages;  // two CTAs per SM
     FSB_CHECK(stages >= 2, "step GEMM: ring too shallow");
-    // One wave: the stream-K ranges assume every CTA runs at once. cudaOccupancyMaxActiveBlocksPerMultiprocessor reports
-    // 1 for every kernel that allocates tensor memory, although two such CTAs do share an SM (verified with %smid
-    // stamps): count registers and shared memory ourselves.
-    int dev = 0, sms = 0, smem_sm = 0, regs_sm = 0, resv = 0;
+    // One wave: the stream-K ranges assume every CTA runs at once.
+    int dev = 0, sms = 0, per_sm = 0;
     FSB_CUDA(cudaGetDevice(&dev));
     FSB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    FSB_CUDA(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
-    FSB_CUDA(cudaDeviceGetAttribute(&regs_sm, cudaDevAttrMaxRegistersPerMultiprocessor, dev));
-    FSB_CUDA(cudaDeviceGetAttribute(&resv, cudaDevAttrReservedSharedMemoryPerBlock, dev));
-    cudaFuncAttributes fa;
-    FSB_CUDA(cudaFuncGetAttributes(&fa, kernel));
-    const int threads = norm ? 192 + kLoaderThreads : 192;
-    const int regs_cta = ((fa.numRegs + 7) / 8) * 8 * threads;
-    const int per_sm = std::min<int>(regs_sm / regs_cta, smem_sm / static_cast<int>(smem_of(stages) + resv + fa.sharedSizeBytes));
-    FSB_CHECK(per_sm >= 1, "step GEMM: kernel does not fit an SM (smem %zu, %d registers)", smem_of(stages), fa.numRegs);
+    FSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kStepThreads + (norm ? kLoaderThreads : 0),
+                                                           smem_of(stages)));
+    FSB_CHECK(per_sm >= 1, "step GEMM: kernel does not fit an SM (smem %zu)", smem_of(stages));
     if (num_ctas > per_sm * sms) num_ctas = per_sm * sms;
     // stream-K: units are (tile, k-block) pairs in tile-major order; CTA c streams units [c*U/n, (c+1)*U/n)
     const long long U = static_cast<long long>(tiles) * kblocks;
@@ -508,7 +474,7 @@ int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K,
     p.prev_rb = 32;
     {
         const char* e = getenv("FSB_L2_PREFETCH");
-        p.l2_prefetch = e ? atoi(e) : 0;  // k-blocks per CTA (16 KB each); measured: no gain on B200 (profiles/)
+        p.l2_prefetch = e ? atoi(e) : 0;  // k-blocks per CTA (16 KB each)
     }
     plan->grid = dim3(static_cast<unsigned>(num_ctas), 1, 1);
     plan->smem = smem_of(stages);

@@ -1,17 +1,17 @@
 // Step GEMM: the weight-streaming matmul of the Dual-AR decode step (llama.py:831-987 one TransformerBlock;
 // inference.py:96-181 one frame).
 //
-//   D[i][j] = sum_k W[i][k] * X[j][k]        i = output feature (128 per tile, on the TMEM lanes)
-//                                            j = sequence slot of the batch (<= 32, the UMMA N)
+//   D[i][j] = sum_k W[i][k] * X[j][k]        i = output feature (128 per tile: two wgmma of 64 rows)
+//                                            j = sequence slot of the batch (<= 32, the wgmma N)
 //
-// Life of one launch (one CTA = 6 warps + 4 normaliser warps, two CTAs per SM, the whole grid in one wave):
+// Life of one launch (one CTA = 5 warps + 4 normaliser warps, two CTAs per SM, the whole grid in one wave):
 //   1. The TMA producer requests the first ring-full of weight tiles at once -- before griddepcontrol.wait, i.e.
 //      while the previous kernels are still finishing: weights do not depend on anything.
 //   2. Main loop: weights HBM -> shared memory by TMA (SWIZZLE_128B, EVICT_FIRST), operand X by TMA from L2; where X
 //      is the residual stream it is *normalised on load* -- four warps apply the reference's RMSNorm
 //      (llama.py:990-1001: round(x * rsqrt(mean(x^2) + eps)) * w, two bf16 roundings) in place in shared memory, with
-//      the per-row sum of squares the producer of the residual stream left behind -- and tcgen05.mma accumulates in
-//      TMEM.  Work is a host-built stream-K schedule: (tile, k-block) units cut into equal contiguous ranges, one per
+//      the per-row sum of squares the producer of the residual stream left behind -- and wgmma accumulates in
+//      registers.  Work is a host-built stream-K schedule: (tile, k-block) units cut into equal contiguous ranges, one per
 //      CTA, so every SM streams the same number of weight bytes whatever the shape.
 //   3. Each CTA stores its fp32 partials and exits: no tail holds shared memory, so the next GEMM's CTAs move in and
 //      start step 1 while this launch drains and its consumer runs.
@@ -22,10 +22,8 @@
 //                              PRO_SWIGLU  silu(w1 x) * w3 x on the row-interleaved w1|w3 result   (llama.py:979-987)
 //   attention (lm_kernels.cuh) bias, per-head nn.RMSNorm, RoPE, KV append for the qkv GEMM          (llama.py:891-911)
 //   sampler (lm_kernels.cuh)   bf16 logits of the two heads                                        (llama.py:447-457)
-// Measured alternatives (profiles/r02_decode_structure.md): finishing a GEMM inside its own kernel (last-arriving CTA
-// or all contributors after a per-tile arrival) or inside the consumer GEMM's prologue behind a grid-wide arrival
-// were 6.2-7.2 ms per frame against 5.5 ms for this schedule: a tail or a prologue holds the shared memory the next
-// GEMM's weight prefetch needs.
+// The finish runs in a kernel of its own rather than in a tail of this GEMM (last-arriving CTA) or in the prologue of
+// the consumer GEMM: a tail or a prologue holds the shared memory the next GEMM's weight prefetch needs.
 #pragma once
 #include "gemm_tc.cuh"
 
@@ -33,7 +31,7 @@ namespace fsb {
 
 enum StepPro { PRO_NONE = 0, PRO_RESID = 1, PRO_SWIGLU = 2 };
 
-constexpr int kStepRows = 32;   // batch rows per step = UMMA N
+constexpr int kStepRows = 32;   // batch rows per step = wgmma N
 constexpr int kSsqStride = 32;  // floats per row of a sum-of-squares array: one per 128-feature tile (D <= 4096)
 
 // fp32 stream-K partials of one step GEMM:

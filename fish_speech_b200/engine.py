@@ -61,7 +61,7 @@ class LmEngine:
                  kv_len: Optional[int] = None, max_rows: int = 2048, max_frames: Optional[int] = None,
                  debug: bool = False):
         if not torch.cuda.is_available():
-            raise _lib.FsbError("fish_speech_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise _lib.FsbError("fish_speech_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.lib = _lib.lib()
         self.cfg = config
         self.im_end_id = int(im_end_id)

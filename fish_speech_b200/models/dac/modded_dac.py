@@ -103,7 +103,7 @@ class _Snake:
 class DAC:
     def __init__(self, cfg: CodecConfig, state_dict: dict, device="cuda"):
         if not torch.cuda.is_available():
-            raise _lib.FsbError("fish_speech_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise _lib.FsbError("fish_speech_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.lib = _lib.lib()
         self.cfg = cfg
         self._device = torch.device(device)

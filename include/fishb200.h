@@ -1,4 +1,4 @@
-/* fishb200 — C-ABI of the B200-native Fish-Speech inference hot path.
+/* fishb200 — C-ABI of the H100-native (sm_90a) Fish-Speech inference hot path.
  *
  * The reference (fishaudio/fish-speech @ 3dd1f85c) is pure Python/PyTorch and has no FFI of its own:
  * its boundary for this path is the Python API listed in SURVEY.md §8(b).  This header is what a

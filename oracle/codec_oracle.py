@@ -7,7 +7,7 @@ CPU restatement of the reference codec ("Firefly VQ-GAN" = modified Descript-DAC
                                          CausalTransConvNet :563-588, WindowLimitedTransformer :349-439
   fish_speech/models/dac/rvq.py          DownsampleResidualVectorQuantize.forward :293-343, decode :352-366,
                                          ConvNeXtBlock :129-191
-  descript-audio-codec 1.0.0 (third party, NOT in /root/reference; pinned by uv.lock:864-865):
+  descript-audio-codec 1.0.0 (third party, NOT in the reference checkout; pinned by uv.lock:864-865):
       dac/nn/layers.py  Snake1d  x + 1/(alpha+1e-9) * sin(alpha x)^2 ; WNConv1d = weight_norm(Conv1d)
       dac/nn/quantize.py VectorQuantize.decode_latents (L2-normalised nearest neighbour),
                          ResidualVectorQuantize.forward / from_codes

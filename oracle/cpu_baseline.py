@@ -3,13 +3,10 @@
 The reference's own CPU implementation of the hot path, timed on the box's host cores for bench.py's
 `--impl reference` arm and its `cpu_baseline` object.
 
-* kind "reference": /root/reference is present (the build container) -> the UNMODIFIED reference modules
-  (`fish_speech.models.text2semantic.{llama,inference}`, `fish_speech.models.dac.{modded_dac,rvq}`) imported
-  through oracle/ref_stubs.py are what is timed: `decode_one_token_ar` for the prefill and for every decode
-  frame (inference.py:96-181, called the way `generate` / `decode_n_tokens` call it, :184-238, :322-352) and
-  `DAC.from_indices` (modded_dac.py:925-946).
-* kind "port": /root/reference does not exist (the GPU box) -> the oracle restatement (oracle/lm_oracle.py,
-  oracle/codec_oracle.py), pinned bit-exact to the reference by oracle/make_golden*.py.
+What is timed is the oracle restatement of the reference (oracle/lm_oracle.py, oracle/codec_oracle.py; kind
+"port"), pinned bit-exact to the reference by oracle/make_golden*.py: `decode_one_token_ar` for the prefill and for
+every decode frame (inference.py:96-181, called the way `generate` / `decode_n_tokens` call it, :184-238, :322-352)
+and `DAC.from_indices` (modded_dac.py:925-946).
 
 Workload = bench.py's (batch-32 text->codec->wav, 64-token prompts, 256 frames per utterance, S2-Pro 4B +
 391 M codec geometry, greedy). The reference is a batch-1 implementation (`max_batch_size=1`, inference.py:285),
@@ -83,20 +80,7 @@ class CpuHotPath:
         self.cfg = O.LMConfig(max_seq_len=512)
         w = _lm_weights(self.cfg)
         self.kind = "port"
-        self._ref = None
-        if os.path.isdir("/root/reference/fish_speech"):
-            try:
-                from oracle import ref_stubs as R
-
-                self._model = R.reference_lm(self.cfg, w, assign=True)
-                from fish_speech.models.text2semantic import inference as ref_inf
-
-                self._ref = ref_inf
-                self.kind = "reference"
-            except Exception:  # pragma: no cover - fall back to the pinned port
-                self._ref = None
-        if self._ref is None:
-            self._st = O.setup(self.cfg, w)
+        self._st = O.setup(self.cfg, w)
         del w
         g = torch.Generator().manual_seed(42)
         self.prompt = torch.zeros(self.cfg.num_codebooks + 1, T_PROMPT, dtype=torch.long)
@@ -111,29 +95,17 @@ class CpuHotPath:
         if with_codec:
             self.ccfg = CO.full_config()
             cw = CO.make_weights(self.ccfg, seed=6)
-            if self.kind == "reference":
-                from oracle.make_golden_codec import reference_dac
-
-                self._dac = reference_dac(self.ccfg, cw)
-                self._codec = lambda codes: self._dac.from_indices(codes)
-            else:
-                self._codec = lambda codes: CO.from_indices(cw, self.ccfg, codes)
+            self._codec = lambda codes: CO.from_indices(cw, self.ccfg, codes)
 
     # ---- LM ----
     def _one(self, x, input_pos, prev):
         C1 = self.cfg.num_codebooks + 1
-        if self._ref is not None:
-            return self._ref.decode_one_token_ar(self._model, x.view(1, C1, -1), input_pos, self._temp, self._top_p, 1,
-                                                 self._bias, None, None, previous_tokens=prev)
         return O.decode_one_token_ar(self._st, x.view(1, C1, -1), input_pos, self._temp, self._top_p, 1, self._bias,
                                      previous_tokens=prev)
 
     @torch.inference_mode()
     def prefill(self) -> float:
         """The prefill call of `generate` (inference.py:322-335) on the 64-token prompt; (re)starts the utterance."""
-        if self._ref is not None and not getattr(self._model, "_cache_setup_done", False):
-            self._model.setup_caches(max_batch_size=1, max_seq_len=self.cfg.max_seq_len, dtype=torch.bfloat16)
-            self._model._cache_setup_done = True
         t0 = time.perf_counter()
         first = self._one(self.prompt, torch.arange(0, T_PROMPT), None)
         dt = time.perf_counter() - t0

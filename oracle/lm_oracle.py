@@ -7,9 +7,9 @@ rounding points) of the reference's Dual-AR text2semantic inference algorithm:
   fish_speech/models/text2semantic/inference.py  (sampling, per-frame decode, generate loop)
 
 Every function cites the reference lines it follows.  The oracle is *pinned*: oracle/make_golden.py
-imports the real reference modules from /root/reference (with the stubs in oracle/ref_stubs.py), runs
+imports the real reference modules from a checkout of the reference (with the stubs in oracle/ref_stubs.py), runs
 both on the same seeded weights and inputs, asserts bit-equality and writes tests/golden/*.npz; the
-CPU test-suite re-checks the oracle against those fixtures without needing /root/reference.
+CPU test-suite re-checks the oracle against those fixtures without needing the reference.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import
 this package.

@@ -1,13 +1,13 @@
 """Pin the oracle against the REAL reference and write the golden fixtures (test infrastructure).
 
-Run in the build container only (needs /root/reference):
+Run where a checkout of the reference exists (its directory in $FISH_SPEECH_REFERENCE):
 
     python -m oracle.make_golden
 
 For every case it (1) runs the unmodified reference (imported through oracle/ref_stubs.py), (2) runs the
 oracle restatement on the same seeded weights / inputs, (3) asserts bit-equality, (4) stores inputs,
 seeds and the reference's outputs under tests/golden/.  The committed fixtures let the CPU test-suite
-and the GPU box (where /root/reference does not exist) re-check both the oracle and the CUDA path
+and the GPU suite (no reference needed) re-check both the oracle and the CUDA path
 against outputs of the reference itself.
 """
 from __future__ import annotations

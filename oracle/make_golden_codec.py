@@ -1,6 +1,6 @@
 """Pin oracle/codec_oracle.py against the REAL reference codec classes and write codec fixtures.
 
-Run in the build container (needs /root/reference): python -m oracle.make_golden_codec
+Run where a checkout of the reference exists ($FISH_SPEECH_REFERENCE): python -m oracle.make_golden_codec
 The reference DAC is instantiated by hand with the values of fish_speech/configs/modded_dac_vq.yaml
 (hydra / omegaconf are not installed here); its third-party bases come from oracle/ref_stubs.py.
 """

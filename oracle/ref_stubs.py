@@ -1,4 +1,4 @@
-"""Import the UNMODIFIED reference modules from /root/reference in this container.
+"""Import the UNMODIFIED reference modules from a checkout of the reference (directory in $FISH_SPEECH_REFERENCE).
 
 Test infrastructure only.  The reference needs three third-party packages that are not installed
 here and not vendored in its tree:
@@ -14,6 +14,7 @@ not on an installed copy.
 from __future__ import annotations
 
 import math
+import os
 import sys
 import types
 
@@ -22,7 +23,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 from torch.nn.utils.parametrizations import weight_norm
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("FISH_SPEECH_REFERENCE", "")
 
 
 def _snake(x, alpha):
@@ -164,6 +165,8 @@ def install() -> None:
     mod("dac.model.base", CodecMixin=CodecMixin)
     mod("audiotools", AudioSignal=object)
     mod("audiotools.ml", BaseModel=BaseModel)
+    if not REF_ROOT:
+        raise RuntimeError("set FISH_SPEECH_REFERENCE to the directory of a fish-speech checkout")
     if REF_ROOT not in sys.path:
         sys.path.insert(0, REF_ROOT)
 

@@ -138,7 +138,7 @@ def test_indices_clamped_in_place_like_reference(tiny):
 # except where the GPU's choice is a near-tie under the ORACLE's own fp32 scores: at the first residual stage
 # where a frame's code differs, score_oracle(best) - score_oracle(GPU's code) <= VQ_EPS (scores are
 # 2*cos - 2 in [-4, 0]); later stages of that frame quantise a different residual and are not comparable.
-# Calibration (B200, this file's five cases incl. the full 391 M geometry): worst observed gap 0.0133.
+# The bound leaves room over the largest gap observed in this file's five cases (incl. the full 391 M geometry).
 VQ_EPS = 0.03
 
 

@@ -2,6 +2,7 @@
 (launch_thread_safe_queue, inference.py:736-799) and TTSInferenceEngine.inference
 (inference_engine/__init__.py:40-142) with the device work replaced by stand-ins."""
 import queue
+from pathlib import Path
 
 import numpy as np
 import pytest
@@ -515,20 +516,15 @@ class _ByteTokenizer:
         return ids
 
 
-def test_generate_long_plan_builds_growing_prompts_with_the_reference_frontend():
-    """The REAL body of the generate_long plan (inference.py:523-733) on CPU: the reference's own prompt builder
-    (fish_speech.content_sequence / conversation from /root/reference) with a byte-level tokenizer, a driver that answers
-    every `generate` with a made-up continuation. Checks what the CUDA side relies on: every chunk's prompt EXTENDS the
-    previous chunk's prompt (prefix K/V reuse, SURVEY §8(f).2), the reference clip enters as semantic rows, each chunk
-    yields y[1:, T:-1] (the last frame is dropped, :708) and the stream ends with "next"."""
-    import sys
-    from pathlib import Path
+GOLD = Path(__file__).parent / "golden"
+_GL_TEXT = ("<|speaker:0|>" + "first sentence of the request. " * 3 + "<|speaker:1|>" +
+            "and a reply that is long enough. " * 3)
 
-    ref = Path("/root/reference")
-    if not (ref / "fish_speech" / "conversation.py").exists():
-        pytest.skip("the reference checkout (CPU-side prompt builder) is not available")
-    if str(ref) not in sys.path:
-        sys.path.insert(0, str(ref))
+
+def drive_generate_long_plan(frontend=None):
+    """The REAL body of the generate_long plan (inference.py:523-733) on CPU with a byte-level tokenizer and a driver
+    that answers every `generate` with a made-up continuation. `frontend` replaces the reference's prompt builder
+    (fish_speech.content_sequence / conversation) when given. Returns (prompts, replies, responses)."""
 
     class Model:
         class config:
@@ -538,32 +534,119 @@ def test_generate_long_plan_builds_growing_prompts_with_the_reference_frontend()
 
     tok = Model.tokenizer
     ref_codes = torch.arange(10 * 6).view(10, 6) % 1024
-    text = "<|speaker:0|>" + "first sentence of the request. " * 3 + "<|speaker:1|>" + "and a reply that is long enough. " * 3
-    plan = inf._generate_long_plan(model=Model, device="cpu", text=text, chunk_length=100, max_new_tokens=64,
-                                   temperature=0.8, top_p=0.8, top_k=30, prompt_text=["reference words"],
-                                   prompt_tokens=[ref_codes])
-    prompts, responses, reply, fake_frames = [], [], None, 0
-    while True:
-        try:
-            kind, payload = plan.send(reply)
-        except StopIteration:
-            break
-        reply = None
-        if kind == "response":
-            responses.append(payload)
-            continue
-        p = payload["prompt"]
-        assert payload["reuse_prefix"] is True and payload["max_new_tokens"] == 64
-        assert p.shape[0] == 11 and p.dtype in (torch.int32, torch.int64)
-        prompts.append(p.clone())
-        fake_frames += 1
-        n = 4 + fake_frames  # frames this "generate" produced; the last one is <|im_end|>
-        gen = torch.zeros(11, n, dtype=p.dtype)
-        gen[0] = tok.semantic_begin_id + 7 * fake_frames
-        gen[1:] = (torch.arange(10).view(10, 1) + fake_frames) % 1024
-        gen[0, -1] = tok.get_token_id("<|im_end|>")
-        reply = torch.cat([p, gen], dim=1)
+    saved = inf._reference_frontend
+    if frontend is not None:
+        inf._reference_frontend = frontend
+    try:
+        plan = inf._generate_long_plan(model=Model, device="cpu", text=_GL_TEXT, chunk_length=100, max_new_tokens=64,
+                                       temperature=0.8, top_p=0.8, top_k=30, prompt_text=["reference words"],
+                                       prompt_tokens=[ref_codes])
+        prompts, replies, responses, reply, fake_frames = [], [], [], None, 0
+        while True:
+            try:
+                kind, payload = plan.send(reply)
+            except StopIteration:
+                break
+            reply = None
+            if kind == "response":
+                responses.append(payload)
+                continue
+            p = payload["prompt"]
+            assert payload["reuse_prefix"] is True and payload["max_new_tokens"] == 64
+            assert p.shape[0] == 11 and p.dtype in (torch.int32, torch.int64)
+            prompts.append(p.clone())
+            fake_frames += 1
+            n = 4 + fake_frames  # frames this "generate" produced; the last one is <|im_end|>
+            gen = torch.zeros(11, n, dtype=p.dtype)
+            gen[0] = tok.semantic_begin_id + 7 * fake_frames
+            gen[1:] = (torch.arange(10).view(10, 1) + fake_frames) % 1024
+            gen[0, -1] = tok.get_token_id("<|im_end|>")
+            reply = torch.cat([p, gen], dim=1)
+            replies.append(reply)
+    finally:
+        inf._reference_frontend = saved
+    return prompts, replies, responses
+
+
+class _ReplayFrontend:
+    """Stand-in for the reference's prompt builder: records the conversation the plan builds at every
+    `encode_for_inference` and answers with the prompt the reference's own builder produced for that conversation
+    (tests/golden/generate_long_prompts.npz, written by oracle/make_golden_frontend.py)."""
+
+    def __init__(self, prompts):
+        self.prompts, self.calls = list(prompts), []
+
+    def __call__(self):
+        fe = self
+
+        class TextPart:
+            def __init__(self, text, cal_loss=False):
+                self.text = text
+
+        class VQPart:
+            def __init__(self, codes, cal_loss=False):
+                self.codes = codes
+
+        class Message:
+            def __init__(self, role, parts, cal_loss=False, modality=None, add_im_start=False, add_im_end=False):
+                self.role, self.parts, self.modality, self.im = role, parts, modality, (add_im_start, add_im_end)
+
+        class Conversation:
+            def __init__(self):
+                self.messages = []
+
+            def append(self, m):
+                self.messages.append(m)
+
+            def encode_for_inference(self, tokenizer, num_codebooks):
+                assert num_codebooks == 10
+                fe.calls.append([(m.role, m.modality, m.im, [getattr(q, "text", None) for q in m.parts],
+                                  [q.codes.clone() for q in m.parts if hasattr(q, "codes")]) for m in self.messages])
+                return torch.from_numpy(fe.prompts[len(fe.calls) - 1]), None, None
+
+        return TextPart, VQPart, Conversation, Message
+
+
+def test_generate_long_plan_builds_growing_prompts_with_the_reference_frontend():
+    """The REAL body of the generate_long plan (inference.py:523-733) on CPU. The reference's prompt builder is replayed
+    from the prompts it produced for this very request (recorded with the unmodified fish_speech.content_sequence /
+    conversation, where it is installed the live builder is compared with that record too). Checks what the CUDA side
+    relies on: the conversation the plan builds (system prompt with the reference clip, user turns, each chunk's codes
+    fed back as an assistant turn), every chunk's prompt EXTENDS the previous chunk's prompt (prefix K/V reuse, SURVEY
+    §8(f).2), the reference clip enters as semantic rows, each chunk yields y[1:, T:-1] (the last frame is dropped,
+    :708) and the stream ends with "next"."""
+    z = np.load(GOLD / "generate_long_prompts.npz")
+    golden = [z[f"prompt_{i}"] for i in range(int(z["count"]))]
+    try:
+        import fish_speech.conversation  # noqa: F401
+    except ImportError:
+        pass
+    else:
+        live, _, _ = drive_generate_long_plan()
+        assert len(live) == len(golden) and all(np.array_equal(a.numpy(), b) for a, b in zip(live, golden))
+    fe = _ReplayFrontend(golden)
+    prompts, replies, responses = drive_generate_long_plan(fe)
+    tok = _ByteTokenizer()
+    ref_codes = torch.arange(10 * 6).view(10, 6) % 1024
     assert len(prompts) >= 2, "the text must split into several chunks"
+    assert len(fe.calls) == len(prompts) == len(golden)
+    # the conversation behind chunk i: system, then (user, assistant-with-codes) per finished chunk, then user i and the
+    # open assistant turn the model continues
+    batches = inf.group_turns_into_batches(inf.split_text_by_speaker(_GL_TEXT), max_speakers=5, max_bytes=100)
+    assert len(batches) == len(prompts)
+    for i, msgs in enumerate(fe.calls):
+        assert len(msgs) == 2 * i + 3
+        role, _, im, texts, codes = msgs[0]
+        assert role == "system" and im == (True, True) and "<|speaker:0|>reference words" in texts
+        assert len(codes) == 1 and torch.equal(codes[0], ref_codes)
+        for k in range(i + 1):
+            assert msgs[1 + 2 * k][0] == "user" and msgs[1 + 2 * k][3] == [batches[k]]
+        for k in range(i):
+            role, modality, im, _, codes = msgs[2 + 2 * k]
+            assert role == "assistant" and modality == "voice" and im == (True, True)
+            T = prompts[k].shape[1]
+            assert len(codes) == 1 and torch.equal(codes[0], replies[k][1:, T:-1])
+        assert msgs[-1][0] == "assistant" and msgs[-1][2] == (True, False) and msgs[-1][4] == []
     # the reference clip: semantic ids on row 0, its codes on rows 1..10
     first = prompts[0]
     sem = (first[0] >= tok.semantic_begin_id) & (first[0] <= tok.semantic_end_id)

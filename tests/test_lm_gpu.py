@@ -60,6 +60,19 @@ def _reference_uniforms(cfg, rng_seed: int, frames: int, head_rows: int) -> torc
     return u
 
 
+def _stored_traces(path, frames: int) -> list:
+    z = np.load(path)
+    out = []
+    for f in range(frames):
+        scores, r = [], 0
+        while f"s_{f}_{r}" in z.files:
+            scores.append((torch.from_numpy(z[f"s_{f}_{r}"]), torch.from_numpy(z[f"cum_{f}_{r}"]), float(z[f"tp_{f}_{r}"]),
+                           torch.from_numpy(z[f"topl_{f}_{r}"])))
+            r += 1
+        out.append({"scores": scores, "ras_changed": bool(z["ras_changed"][f])})
+    return out
+
+
 @pytest.mark.parametrize("name", ["lm_tiny_topk.npz", "lm_tiny_ras.npz"])
 def test_stochastic_decode_replays_reference_rng(name):
     """top-k / top-p / temperature sampling AND the RAS substitution, bit-exact: the sampler is fed the very
@@ -89,12 +102,9 @@ def test_stochastic_decode_replays_reference_rng(name):
     # keeps one candidate more or less; or the logits on either side of the top-k cut closer than the logit tolerance
     # of this suite, so that another candidate enters the top k -- all taken from the oracle's trace of the same run);
     # the runs then follow different histories, so the comparison stops there. Everything before must be identical,
-    # RAS substitutions included.
-    traces = []
-    torch.manual_seed(int(z["rng_seed"]))
-    oref = O.generate(O.setup(cfg, w), torch.from_numpy(z["prompt"]), n, temperature=float(z["temperature"]),
-                      top_p=float(z["top_p"]), top_k=int(z["top_k"]), traces=traces)
-    assert torch.equal(oref.to(torch.int32), ref)
+    # RAS substitutions included.  The oracle's trace is stored with the golden (oracle/make_golden_traces.py, recorded
+    # where the oracle reproduces the reference run exactly): its CPU bf16 matmuls depend on the host's instruction set.
+    traces = _stored_traces(GOLD / ("trace_" + name), n)
     frames_equal, ras_verified = 0, 0
     for f in range(n):
         if T + f >= got.shape[1] or T + f >= ref.shape[1]:

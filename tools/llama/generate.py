@@ -1,5 +1,5 @@
 """tools/llama/generate.py — the entry point BASELINE.json's north_star names. In the reference commit its
-contents live in fish_speech/models/text2semantic/inference.py; this shim re-exports the B200-native
+contents live in fish_speech/models/text2semantic/inference.py; this shim re-exports the H100-native
 equivalents under the old path."""
 from fish_speech_b200.models.text2semantic.inference import (  # noqa: F401
     GenerateRequest,

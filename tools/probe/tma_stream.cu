@@ -44,6 +44,8 @@ __global__ void __launch_bounds__(64, 2) stream_kernel(const __grid_constant__ C
 }
 
 int main(int argc, char** argv) {
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     const int N = 19456, K = 2560;  // w1|w3 of one S2-Pro layer: 99.6 MB
     const int tiles = N / 128, kblocks = K / 64;
     const int layers = 12;  // rotate over distinct matrices >> L2
@@ -67,11 +69,11 @@ int main(int argc, char** argv) {
                     }
                     const size_t smem = 1024 + stages * 16384 + 16 * stages + 64;
                     const unsigned long long hint = hintsel ? kEvictFirst : kEvictNormal;
-                    for (int l = 0; l < layers; ++l) stream_kernel<<<148 * per_sm, 64, smem>>>(tms[l], tiles, kblocks, stages, tiled, hint, sink);
+                    for (int l = 0; l < layers; ++l) stream_kernel<<<sms * per_sm, 64, smem>>>(tms[l], tiles, kblocks, stages, tiled, hint, sink);
                     cudaEventRecord(e0);
                     const int reps = 3;
                     for (int r = 0; r < reps; ++r)
-                        for (int l = 0; l < layers; ++l) stream_kernel<<<148 * per_sm, 64, smem>>>(tms[l], tiles, kblocks, stages, tiled, hint, sink);
+                        for (int l = 0; l < layers; ++l) stream_kernel<<<sms * per_sm, 64, smem>>>(tms[l], tiles, kblocks, stages, tiled, hint, sink);
                     cudaEventRecord(e1);
                     cudaError_t err = cudaDeviceSynchronize();
                     float ms; cudaEventElapsedTime(&ms, e0, e1);

@@ -81,9 +81,6 @@ def lib() -> C.CDLL:
     L.fsb_lm_buffer.argtypes = [vp, C.c_char_p, C.POINTER(vp), C.POINTER(C.c_size_t)]
     L.fsb_lm_set_sampler_noise.argtypes = [vp, vp, i32, i32]
     L.fsb_lm_copy_kv.argtypes = [vp, i32, i32, i32, vp]
-    L.fsb_lm_repeat_step_gemm.argtypes = [vp, i32, i32, i32, vp]
-    L.fsb_lm_trace_frame.argtypes = [vp, i32, C.POINTER(Sampling), vp, i32, vp, i32, vp]
-    L.fsb_lm_trace_step_gemms.argtypes = [vp, vp, i32, C.POINTER(i32), vp]
     L.fsb_lm_bench_gemms.argtypes = [vp, i32, C.POINTER(C.c_double), C.POINTER(i32), vp]
     f32p, i32p, ll = C.c_void_p, C.POINTER(C.c_int), C.c_longlong
     L.fsb_conv_gemm.argtypes = [vp, i32, i32, i32, i32, ll, vp, i32, i32, i32, i32p, i32, vp, vp, vp, i32, vp, vp, vp,
@@ -99,7 +96,6 @@ def lib() -> C.CDLL:
     L.fsb_qkv_rope.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp]
     L.fsb_res_unit_supported.argtypes = [i32]
     L.fsb_res_unit.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    L.fsb_op_res_unit_trace.argtypes = [vp]
     L.fsb_op_attn_score_chunk.argtypes = [i32]
     L.fsb_op_attn_per_row.argtypes = [i32]
     L.fsb_window_attn.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp]

@@ -360,10 +360,6 @@ int fsb_conv_gemm(const void* d_x, int B, int T_in, int C_in, int row_stride, lo
 
 // One decoder ResidualUnit (Snake -> dilated conv7 -> Snake -> conv1 -> + x) as one kernel: csrc/codec_resunit.cu.
 int fsb_res_unit_supported(int C) { return res_unit_supported(C) ? 1 : 0; }
-int fsb_op_res_unit_trace(unsigned long long* d_trace) {
-    res_unit_set_trace(d_trace);
-    return 0;
-}
 int fsb_res_unit(const void* d_a, const void* d_x, int B, int T, int C, int dilation, const void* d_w7,
                  const float* d_b7, const float* d_alpha1, const float* d_inv1, const void* d_w1, const float* d_b1,
                  void* d_out0, void* d_out1, const float* d_alpha_n, const float* d_inv_n, void* stream) {

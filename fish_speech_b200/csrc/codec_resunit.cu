@@ -50,7 +50,6 @@ struct ResUnitParams {
     __nv_bfloat16* out1;      // snake_next(y)
     const float* alpha_n;
     const float* inv_n;
-    unsigned long long* trace;  // diagnostics: CTA 0, per tile 6 globaltimer stamps of thread 0 (or null)
 };
 
 __device__ __forceinline__ float ru_snake(float v, float a, float ia) {
@@ -191,15 +190,11 @@ res_unit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         for (int n = item_begin; n < item_end; ++n) {
             const int z = n / p.tiles_t;
             const int t0 = (n - z * p.tiles_t) * S::BM;
-            unsigned long long* tr = (p.trace && blockIdx.x == 0 && threadIdx.x == 0 && n - item_begin < 64)
-                                         ? p.trace + (n - item_begin) * 6 : nullptr;
-            if (tr) tr[0] = globaltimer_ns();
             float d[S::NB / 2];
             // ---- phase 1: conv7 ----
 #pragma unroll
             for (int e = 0; e < S::NB / 2; ++e) d[e] = 0.f;
             run(d, S::kQ1, [](int, uint32_t src) { return src; });
-            if (tr) tr[1] = globaltimer_ns();
             // the previous tile's bulk stores read the h / y0 buffers: they must have finished reading
             if (S::kStaged && n > item_begin && threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
             ru_bar(1, S::kMmaThreads);
@@ -220,13 +215,11 @@ res_unit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             }
             fence_proxy_async();  // generic-proxy writes of h -> visible to the tensor core's async proxy
             ru_bar(1, S::kMmaThreads);
-            if (tr) tr[2] = globaltimer_ns();
             // ---- phase 2: conv1 over h ----
 #pragma unroll
             for (int e = 0; e < S::NB / 2; ++e) d[e] = 0.f;
             run(d, S::KB, [&](int q, uint32_t) { return h_smem + static_cast<uint32_t>(q) * S::kABytes; });
             ru_bar(1, S::kMmaThreads);  // every warpgroup is done reading h before it takes snake_next(y)
-            if (tr) tr[3] = globaltimer_ns();
             // ---- epilogue 2: y = conv1 + b1 + x; store y and snake_next(y) ----
 #pragma unroll
             for (int b = 0; b < S::NB / 8; ++b) {
@@ -255,7 +248,6 @@ res_unit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     }
                 }
             }
-            if (tr) tr[4] = globaltimer_ns();
             if (S::kStaged) {
                 fence_proxy_async();  // the staged tiles -> visible to the TMA engine
                 ru_bar(1, S::kMmaThreads);
@@ -268,7 +260,6 @@ res_unit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
                 }
             }
-            if (tr) tr[5] = globaltimer_ns();
         }
         if (S::kStaged && threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete
     }
@@ -342,9 +333,6 @@ int ru_plan(RuPlan* plan, const void* a, const void* w7, const void* w1, const v
 
 }  // namespace
 
-static unsigned long long* g_ru_trace = nullptr;
-void res_unit_set_trace(unsigned long long* d_trace) { g_ru_trace = d_trace; }
-
 bool res_unit_supported(int C) { return C == 96 || C == 192 || C == 384; }
 
 int res_unit_run(const void* d_a, const void* d_x, int B, int T, int C, int dilation, const void* d_w7,
@@ -385,7 +373,6 @@ int res_unit_run(const void* d_a, const void* d_x, int B, int T, int C, int dila
     p.out0 = reinterpret_cast<__nv_bfloat16*>(d_out0);
     p.out1 = reinterpret_cast<__nv_bfloat16*>(d_out1);
     p.alpha_n = d_alpha_n; p.inv_n = d_inv_n;
-    p.trace = g_ru_trace;
     switch (C) {
         case 96: return ru_launch<96>(plan, p, st);
         case 192: return ru_launch<192>(plan, p, st);

@@ -53,7 +53,6 @@ extern thread_local int g_launch_count;  // kernels launched by this thread (ben
 // Launch with the programmatic-stream-serialization attribute (PDL): the kernel may start while its
 // predecessor in the stream is still running; every kernel launched this way executes
 // griddepcontrol.wait before it touches anything a predecessor produces (or still reads).
-bool pdl_enabled();
 template <typename... Args>
 static inline cudaError_t launch_pdl(const void* kernel, dim3 grid, dim3 block, size_t smem,
                                      cudaStream_t st, Args... args) {
@@ -68,7 +67,7 @@ static inline cudaError_t launch_pdl(const void* kernel, dim3 grid, dim3 block, 
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelExC(&cfg, kernel, kargs);
 }
 #define FSB_LAUNCH(kernel, grid, block, smem, st, ...)                                            \
@@ -217,22 +216,12 @@ __device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t src, int
                  ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(src), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
 }
-// TMA prefetch of a tile into L2 only (no shared memory, no barrier).
+// Prefetch of the line at `p` into L2 only.
 __device__ __forceinline__ void prefetch_l2(const void* p) {
     asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }
-__device__ __forceinline__ void tma_prefetch_l2_3d(const void* tmap, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
-                 ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(c2)
-                 : "memory");
-}
 
 // Programmatic dependent launch: wait for the producing grid / allow the dependent grid to start.
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");

@@ -1,6 +1,5 @@
 // Last-error storage for the C-ABI (one message per host thread).
 #include <stdarg.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -16,14 +15,5 @@ void set_error(const char* fmt, ...) {
     va_end(ap);
 }
 const char* get_error() { return g_err; }
-
-bool pdl_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("FSB_PDL");
-        v = (e && e[0] == '0') ? 0 : 1;
-    }
-    return v == 1;
-}
 
 }  // namespace fsb

@@ -29,7 +29,6 @@ struct GemmParams {
     unsigned long long a_hint, b_hint;         // L2 eviction policy per operand
     int stages;
     int a_static;  // operand A is constant data (weights): prefetch it before griddepcontrol.wait
-    int l2_prefetch;  // extra k-blocks of A per CTA prefetched into L2 before the wait
     // ---- work decomposition ----
     const int4* sched;     // optional items {tile_i | tile_j<<16, kb_begin, kb_end, slot}; else blockIdx
     const int* cta_items;  // [grid.x + 1] item range of each CTA (stream-K)
@@ -94,7 +93,6 @@ int gemm_make_tmap(CUtensorMap* tm, const GemmOperand& op, int box_rows);
 // input, d_x = raw residual stream, both bf16 [B][T][C]; w7 = [C][7][pad64(C)], w1 = [C][pad64(C)] bf16; out0 (raw, may
 // alias d_x, may be null) and out1 = Snake_next(result) (must not alias d_a).
 bool res_unit_supported(int C);
-void res_unit_set_trace(unsigned long long* d_trace);  // diagnostics: [64][6] stamps of CTA 0 (null = off)
 int res_unit_run(const void* d_a, const void* d_x, int B, int T, int C, int dilation, const void* d_w7,
                  const float* d_b7, const float* d_alpha1, const float* d_inv1, const void* d_w1, const float* d_b1,
                  void* d_out0, void* d_out1, const float* d_alpha_n, const float* d_inv_n, cudaStream_t st);

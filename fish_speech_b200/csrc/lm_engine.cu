@@ -18,8 +18,6 @@
 //
 // Reference: fish_speech/models/text2semantic/llama.py:390-466 (slow step), :799-817 (fast step),
 // fish_speech/models/text2semantic/inference.py:96-181 (one frame), :184-238 (frame loop).
-#include <stdlib.h>
-
 #include <algorithm>
 #include <map>
 #include <string>
@@ -36,6 +34,7 @@ namespace {
 
 typedef __nv_bfloat16 bf16;
 constexpr int kDecRows = kStepRows;  // decode GEMM N tile: up to 32 sequences per step
+constexpr int kStepStages = 4;       // ring depth the step GEMM plans start from (step_plan_init may shrink it)
 
 struct LayerW {
     const bf16 *attn_norm, *wqkv, *bqkv, *q_norm, *k_norm, *wo, *bo, *ffn_norm, *w13, *w2;
@@ -77,7 +76,7 @@ struct fsb_lm {
     bool graph_slot_control = false;
     fsb_lm_config cfg;
     int num_sms = 0;
-    int step_ctas = 0, step_stages = 4;
+    int step_ctas = 0;
     Stack slow, fast;
     const bf16 *emb = nullptr, *cb_emb = nullptr, *norm_w = nullptr, *head_w = nullptr;
     const bf16 *fast_emb = nullptr, *fast_norm_w = nullptr, *fast_out_w = nullptr;
@@ -102,10 +101,6 @@ struct fsb_lm {
     const float* noise_u = nullptr;
     int noise_draws = 0, noise_ld = 0;
     int ctx_lcap = 0;  // score-buffer bound for the slow attention (0 = capacity)
-    unsigned long long* trace_base = nullptr;  // fsb_lm_trace_frame: per-CTA stamps of every step GEMM of one frame
-    int trace_next = 0, trace_max = 0;
-    unsigned long long* attn_trace_base = nullptr;  // 8 stamps of CTA (0, 0) of every decode attention launch
-    int attn_trace_next = 0, attn_trace_max = 0;
     int graph_lcap = -1;
     // decode graph cache
     cudaGraphExec_t graph_exec = nullptr;
@@ -165,7 +160,6 @@ int launch_rows_of(const GemmPlan& plan, int rows, cudaStream_t st) {
 }
 
 int launch_rows_of(const GemmPlan& plan, const GemmPlan& wide, int rows, cudaStream_t st) {
-    static const bool on = [] { const char* e = getenv("FSB_PREFILL_WIDE"); return !(e && e[0] == '0'); }();
     static const int sms = [] {
         int d = 0, n = 0;
         cudaGetDevice(&d);
@@ -173,7 +167,7 @@ int launch_rows_of(const GemmPlan& plan, const GemmPlan& wide, int rows, cudaStr
         return n;
     }();
     const long long tiles_wide = static_cast<long long>(wide.grid.x) * cdiv(rows, 256);
-    return (on && rows >= 512 && tiles_wide >= 2 * sms) ? launch_rows_of(wide, rows, st) : launch_rows_of(plan, rows, st);
+    return (rows >= 512 && tiles_wide >= 2 * sms) ? launch_rows_of(wide, rows, st) : launch_rows_of(plan, rows, st);
 }
 
 // Step GEMM over the weight `w` [n_out, K]. act != null: operand X = act, used as it is; act == null: operand X = the
@@ -182,7 +176,7 @@ int make_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, int 
                    const Stack* norm_of = nullptr) {
     const bool norm = act == nullptr;
     if (norm) act = norm_of->xres;
-    return step_plan_init(plan, w, n_out, K, act, norm, h->step_ctas, h->step_stages, h->step_ws, h->step_ws_floats);
+    return step_plan_init(plan, w, n_out, K, act, norm, h->step_ctas, kStepStages, h->step_ws, h->step_ws_floats);
 }
 
 void bind_norm_on_load(StepGemmPlan* plan, const Stack& s, const bf16* norm_w, float eps) {
@@ -214,26 +208,25 @@ SlotCtl slot_ctl(const fsb_lm* h) {
     return c;
 }
 
+// One step GEMM over `rows` batch rows: first finish the producer of its operand (residual add / SwiGLU), then the GEMM.
+int launch_step(const StepGemmPlan& plan, int rows, cudaStream_t st) {
+    StepGemmPlan q = plan;
+    q.p.rows = rows;
+    FSB_TRY(step_finalize_launch(q, st));
+    return step_gemm_launch(q, st);
+}
+
 // ---- decode: one transformer stack over the batch rows, five kernels per layer. `first_qkv`: the plan of layer 0's
 // qkv GEMM when its operand is produced by a GEMM (fast_project_in) instead of a row kernel. After the last layer the
 // residual stream is complete only once the NEXT step GEMM (head / fast_output) has run its prologue. ----
 int run_stack_decode(fsb_lm* h, Stack& s, int rows, const int* row_seq, const int* row_pos, bool stop_after_kv,
                      cudaStream_t st, const StepGemmPlan* first_qkv = nullptr) {
     const float eps = h->cfg.norm_eps;
-    // finish the producer of the operand (residual add / SwiGLU), then the GEMM itself
-    auto launch = [&](const StepGemmPlan& plan) -> int {
-        StepGemmPlan q = plan;
-        q.p.rows = rows;
-        FSB_TRY(step_finalize_launch(q, st));
-        if (h->trace_base && h->trace_next < h->trace_max && q.grid.x <= 512)
-            q.p.trace = h->trace_base + static_cast<size_t>(h->trace_next++) * 8 * 512;
-        return step_gemm_launch(q, st);
-    };
     for (int l = 0; l < s.nl; ++l) {
         StepLayer& P = s.dec[l];
         const LayerW& w = s.w[l];
         const StepGemmPlan& qkv = (l == 0 && first_qkv) ? *first_qkv : P.qkv;
-        FSB_TRY(launch(qkv));
+        FSB_TRY(launch_step(qkv, rows, st));
         AttnDecodeArgs aa{};
         aa.qkv = step_plan_partials(qkv);
         aa.bias = w.bqkv;
@@ -250,13 +243,11 @@ int run_stack_decode(fsb_lm* h, Stack& s, int rows, const int* row_seq, const in
         aa.bf16_math = s.bf16_math;
         aa.kv_only = (stop_after_kv && l == s.nl - 1) ? 1 : 0;  // fast pass 0 only fills the KV cache (inference.py:147)
         aa.eps = eps;
-        if (h->attn_trace_base && h->attn_trace_next < h->attn_trace_max)
-            aa.trace = h->attn_trace_base + static_cast<size_t>(h->attn_trace_next++) * 8;
         FSB_TRY(launch_attn_decode(aa, st));
         if (aa.kv_only) return 0;
-        FSB_TRY(launch(P.wo));
-        FSB_TRY(launch(P.w13));
-        FSB_TRY(launch(P.w2));
+        FSB_TRY(launch_step(P.wo, rows, st));
+        FSB_TRY(launch_step(P.w13, rows, st));
+        FSB_TRY(launch_step(P.w2, rows, st));
     }
     return 0;
 }
@@ -332,14 +323,6 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
     const int* slots = row_slot ? row_slot : h->iota;
     Stack& s = h->slow;
     Stack& f = h->fast;
-    auto launch = [&](const StepGemmPlan& plan) -> int {
-        StepGemmPlan q = plan;
-        q.p.rows = rows;
-        FSB_TRY(step_finalize_launch(q, st));
-        if (h->trace_base && h->trace_next < h->trace_max && q.grid.x <= 512)
-            q.p.trace = h->trace_base + static_cast<size_t>(h->trace_next++) * 8 * 512;
-        return step_gemm_launch(q, st);
-    };
     auto sample_args = [&](int n, const StepGemmPlan& head) {
         SampleArgs a{};
         a.ctl = slot_ctl(h);
@@ -360,7 +343,7 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
     // ---- slow head over the selectable rows (first the last layer's FFN output is added to the residual stream,
     // unless the rows come from a prefill; the final norm is applied on load) ----
     const StepGemmPlan& head = x_is_final ? h->head_plan_direct : h->head_plan;
-    FSB_TRY(launch(head));
+    FSB_TRY(launch_step(head, rows, st));
     SampleArgs sa = sample_args(h->head_rows, head);
     sa.slow = 1;
     sa.n_sem = h->head_rows - 1;
@@ -385,7 +368,8 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
     if (h->has_proj) {
         hr.y = h->hid_d;
         FSB_TRY(launch_rows(hr, st));
-        FSB_TRY(launch(h->proj_plan));  // fast_project_in; the finalize in front of layer 0's qkv GEMM adds the bias
+        // fast_project_in; the finalize in front of layer 0's qkv GEMM adds the bias
+        FSB_TRY(launch_step(h->proj_plan, rows, st));
     } else {
         hr.y = f.xres;
         hr.ssq = f.ssq;
@@ -407,7 +391,7 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
         FSB_TRY(run_stack_decode(h, f, rows, slots, h->fpos + p * kDecRows, p == 0, st,
                                  (p == 0 && h->has_proj) ? &h->fast_qkv0_proj : nullptr));
         if (p == 0) continue;
-        FSB_TRY(launch(h->fast_out_plan));
+        FSB_TRY(launch_step(h->fast_out_plan, rows, st));
         SampleArgs fa = sample_args(c.codebook_size, h->fast_out_plan);
         fa.slow = 0;
         fa.draw_id = p;
@@ -487,14 +471,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
         delete h;
         return 1;
     }
-    {
-        // ring depth / CTAs per SM of the step GEMMs are tunable for experiments
-        const char* es = getenv("FSB_STAGES");
-        const char* ec = getenv("FSB_CTAS_PER_SM");
-        h->step_stages = es ? atoi(es) : 4;
-        const int per_sm = ec ? std::max(1, std::min(2, atoi(ec))) : 2;
-        h->step_ctas = h->num_sms * per_sm;
-    }
+    h->step_ctas = h->num_sms * 2;  // two step-GEMM CTAs per SM
 
     auto B16 = [](const void* p) { return reinterpret_cast<const bf16*>(p); };
     h->emb = B16(w->d_embeddings);
@@ -806,10 +783,7 @@ int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* l
     auto run = [&](const StepGemmPlan& p) -> int {
         bytes += p.weight_bytes;
         ++launches;
-        StepGemmPlan q = p;
-        q.p.rows = rows;
-        FSB_TRY(step_finalize_launch(q, st));
-        return step_gemm_launch(q, st);
+        return launch_step(p, rows, st);
     };
     for (int r = 0; r < reps; ++r) {
         bytes = 0;
@@ -844,61 +818,6 @@ int fsb_lm_copy_kv(fsb_lm* h, int src_slot, int dst_slot, int n_pos, void* strea
     FSB_TRY(launch_kv_copy(s.kcache, s.nl, h->cfg.max_batch, s.Hkv, s.S, s.Dh, src_slot, dst_slot, n_pos, st));
     FSB_TRY(launch_kv_copy(s.vcache, s.nl, h->cfg.max_batch, s.Hkv, s.S, s.Dh, src_slot, dst_slot, n_pos, st));
     return 0;
-}
-
-int fsb_lm_trace_frame(fsb_lm* h, int batch, const fsb_sampling* sp, unsigned long long* d_trace, int max_launches,
-                       unsigned long long* d_attn_trace, int max_attn, void* stream) {
-    // Diagnostic: ONE decode frame, eager launches (same kernels, same programmatic dependent launch as the graph),
-    // every step GEMM recording its per-CTA stamps in launch order: the in-frame timeline at GEMM granularity.
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    FSB_CHECK(h != nullptr && sp != nullptr && d_trace != nullptr, "trace_frame: null argument");
-    FSB_CHECK(batch >= 1 && batch <= h->cfg.max_batch, "trace_frame: batch=%d", batch);
-    h->trace_base = d_trace;
-    h->trace_next = 0;
-    h->trace_max = max_launches;
-    h->attn_trace_base = d_attn_trace;
-    h->attn_trace_next = 0;
-    h->attn_trace_max = d_attn_trace ? max_attn : 0;
-    const int rc = decode_one_frame(h, batch, *sp, st);
-    const int n = h->trace_next;
-    h->attn_trace_base = nullptr;
-    h->trace_base = nullptr;
-    h->trace_next = h->trace_max = 0;
-    return rc != 0 ? -1 : n;
-}
-
-int fsb_lm_repeat_step_gemm(fsb_lm* h, int layer, int kind, int reps, void* stream) {
-    // Diagnostic: the SAME step GEMM of one slow layer `reps` times back to back: from the second launch on its weights
-    // come from L2 where they fit (126 MB), which separates "bound by HBM" from "bound by the SM-side pipeline".
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    Stack& s = h->slow;
-    FSB_CHECK(layer >= 0 && layer < s.nl && kind >= 0 && kind < 4, "repeat_step_gemm: layer %d kind %d", layer, kind);
-    const StepGemmPlan* plans[4] = {&s.dec[layer].qkv, &s.dec[layer].wo, &s.dec[layer].w13, &s.dec[layer].w2};
-    StepGemmPlan q = *plans[kind];
-    q.p.rows = h->cfg.max_batch;
-    for (int i = 0; i < reps; ++i) FSB_TRY(step_gemm_launch(q, st));
-    return 0;
-}
-
-int fsb_lm_trace_step_gemms(fsb_lm* h, unsigned long long* d_trace, int max_launches, int* grid_out, void* stream) {
-    // Diagnostic: the four step GEMMs of the first slow layers, each CTA recording globaltimer stamps
-    // (lm_gemm.cuh StepGemmParams::trace): shows where a launch spends its time and which CTAs share an SM.
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    Stack& s = h->slow;
-    int id = 0, grid = 0;
-    for (int l = 0; l < s.nl && id + 4 <= max_launches; ++l) {
-        const StepGemmPlan* plans[4] = {&s.dec[l].qkv, &s.dec[l].wo, &s.dec[l].w13, &s.dec[l].w2};
-        for (int k = 0; k < 4; ++k) {
-            StepGemmPlan q = *plans[k];
-            grid = std::max(grid, static_cast<int>(q.grid.x));
-            q.p.rows = h->cfg.max_batch;
-            q.p.trace = d_trace + static_cast<size_t>(id++) * 8 * 512;  // 512 CTA records per launch
-            FSB_CHECK(q.grid.x <= 512, "trace: grid too large");
-            FSB_TRY(step_gemm_launch(q, st));
-        }
-    }
-    if (grid_out) *grid_out = grid;
-    return id;
 }
 
 int fsb_lm_set_context_bound(fsb_lm* h, int max_positions) {

@@ -6,8 +6,6 @@
 #include "lm_gemm.cuh"
 #include "wgmma.cuh"
 
-#include <stdlib.h>
-
 #include <algorithm>
 #include <vector>
 
@@ -112,7 +110,7 @@ __device__ __forceinline__ void pro_swiglu(const StepGemmParams& p, int tile, in
     const bool hi = (lane & 16) != 0;  // lanes 16..31 hold the w3 ("up") rows of the features lanes 0..15 gate
     const int f = tile * 64 + quad * 16 + (lane & 15);
     float acc[R];
-    prev_sums<R, (R == 32 ? 2 : (R == 16 ? 3 : 32 / R))>(p, tile, tid, j0, acc);
+    prev_sums<R, 32 / R>(p, tile, tid, j0, acc);
 #pragma unroll
     for (int r = 0; r < R; ++r) {
         const float up = __shfl_xor_sync(0xffffffffu, acc[r], 16);
@@ -124,31 +122,23 @@ __device__ __forceinline__ void pro_swiglu(const StepGemmParams& p, int tile, in
     }
 }
 
-template <int PRO, int R>
-__device__ __forceinline__ void pro_units(const StepGemmParams& p, int tid, float* red) {
-    const int rblocks = (p.rows + R - 1) / R;
-    const int units = p.prev.tiles * rblocks;
-    for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int tile = u % p.prev.tiles, j0 = (u / p.prev.tiles) * R;
-        if (PRO == PRO_RESID) pro_resid<R>(p, tile, tid, j0, red);
-        else pro_swiglu<R>(p, tile, tid, j0);
-    }
-}
+// Batch rows per finalize unit: one load round per unit (<= 16 partials for PRO_RESID, <= 4 for PRO_SWIGLU).
+template <int PRO>
+constexpr int kFinalizeRows = PRO == PRO_SWIGLU ? 8 : 2;
 
 // step_finalize: finishes the GEMM that produced the next GEMM's operand (one unit = R batch rows x one 128-feature
 // tile per CTA); launched between the two GEMMs, so the consumer GEMM finds its operand complete.
 template <int PRO>
 __global__ void __launch_bounds__(kEpiThreads) step_finalize_kernel(const __grid_constant__ StepGemmParams p) {
+    constexpr int R = kFinalizeRows<PRO>;
     __shared__ float red[4 * 32];
     pdl_launch_dependents();
     pdl_wait();
-    switch (p.prev_rb) {
-        case 1: pro_units<PRO, 1>(p, threadIdx.x, red); break;
-        case 2: pro_units<PRO, 2>(p, threadIdx.x, red); break;
-        case 4: pro_units<PRO, 4>(p, threadIdx.x, red); break;
-        case 8: pro_units<PRO, 8>(p, threadIdx.x, red); break;
-        case 16: pro_units<PRO, 16>(p, threadIdx.x, red); break;
-        default: pro_units<PRO, 32>(p, threadIdx.x, red); break;
+    const int units = p.prev.tiles * ((p.rows + R - 1) / R);
+    for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        const int tile = u % p.prev.tiles, j0 = (u / p.prev.tiles) * R;
+        if (PRO == PRO_RESID) pro_resid<R>(p, tile, threadIdx.x, j0, red);
+        else pro_swiglu<R>(p, tile, threadIdx.x, j0);
     }
 }
 
@@ -172,8 +162,6 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int item_begin = p.cta_items[blockIdx.x], item_end = p.cta_items[blockIdx.x + 1];
-    unsigned long long* trace = p.trace ? p.trace + static_cast<size_t>(blockIdx.x) * 8 : nullptr;
-    if (trace && threadIdx.x == 0) trace[0] = globaltimer_ns();
 
     if (warp == kProducerWarp && lane == 0) {
         tma_prefetch_desc(&tmA);
@@ -214,19 +202,8 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                         }
                     }
                 }
-                // ... optionally (FSB_L2_PREFETCH, default 0) the weight tiles after those are requested into L2
-                for (int q = 0; q < p.l2_prefetch && n < item_end; ++q) {
-                    tma_prefetch_l2_3d(&tmA, kb * kBlockK, w.x * kBlockM, 0);
-                    if (++kb >= w.z) {
-                        if (++n < item_end) {
-                            w = p.sched[n];
-                            kb = w.y;
-                        }
-                    }
-                }
             }
             pdl_wait();
-            if (trace) trace[1] = globaltimer_ns();
             int it = 0;
             for (int n = item_begin; n < item_end; ++n) {
                 const int4 w = p.sched[n];
@@ -275,7 +252,6 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 r_s[t] = rsqrtf(tot / static_cast<float>(p.K) + p.eps);
             }
             bar_sync(2, kLoaderThreads);
-            if (trace && t == 0) trace[6] = globaltimer_ns();
             // 32 rows x 8 sixteen-byte chunks per k-block; thread t owns chunk (t & 7) of rows (t >> 3) + 16e
             constexpr int kCells = 256 / kLoaderThreads;
             const int c = t & 7, rb = t >> 3;
@@ -317,7 +293,6 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     fence_proxy_async();  // generic-proxy stores -> visible to the tensor core's async proxy
                     __syncwarp();
                     if (lane == 0) mbar_arrive(full0 + 8u * s);
-                    if (trace && t == 0 && it == 0) trace[7] = globaltimer_ns();
                 }
             }
         }
@@ -354,7 +329,6 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             wgmma_wait<0>();
             __syncwarp();
             if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
-            if (trace && threadIdx.x == 0 && n == item_begin) trace[4] = globaltimer_ns();
             // accumulator element (feature i, batch row j) -> ws[slot][tile][j][i]
             float* dst = p.ws + ((static_cast<size_t>(slot) * p.tiles + tile) * 32) * 128;
             const int i0 = warp * 16 + (lane >> 2);
@@ -370,10 +344,6 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     }
                 }
         }
-    }
-    if (trace) {
-        __syncthreads();
-        if (threadIdx.x == 0) trace[5] = globaltimer_ns();
     }
 }
 
@@ -471,11 +441,6 @@ int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K,
     p.a_hint = kEvictFirst;  // weights are streamed once per step (>> L2)
     p.b_hint = kEvictLast;   // the activation tile is re-read by every CTA
     p.ws = ws;
-    p.prev_rb = 32;
-    {
-        const char* e = getenv("FSB_L2_PREFETCH");
-        p.l2_prefetch = e ? atoi(e) : 0;  // k-blocks per CTA (16 KB each)
-    }
     plan->grid = dim3(static_cast<unsigned>(num_ctas), 1, 1);
     plan->smem = smem_of(stages);
     plan->pro = PRO_NONE;
@@ -512,16 +477,14 @@ int step_finalize_launch(const StepGemmPlan& consumer, cudaStream_t st) {
     // `consumer`'s finalize fields (prev, bias / resid / x_out / ssq_out or h / I, rows) describe the work; one unit per CTA
     const int pro = consumer.pro;
     if (pro == PRO_NONE) return 0;
-    StepGemmParams p = consumer.p;
-    // one load round per unit (<= 4 / <= 16 partials), every unit on its own CTA
-    static const int rb_swiglu = [] { const char* e = getenv("FSB_SWIGLU_RB"); return e ? atoi(e) : 8; }();
-    static const int rb_resid = [] { const char* e = getenv("FSB_RESID_RB"); return e ? atoi(e) : 2; }();
-    const int rb = pro == PRO_SWIGLU ? rb_swiglu : rb_resid;
-    FSB_CHECK(rb >= 1 && rb <= 32 && (rb & (rb - 1)) == 0, "finalize: row block %d is not a power of two <= 32", rb);
-    p.prev_rb = rb;
-    const int units = p.prev.tiles * cdiv(p.rows, rb);
-    if (pro == PRO_RESID) FSB_LAUNCH(step_finalize_kernel<PRO_RESID>, dim3(units), dim3(kEpiThreads), 0, st, p);
-    else FSB_LAUNCH(step_finalize_kernel<PRO_SWIGLU>, dim3(units), dim3(kEpiThreads), 0, st, p);
+    const StepGemmParams& p = consumer.p;
+    if (pro == PRO_RESID) {
+        const dim3 units(p.prev.tiles * cdiv(p.rows, kFinalizeRows<PRO_RESID>));
+        FSB_LAUNCH(step_finalize_kernel<PRO_RESID>, units, dim3(kEpiThreads), 0, st, p);
+    } else {
+        const dim3 units(p.prev.tiles * cdiv(p.rows, kFinalizeRows<PRO_SWIGLU>));
+        FSB_LAUNCH(step_finalize_kernel<PRO_SWIGLU>, units, dim3(kEpiThreads), 0, st, p);
+    }
     return 0;
 }
 

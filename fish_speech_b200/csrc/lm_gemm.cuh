@@ -102,12 +102,10 @@ struct StepGemmParams {
     int tiles, stages;
     int n_out, K;           // output features, reduction length
     int rows;               // live batch rows (<= 32)
-    int l2_prefetch;        // weight k-blocks per CTA prefetched into L2 behind the ring, before the operand exists
     unsigned long long a_hint, b_hint;
     float* ws;              // out: [slot][tile][32 rows][128 features] fp32 partials
     // ---- step_finalize of the GEMM that produces this one's operand (pro != PRO_NONE) ----
     StepPartials prev;
-    int prev_rb;                  // batch rows per finalize unit (power of two)
     const __nv_bfloat16* bias;    // PRO_RESID: [prev.n_out] or null
     const __nv_bfloat16* resid;   // PRO_RESID: [32][prev.n_out]; may alias x_out; null => no add
     __nv_bfloat16* x_out;         // PRO_RESID: [32][prev.n_out] new residual stream
@@ -119,9 +117,6 @@ struct StepGemmParams {
     const __nv_bfloat16* norm_w;  // [K]
     int x_nt;                     // tiles per row in x_ssq
     float eps;
-    // diagnostics: optional [grid][8] globaltimer stamps {start, previous grid complete, -, -, first accumulator done,
-    // end, normalisers ready, first tile normalised}
-    unsigned long long* trace;
 };
 
 struct StepGemmPlan {

@@ -357,7 +357,7 @@ constexpr int kAttnPrefetchPos = 2048;  // positions of K/V history the decode a
 template <int DH, int G>
 __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, const __nv_bfloat16* kc,
                                        const __nv_bfloat16* vc, int L, int lcap, float scale, int bf16_math,
-                                       __nv_bfloat16* out, unsigned long long* trace = nullptr) {
+                                       __nv_bfloat16* out) {
     static_assert(G <= kAttnWarps, "one warp per query head in the softmax");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     constexpr int LPR = DH / 8;    // lanes per cache row (16-byte loads)
@@ -405,7 +405,6 @@ __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, c
     float m = -INFINITY, z = 0.f;  // of head `warp` (warps < G)
     if (one) {
         scores(0, L);
-        if (trace && threadIdx.x == 0) trace[4] = globaltimer_ns();
         if (warp < G) {
             float* s = sc + warp * lcap;
             for (int p = lane; p < L; p += 32) m = fmaxf(m, s[p]);
@@ -422,7 +421,6 @@ __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, c
             }
         }
         __syncthreads();
-        if (trace && threadIdx.x == 0) trace[5] = globaltimer_ns();
     } else {
         for (int c0 = 0; c0 < L; c0 += lcap) {
             const int n = min(lcap, L - c0);
@@ -498,14 +496,12 @@ __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, c
 #pragma unroll
         for (int e = 0; e < DPL; ++e) red[(warp * G + gg) * DH + lane * DPL + e] = acc[gg][e];
     __syncthreads();
-    if (trace && threadIdx.x == 0) trace[6] = globaltimer_ns();
     for (int e = threadIdx.x; e < G * DH; e += kAttnThreads) {
         float s = 0.f;
 #pragma unroll
         for (int w = 0; w < kAttnWarps; ++w) s += red[w * G * DH + e];
         out[e] = f2bf(s);
     }
-    if (trace && threadIdx.x == 0) trace[7] = globaltimer_ns();
 }
 
 
@@ -546,8 +542,6 @@ __global__ void __launch_bounds__(kAttnThreads) attn_kernel(AttnArgs a, float sc
 // ------------------------------------------------------------------------------------------------
 template <int DH, int G>
 __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArgs a, float scale, int lcap) {
-    unsigned long long* trace = (a.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0) ? a.trace : nullptr;
-    if (trace && threadIdx.x == 0) trace[0] = globaltimer_ns();
     pdl_launch_dependents();
     const int row = blockIdx.y, g = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -583,7 +577,6 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
         normw_r[r] = (nw != nullptr && hh < NH) ? bf2f(nw[d]) : 0.f;
     }
     pdl_wait();
-    if (trace && threadIdx.x == 0) trace[1] = globaltimer_ns();
     extern __shared__ float sm[];
     float* qs = sm;                      // [G][DH]
     float* sc = qs + G * DH;             // [G][lcap]
@@ -613,7 +606,6 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
     const int wpos = min(rpos, a.S - 1);
     // (cos, sin) of this lane's rotary pair at the row's position: the same for q and k
     const uint32_t cs = *reinterpret_cast<const uint32_t*>(a.freqs + (static_cast<size_t>(wpos) * (DH / 2) + (d >> 1)) * 2);
-    if (trace && threadIdx.x == 0) trace[2] = globaltimer_ns() + (vsum[0] == 12345.f ? 1 : 0);  // after the sums arrive
     // bias, the GEMM output's bf16 rounding, and per-head nn.RMSNorm (fp32 math, weight multiply included, ONE
     // rounding): the sums of squares of all rounds cross the warps behind one barrier
     const bool any_norm = a.q_norm != nullptr || a.k_norm != nullptr;
@@ -665,7 +657,6 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
     }
     if (a.kv_only) return;
     __syncthreads();  // q in shared memory, this row's new K/V visible to the whole CTA
-    if (trace && threadIdx.x == 0) trace[3] = globaltimer_ns();
 
     const int pos = wpos;
     const int L = pos + 1;
@@ -674,7 +665,7 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
     const __nv_bfloat16* vc = a.vcache + cache_base;
 
     attend<DH, G>(qs, sc, red, kc, vc, L, lcap, scale, a.bf16_math,
-                  a.out + (static_cast<size_t>(row) * a.H + g * G) * DH, trace);
+                  a.out + (static_cast<size_t>(row) * a.H + g * G) * DH);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1097,8 +1088,7 @@ int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st) {
 int launch_attn(const AttnArgs& a, cudaStream_t st) {
     if (a.rows <= 0) return 0;
     // one kernel whatever the number of rows: a sequence must get the same bits alone, in a batch or in pieces
-    static const bool tile_on = [] { const char* e = getenv("FSB_ATTN_TILE"); return !(e && e[0] == '0'); }();
-    if (tile_on && !g_attn_per_row && attn_tile_supported(a)) return launch_attn_tile(a, st);
+    if (!g_attn_per_row && attn_tile_supported(a)) return launch_attn_tile(a, st);
     const int G = a.H / a.Hkv;
     FSB_CHECK(a.H % a.Hkv == 0, "attention: H %% Hkv != 0");
 #define FSB_ATTN_CASE(DH_, G_) \

@@ -95,7 +95,7 @@ struct AttnArgs {
 };
 int launch_attn(const AttnArgs& a, cudaStream_t st);
 // csrc/attn_tile.cu: 64 rows of one head per CTA, K/V tiles staged once, mma.sync tensor cores, online softmax; what
-// launch_attn uses for >= 64 rows (prefill, codec transformer).  FSB_ATTN_TILE=0 keeps the per-row kernel.
+// launch_attn uses for >= 64 rows (prefill, codec transformer).
 bool attn_tile_supported(const AttnArgs& a);
 int launch_attn_tile(const AttnArgs& a, cudaStream_t st);
 int attn_init();  // set kernel attributes (idempotent)
@@ -123,9 +123,6 @@ struct AttnDecodeArgs {
     int bf16_math;  // the fast stack's all-bf16 attention (llama.py:948-976)
     int kv_only;
     float eps;
-    // diagnostics: optional 8 globaltimer stamps of CTA (0, 0): {start, wait returned, partials summed, q/k/v finished,
-    // scores done, softmax done, values summed, end}
-    unsigned long long* trace;
 };
 int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st);
 

@@ -341,10 +341,6 @@ class LmEngine:
         return reused
 
     def decode(self, batch: int, nframes: int, sp: Optional[_lib.Sampling], use_graph: bool = True) -> None:
-        import os
-
-        if os.environ.get("FSB_NO_GRAPH") == "1":  # diagnostic: eager launches instead of graph replays
-            use_graph = False
         if not self.slot_control and self._ctx_bound - 1 + nframes > self.kv_len:
             raise ValueError(f"decode: {nframes} more frames from position {self._ctx_bound - 1} run past the KV "
                              f"cache ({self.kv_len} positions)")

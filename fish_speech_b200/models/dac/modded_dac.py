@@ -19,7 +19,6 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
 import threading
 from dataclasses import dataclass, field
 from typing import Iterator, Optional
@@ -117,9 +116,8 @@ class DAC:
         self._bufs: dict = {}
         self._graphs: dict = {}   # (B, S, T) -> (CUDAGraph, static index buffer, static waveform) of from_indices
         self._graph_seen: dict = {}
-        self._use_graphs = os.environ.get("FSB_CODEC_GRAPH", "1") != "0"
-        # decoder ResidualUnits as one kernel each (csrc/codec_resunit.cu); 0 = two conv GEMM launches per unit
-        self._fused_units = os.environ.get("FSB_FUSED_RESUNIT", "1") != "0"
+        # decoder ResidualUnits as one kernel each (csrc/codec_resunit.cu); False = two conv GEMM launches per unit
+        self._fused_units = True
         self._lock = threading.RLock()
         self._rope: dict = {}
         self._sd = {k: v.detach().float() for k, v in state_dict.items()}  # folded on the device they live on
@@ -445,8 +443,8 @@ class DAC:
                 return g_wav.clone().view(B, 1, -1)
             seen = self._graph_seen.get(key, 0)
             self._graph_seen[key] = seen + 1
-            if not self._use_graphs or seen == 0 or len(self._graphs) >= 4:
-                # first sight of a shape (warms the plan cache and sizes the workspaces), or capture disabled / full
+            if seen == 0 or len(self._graphs) >= 4:
+                # first sight of a shape (warms the plan cache and sizes the workspaces), or the graph cache is full
                 idx = indices.to(device=self._device, dtype=torch.int32).contiguous()
                 wav = self._from_indices_body(idx, B, S, T)
                 self._idx_keepalive = idx

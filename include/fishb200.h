@@ -164,22 +164,6 @@ int fsb_lm_buffer(fsb_lm* h, const char* name, void** d_ptr, size_t* bytes);
 int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* launches_per_rep,
                        void* stream);
 
-/* Diagnostics: per-CTA globaltimer stamps of step GEMM launches, d_trace[launch][512][8] = {start, previous grid
- * complete (griddepcontrol.wait returned), -, -, first accumulator complete, end, normaliser warps ready,
- * first operand tile normalised} (0 = not recorded).
- * fsb_lm_trace_step_gemms: the step GEMMs of the first slow layers (qkv, wo, w1|w3, w2, ...) launched back to back;
- * returns the number of launches traced (0 = failure); overwrites the decode state like fsb_lm_bench_gemms.
- * fsb_lm_repeat_step_gemm: the SAME step GEMM of one slow layer `reps` times back to back (weights from L2 after the
- * first launch, where they fit); overwrites the decode state.
- * fsb_lm_trace_frame: ONE whole decode frame (eager launches, the kernels and launch attributes of the graph), every
- * step GEMM traced in launch order; advances the decode state by one frame; returns the launches traced or -1.
- * d_attn_trace (optional) [max_attn][8]: stamps of CTA (0, 0) of every decode attention launch = {start, wait returned,
- * qkv partials summed, q/k/v finished, scores, softmax, values summed, end}. */
-int fsb_lm_repeat_step_gemm(fsb_lm* h, int layer, int kind, int reps, void* stream); /* kind: 0 qkv, 1 wo, 2 w1|w3, 3 w2 */
-int fsb_lm_trace_frame(fsb_lm* h, int batch, const fsb_sampling* sampling, unsigned long long* d_trace,
-                       int max_launches, unsigned long long* d_attn_trace, int max_attn, void* stream);
-int fsb_lm_trace_step_gemms(fsb_lm* h, unsigned long long* d_trace, int max_launches, int* grid_out, void* stream);
-
 /* Test hook for bit-exact parity of the STOCHASTIC sampler with the reference's torch RNG stream
  * (inference.py:43-46 multinomial_sample_one_no_sync, :114-144 RAS): when d_u != NULL, slot 0 takes the uniforms
  * of draw d of frame f from d_u[(f * draws_per_frame + d) * ld + candidate] (f = frames produced since
@@ -259,9 +243,6 @@ int fsb_op_attn_score_chunk(int positions);
 /* fsb_window_attn normally runs the tiled tensor-core kernel (csrc/attn_tile.cu); on != 0 makes it run the per-row
  * kernel, whose attention core is the one of the decode step (what the chunking test above exercises). */
 int fsb_op_attn_per_row(int on);
-/* Diagnostics of fsb_res_unit: d_trace [64][6] globaltimer stamps of CTA 0's first tiles = {epilogue idle, conv7
- * accumulator ready, h written, conv1 accumulator ready, outputs staged, stores issued}; NULL switches it off. */
-int fsb_op_res_unit_trace(unsigned long long* d_trace);
 
 #ifdef __cplusplus
 }

@@ -27,7 +27,6 @@ def timed(fn, n=5):
     return e0.elapsed_time(e1) / n
 
 
-trace_lines = []
 print("| C | T/utt | dilation | conv7 ms | conv1 ms | two launches ms | fused ms | fused TFLOP/s | fused GB/s (3 N C x 2 B) |")
 print("|---|---|---|---|---|---|---|---|---|")
 for C, T in ((384, 65536), (192, 262144), (96, 524288)):
@@ -53,21 +52,8 @@ for C, T in ((384, 65536), (192, 262144), (96, 524288)):
                                                a1.data_ptr(), i1.data_ptr(), w1.data_ptr(), b1.data_ptr(), x.data_ptr(),
                                                y1.data_ptr(), an.data_ptr(), inn.data_ptr(), st()))
         t7, t1, tf = timed(c7), timed(c1), timed(fu)
-        if dil == 1:
-            trb = torch.zeros(64, 6, dtype=torch.int64, device=dev)
-            L.fsb_op_res_unit_trace(trb.data_ptr())
-            fu()
-            torch.cuda.synchronize()
-            L.fsb_op_res_unit_trace(None)
-            tt = trb.cpu().double()[8:40]
-            d = (tt[:, 1:] - tt[:, :-1]).mean(0) / 1e3
-            gap = ((tt[1:, 0] - tt[:-1, 5]).mean() / 1e3).item()
-            trace_lines.append(f"C={C}: per tile (CTA 0, tiles 8..39), us: wait conv7 {d[0]:.2f}, epilogue 1 {d[1]:.2f}, wait conv1 "
-                               f"{d[2]:.2f}, epilogue 2 {d[3]:.2f}, barrier + store issue {d[4]:.2f}, loop gap {gap:.2f}; tile "
-                               f"{((tt[-1, 0] - tt[0, 0]) / (len(tt) - 1) / 1e3).item():.2f}")
         flops = 2.0 * B * T * C * C * 8
         print(f"| {C} | {T} | {dil} | {t7:.2f} | {t1:.2f} | {t7 + t1:.2f} | {tf:.2f} | {flops / tf / 1e9:.0f} | "
               f"{4 * B * T * C * 2 / tf / 1e6:.0f} |")
     del x, a, h, y1
     torch.cuda.empty_cache()
-print("\n".join(trace_lines))

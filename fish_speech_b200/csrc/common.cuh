@@ -182,13 +182,10 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     const long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {
-        if (clock64() - t0 > 4000000000ll) {  // ~2 s at ~2 GHz
-            printf("fsb: mbarrier timeout block=(%d,%d,%d) thread=%d bar=%u parity=%u\n",
-                   blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, bar, parity);
-            __trap();
-        }
-    }
+    // ~2 s at ~2 GHz: a lost arrival or TMA completion traps instead of hanging. No printf here: a function call
+    // between wgmma issue and wgmma wait makes ptxas serialize every wgmma of the kernel (warning C7510).
+    while (!mbar_try_wait(bar, parity))
+        if (clock64() - t0 > 4000000000ll) __trap();
 }
 
 constexpr uint64_t kEvictNormal = 0x1000000000000000ull;

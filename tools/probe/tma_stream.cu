@@ -58,7 +58,7 @@ int main(int argc, char** argv) {
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     for (int tiled = 0; tiled < 2; ++tiled)
         for (int per_sm : {1, 2})
-            for (int stages : {3, 5, 6})
+            for (int stages : {3, 4, 5, 6})
                 for (int hintsel = 0; hintsel < 2; ++hintsel) {
                     if (per_sm == 2 && stages > 6) continue;
                     std::vector<CUtensorMap> tms(layers);

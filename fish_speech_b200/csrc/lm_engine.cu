@@ -208,12 +208,13 @@ SlotCtl slot_ctl(const fsb_lm* h) {
     return c;
 }
 
-// One step GEMM over `rows` batch rows: first finish the producer of its operand (residual add / SwiGLU), then the GEMM.
-int launch_step(const StepGemmPlan& plan, int rows, cudaStream_t st) {
+// One step GEMM over `rows` batch rows: first finish the producer of its operand (residual add / SwiGLU), then the GEMM
+// (only the finish when finalize_only).
+int launch_step(const StepGemmPlan& plan, int rows, cudaStream_t st, bool finalize_only = false) {
     StepGemmPlan q = plan;
     q.p.rows = rows;
     FSB_TRY(step_finalize_launch(q, st));
-    return step_gemm_launch(q, st);
+    return finalize_only ? 0 : step_gemm_launch(q, st);
 }
 
 // ---- decode: one transformer stack over the batch rows, five kernels per layer. `first_qkv`: the plan of layer 0's
@@ -525,14 +526,14 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     } while (0)
     TRYC(dalloc(h, &h->ws, h->ws_floats));
     TRYC(dalloc(h, &h->step_ws, h->step_ws_floats));
-    TRYC(dalloc(h, &s.xres, static_cast<size_t>(kDecRows) * s.D));
-    TRYC(dalloc(h, &s.ssq, static_cast<size_t>(kDecRows) * kSsqStride));
-    TRYC(dalloc(h, &f.xres, static_cast<size_t>(kDecRows) * f.D));
-    TRYC(dalloc(h, &f.ssq, static_cast<size_t>(kDecRows) * kSsqStride));
+    TRYC(dalloc(h, &s.xres, static_cast<size_t>(kDecRows) * s.D, "x_slow"));
+    TRYC(dalloc(h, &s.ssq, static_cast<size_t>(kDecRows) * kSsqStride, "ssq_slow"));
+    TRYC(dalloc(h, &f.xres, static_cast<size_t>(kDecRows) * f.D, "x_fast"));
+    TRYC(dalloc(h, &f.ssq, static_cast<size_t>(kDecRows) * kSsqStride, "ssq_fast"));
     TRYC(dalloc(h, &h->hid_d, static_cast<size_t>(kDecRows) * Dm));
     TRYC(dalloc(h, &h->q_d, static_cast<size_t>(kDecRows) * Qm));
-    TRYC(dalloc(h, &h->attn_d, static_cast<size_t>(kDecRows) * Qm));
-    TRYC(dalloc(h, &h->h_d, static_cast<size_t>(kDecRows) * Im));
+    TRYC(dalloc(h, &h->attn_d, static_cast<size_t>(kDecRows) * Qm, "attn"));
+    TRYC(dalloc(h, &h->h_d, static_cast<size_t>(kDecRows) * Im, "ffn_h"));
     TRYC(dalloc(h, &h->xres_p, static_cast<size_t>(R) * s.D));
     TRYC(dalloc(h, &h->xn_p, static_cast<size_t>(R) * s.D));
     TRYC(dalloc(h, &h->q_p, static_cast<size_t>(R) * s.H * s.Dh));
@@ -808,6 +809,21 @@ int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* l
     if (weight_bytes_per_rep) *weight_bytes_per_rep = bytes;
     if (launches_per_rep) *launches_per_rep = launches;
     return 0;
+}
+
+int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(h != nullptr, "test_layer_gemms: null handle");
+    Stack& s = fast ? h->fast : h->slow;
+    FSB_CHECK(layer >= 0 && layer < s.nl, "test_layer_gemms: layer=%d outside [0, %d)", layer, s.nl);
+    FSB_CHECK(rows >= 1 && rows <= h->cfg.max_batch, "test_layer_gemms: rows=%d outside [1, %d]", rows, h->cfg.max_batch);
+    FSB_CHECK(upto >= 1 && upto <= 3, "test_layer_gemms: upto=%d outside [1, 3]", upto);
+    StepLayer& P = s.dec[layer];
+    // the GEMMs in run_stack_decode's order, then the plan whose finalize finishes the last of them
+    const StepGemmPlan* next = layer + 1 < s.nl ? &s.dec[layer + 1].qkv : fast ? &h->fast_out_plan : &h->head_plan;
+    const StepGemmPlan* seq[4] = {&P.wo, &P.w13, &P.w2, next};
+    for (int k = 0; k < upto; ++k) FSB_TRY(launch_step(*seq[k], rows, st));
+    return launch_step(*seq[upto], rows, st, /*finalize_only=*/true);
 }
 
 int fsb_lm_copy_kv(fsb_lm* h, int src_slot, int dst_slot, int n_pos, void* stream) {

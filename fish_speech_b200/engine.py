@@ -182,6 +182,14 @@ class LmEngine:
             "slot_seed": ((self.max_batch,), "<i8"),
             "slow_logits": ((self.max_batch, self.head_rows), "<f4"),
             "fast_logits": ((c.num_codebooks, self.max_batch, c.codebook_size), "<f4"),
+            # decode state (include/fishb200.h fsb_lm_test_layer_gemms); "attn" / "ffn_h" are flat: the rows of the
+            # stack being run sit at stride H*Dh / I of that stack
+            "x_slow": ((MAX_DECODE_BATCH, c.dim), "<u2"),
+            "x_fast": ((MAX_DECODE_BATCH, c.fast_dim), "<u2"),
+            "ssq_slow": ((MAX_DECODE_BATCH, 32), "<f4"),
+            "ssq_fast": ((MAX_DECODE_BATCH, 32), "<f4"),
+            "attn": ((MAX_DECODE_BATCH * max(c.n_head * c.head_dim, c.fast_n_head * c.fast_head_dim),), "<u2"),
+            "ffn_h": ((MAX_DECODE_BATCH * max(c.intermediate_size, c.fast_intermediate_size),), "<u2"),
         }
         shape, ts = shapes[name]
         with torch.cuda.device(self.device):

@@ -155,7 +155,11 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
  *   "out_tokens" int32 [max_batch][C+1][max_frames], "n_out" int32 [max_batch], "pos" int32 [max_batch],
  *   "finished" int32 [max_batch], "cur_tok" int32 [max_batch][C+1], "ras_window" int32 [max_batch][10],
  *   the slot-control arrays listed at fsb_lm_set_slot_control,
- *   debug only: "slow_logits" f32 [max_batch][head_rows], "fast_logits" f32 [C][max_batch][codebook_size] */
+ *   debug only: "slow_logits" f32 [max_batch][head_rows], "fast_logits" f32 [C][max_batch][codebook_size];
+ *   the decode state (for fsb_lm_test_layer_gemms): "x_slow" / "x_fast" bf16 [32][dim] / [32][fast_dim] residual
+ *   streams, "ssq_slow" / "ssq_fast" f32 [32][32] their per-128-feature sums of squares, "attn" bf16 [32 * max H*Dh]
+ *   (the wo operand: rows of the stack being run at stride H*Dh), "ffn_h" bf16 [32 * max I] (the w2 operand:
+ *   rows at stride I of the stack being run) */
 int fsb_lm_buffer(fsb_lm* h, const char* name, void** d_ptr, size_t* bytes);
 
 /* Measurement hook for bench.py: launch every weight-streaming step GEMM of one decode frame `reps` times
@@ -232,10 +236,33 @@ int fsb_swiglu_f32(const float* d_y, int rows, int I, void* d_h, void* stream);
 /* ------------------------------------------------------------------------------------------------
  * Unit-test hooks (used by tests/ only)
  * ---------------------------------------------------------------------------------------------- */
-/* out[j][i] (fp32, ld = m) = sum_k A[i][k] * B[j][k]; A [m,k], B [n,k] bf16 row-major.
- * bn in {32,64,128,256}; streamk_ctas > 0 uses the decode-style stream-K schedule + partial sums. */
+/* out[j][i] (fp32, ld = m) = sum_k A[i][k] * B[j][k]; A [m,k], B [n,k] bf16 row-major, by the prefill / codec GEMM
+ * (csrc/gemm_tc.cu). bn in {32,64,128,256}; streamk_ctas > 0 splits the k-blocks over that many CTAs with
+ * gemm_plan_streamk and adds the partials in a separate kernel. This is not the decode step GEMM: that one is
+ * fsb_op_step_gemm below. */
 int fsb_op_gemm(const void* d_a, const void* d_b, float* d_out, int m, int n, int k, int bn,
                 int streamk_ctas, void* stream);
+
+/* One decode step GEMM (csrc/lm_gemm.cu) on its own: out[j][i] (fp32, [rows][n_out]) = sum_k W[i][k] * X'[j][k],
+ * summed from the stream-K partials in slot order by step_partial_sums, the consumers' own helper (an element where
+ * step_partial_sum disagrees with it in any bit is returned as NaN). W bf16 [n_out][K]; X bf16 [32][K], all 32 rows
+ * readable; X' = X as given, or, when d_norm_w != NULL, X normalised on load with d_x_ssq (f32 [32][32]: per row, the
+ * sums of squares of its 128-feature tiles) and eps. rows in [1, 32]; K a multiple of 8 (<= 4096 with the norm).
+ * num_ctas / stages are requests that step_plan_init may clamp; info (host, 5 ints, may be NULL) = CTAs, stages,
+ * max partial slots of a tile, max (tile, k-block) units of a CTA, max items (tile ranges) of a CTA of the plan
+ * that ran. Synchronises `stream`. */
+int fsb_op_step_gemm(const void* d_w, int n_out, int K, const void* d_x, int rows, const void* d_norm_w,
+                     const float* d_x_ssq, float eps, int num_ctas, int stages, float* d_out, int* info, void* stream);
+
+/* Runs the step GEMMs of decode layer `layer` of the slow (fast = 0) or fast (fast = 1) stack for `rows` batch rows
+ * exactly as fsb_lm_decode does (the handle's own plans, launch order and partial workspace), without attention:
+ *   upto = 1: wo GEMM + its residual-add finalize (x += wo(attn) + bo, and the sums of squares of x)
+ *   upto = 2: + w1|w3 GEMM (normalised on load) + SwiGLU finalize (h)
+ *   upto = 3: + w2 GEMM + the residual-add finalize run in front of the next consumer (next layer's qkv GEMM; the
+ *             head / fast output GEMM after the last layer)
+ * Inputs and outputs are the fsb_lm_buffer arrays "x_slow" / "x_fast", "ssq_slow" / "ssq_fast", "attn" and "ffn_h".
+ * rows in [1, max_batch]. */
+int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, void* stream);
 
 /* Attention keeps one fp32 score per position and head in shared memory; contexts longer than the buffer are walked
  * in chunks, bit-identically (csrc/lm_kernels.cu attend()).  positions > 0 forces a smaller chunk; 0 = automatic. */

@@ -1,4 +1,7 @@
-"""tcgen05/TMA GEMM (csrc/gemm_tc.cu) against an fp32 matmul of the same bf16 operands."""
+"""The prefill / codec GEMM (csrc/gemm_tc.cu: TMA + wgmma) against an fp32 matmul of the same bf16 operands.
+
+Its stream-K mode (gemm_plan_streamk) is not the decode step GEMM: that one is csrc/lm_gemm.cu, tested in
+test_step_gemm_gpu.py."""
 import pytest
 import torch
 
@@ -44,11 +47,13 @@ def test_gemm_direct(m, n, k, bn):
     (128, 32, 256, 1),
     (128, 32, 256, 3),      # split one tile over 3 CTAs
     (640, 32, 2560, 148),   # many segments, ragged ranges
-    (6144, 32, 2560, 148),  # wqkv shape
-    (2560, 8, 9728, 148),   # w2 shape, small batch
-    (4097, 5, 2560, 148),   # restricted LM head
+    (6144, 32, 2560, 148),  # large m, 48 tiles over 148 CTAs
+    (2560, 8, 9728, 148),   # long k, few columns
+    (4097, 5, 2560, 148),   # ragged last row tile (m % 128 == 1)
 ])
 def test_gemm_streamk(m, n, k, ctas):
+    """gemm_tc_kernel's own stream-K branch (gemm_plan_streamk), which only this hook uses; the shapes borrow S2-Pro
+    sizes but do not run the decode step GEMM."""
     _run(m, n, k, 32, ctas)
 
 

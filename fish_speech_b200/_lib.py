@@ -82,6 +82,7 @@ def lib() -> C.CDLL:
     L.fsb_lm_set_sampler_noise.argtypes = [vp, vp, i32, i32]
     L.fsb_lm_copy_kv.argtypes = [vp, i32, i32, i32, vp]
     L.fsb_lm_bench_gemms.argtypes = [vp, i32, C.POINTER(C.c_double), C.POINTER(i32), vp]
+    L.fsb_lm_bench_step_kind.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_double), C.POINTER(i32), vp]
     f32p, i32p, ll = C.c_void_p, C.POINTER(C.c_int), C.c_longlong
     L.fsb_conv_gemm.argtypes = [vp, i32, i32, i32, i32, ll, vp, i32, i32, i32, i32p, i32, vp, vp, vp, i32, vp, vp, vp,
                                 vp, i32, vp]

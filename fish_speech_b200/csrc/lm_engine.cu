@@ -209,11 +209,11 @@ SlotCtl slot_ctl(const fsb_lm* h) {
 }
 
 // One step GEMM over `rows` batch rows: first finish the producer of its operand (residual add / SwiGLU), then the GEMM
-// (only the finish when finalize_only).
-int launch_step(const StepGemmPlan& plan, int rows, cudaStream_t st, bool finalize_only = false) {
+// (only the finish when finalize_only; only the GEMM when !finalize).
+int launch_step(const StepGemmPlan& plan, int rows, cudaStream_t st, bool finalize_only = false, bool finalize = true) {
     StepGemmPlan q = plan;
     q.p.rows = rows;
-    FSB_TRY(step_finalize_launch(q, st));
+    if (finalize) FSB_TRY(step_finalize_launch(q, st));
     return finalize_only ? 0 : step_gemm_launch(q, st);
 }
 
@@ -808,6 +808,28 @@ int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* l
     }
     if (weight_bytes_per_rep) *weight_bytes_per_rep = bytes;
     if (launches_per_rep) *launches_per_rep = launches;
+    return 0;
+}
+
+int fsb_lm_bench_step_kind(fsb_lm* h, int kind, int reps, int finalize, double* weight_bytes_per_rep,
+                           int* launches_per_rep, void* stream) {
+    // The slow stack's step GEMMs of one kind back to back: per kind, the time of a launch against its weight bytes,
+    // with and without the finalize kernel in front of it (tools/step_gemm_boundaries.py). Overwrites the decode state.
+    FSB_CHECK(h != nullptr, "bench_step_kind: null handle");
+    FSB_CHECK(kind >= 0 && kind <= 3, "bench_step_kind: kind=%d outside [0, 3]", kind);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int rows = h->cfg.max_batch;
+    double bytes = 0;
+    for (int r = 0; r < reps; ++r) {
+        bytes = 0;
+        for (StepLayer& P : h->slow.dec) {
+            const StepGemmPlan* k[4] = {&P.qkv, &P.wo, &P.w13, &P.w2};
+            bytes += k[kind]->weight_bytes;
+            FSB_TRY(launch_step(*k[kind], rows, st, false, finalize != 0));
+        }
+    }
+    if (weight_bytes_per_rep) *weight_bytes_per_rep = bytes;
+    if (launches_per_rep) *launches_per_rep = h->slow.nl;
     return 0;
 }
 

@@ -122,9 +122,11 @@ __device__ __forceinline__ void pro_swiglu(const StepGemmParams& p, int tile, in
     }
 }
 
-// Batch rows per finalize unit: one load round per unit (<= 16 partials for PRO_RESID, <= 4 for PRO_SWIGLU).
+// Batch rows per finalize unit; a load round fetches 32 / R partial slots. PRO_RESID: 4 rows (two rounds for the ~14
+// slots of wo / w2 at the engine's schedules) measured faster than 2 or 1 on an H100 SXM. PRO_SWIGLU: 8 rows, one
+// round for the <= 4 slots of w1|w3. The sums are added in slot order whatever R is.
 template <int PRO>
-constexpr int kFinalizeRows = PRO == PRO_SWIGLU ? 8 : 2;
+constexpr int kFinalizeRows = PRO == PRO_SWIGLU ? 8 : 4;
 
 // step_finalize: finishes the GEMM that produced the next GEMM's operand (one unit = R batch rows x one 128-feature
 // tile per CTA); launched between the two GEMMs, so the consumer GEMM finds its operand complete.
@@ -320,15 +322,12 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     wgmma_bf16<kBN>(d1, a1 + 2u * k, bd + 2u * k, 1);
                 }
                 wgmma_commit();
-                wgmma_wait<1>();  // the previous k-block's MMAs have retired: release its ring slot
-                if (kb > w.y) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
-                }
+                // release the slot as soon as its own MMAs retire: the producer refills it while the next k-block
+                // is multiplied, so the whole ring depth stays in flight
+                wgmma_wait<0>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty0 + 8u * s);
             }
-            wgmma_wait<0>();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(empty0 + 8u * ((it - 1) % stages));
             // accumulator element (feature i, batch row j) -> ws[slot][tile][j][i]
             float* dst = p.ws + ((static_cast<size_t>(slot) * p.tiles + tile) * 32) * 128;
             const int i0 = warp * 16 + (lane >> 2);

@@ -168,6 +168,13 @@ int fsb_lm_buffer(fsb_lm* h, const char* name, void** d_ptr, size_t* bytes);
 int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* launches_per_rep,
                        void* stream);
 
+/* Measurement hook for tools/step_gemm_boundaries.py: the slow stack's step GEMMs of ONE kind (0 = qkv, 1 = wo,
+ * 2 = w1|w3, 3 = w2), layers 0..n_layer-1, `reps` times back to back through the decode path's own plans, each with
+ * the finalize kernel in front of it (finalize != 0) or without. Returns the weight bytes and launches of one
+ * repetition. Overwrites the decode state, like fsb_lm_bench_gemms. */
+int fsb_lm_bench_step_kind(fsb_lm* h, int kind, int reps, int finalize, double* weight_bytes_per_rep,
+                           int* launches_per_rep, void* stream);
+
 /* Test hook for bit-exact parity of the STOCHASTIC sampler with the reference's torch RNG stream
  * (inference.py:43-46 multinomial_sample_one_no_sync, :114-144 RAS): when d_u != NULL, slot 0 takes the uniforms
  * of draw d of frame f from d_u[(f * draws_per_frame + d) * ld + candidate] (f = frames produced since

@@ -128,11 +128,14 @@ static __global__ void step_sum_kernel(StepPartials P, int rows, float* out) {
     }
 }
 
-int fsb_op_step_gemm(const void* d_w, int n_out, int K, const void* d_x, int rows, const void* d_norm_w,
-                     const float* d_x_ssq, float eps, int num_ctas, int stages, float* d_out, int* info, void* stream) {
+int fsb_op_step_gemm_tile(const void* d_w, int n_out, int K, const void* d_x, int row_tile, int rows,
+                          const void* d_norm_w, const float* d_x_ssq, float eps, int num_ctas, int stages, float* d_out,
+                          int* info, void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     FSB_CHECK(d_w && d_x && d_out, "step GEMM hook: null operand");
-    FSB_CHECK(rows >= 1 && rows <= kStepRows, "step GEMM hook: rows=%d outside [1, %d]", rows, kStepRows);
+    FSB_CHECK(row_tile == kStepRows || row_tile == kStepRowsMax, "step GEMM hook: row_tile=%d is not %d or %d",
+              row_tile, kStepRows, kStepRowsMax);
+    FSB_CHECK(rows >= 1 && rows <= row_tile, "step GEMM hook: rows=%d outside [1, %d]", rows, row_tile);
     FSB_CHECK(n_out >= 1 && K >= 1, "step GEMM hook: empty GEMM (n_out=%d, K=%d)", n_out, K);
     FSB_CHECK(num_ctas >= 1 && stages >= 2, "step GEMM hook: num_ctas=%d, stages=%d", num_ctas, stages);
     const bool norm = d_norm_w != nullptr;
@@ -141,11 +144,12 @@ int fsb_op_step_gemm(const void* d_w, int n_out, int K, const void* d_x, int row
     StepGemmPlan plan;
     // the workspace is sized from the plan's own slot count, so the bound check of step_plan_init is not needed here
     if (step_plan_init(&plan, reinterpret_cast<const __nv_bfloat16*>(d_w), n_out, K,
-                       reinterpret_cast<const __nv_bfloat16*>(d_x), norm, num_ctas, stages, nullptr, SIZE_MAX) != 0) {
+                       reinterpret_cast<const __nv_bfloat16*>(d_x), norm, row_tile, num_ctas, stages, nullptr,
+                       SIZE_MAX) != 0) {
         step_plan_free(&plan);
         return 1;
     }
-    const size_t ws_floats = static_cast<size_t>(plan.max_parts) * plan.p.tiles * 128 * kStepRows;
+    const size_t ws_floats = static_cast<size_t>(plan.max_parts) * plan.p.tiles * 128 * row_tile;
     float* ws = nullptr;
     cudaError_t e = cudaMalloc(&ws, ws_floats * sizeof(float));
     int rc = e == cudaSuccess ? 0 : 1;
@@ -209,6 +213,13 @@ int fsb_op_step_gemm(const void* d_w, int n_out, int K, const void* d_x, int row
     if (rc != 0) return rc;
     FSB_CUDA(e);
     return 0;
+}
+
+int fsb_op_step_gemm(const void* d_w, int n_out, int K, const void* d_x, int rows, const void* d_norm_w,
+                     const float* d_x_ssq, float eps, int num_ctas, int stages, float* d_out, int* info, void* stream) {
+    FSB_CHECK(rows >= 1 && rows <= kStepRows, "step GEMM hook: rows=%d outside [1, %d]", rows, kStepRows);
+    return fsb_op_step_gemm_tile(d_w, n_out, K, d_x, kStepRows, rows, d_norm_w, d_x_ssq, eps, num_ctas, stages, d_out,
+                                 info, stream);
 }
 
 }  // extern "C"

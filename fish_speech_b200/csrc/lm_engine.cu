@@ -6,9 +6,10 @@
 //                      w1|w3 matrix has its rows interleaved per 128-row tile (lm_gemm.cuh, w13_gate_row)
 //   slow KV cache      [n_layer][max_batch][Hkv][kv_len][Dh]   x2 (K, V)
 //   fast KV cache      [n_fast_layer][max_batch][fHkv][num_codebooks][fDh]  x2
-//   decode state       residual streams x_slow / x_fast [32][D] + their per-128-feature sums of squares
-//                      (fp32 [32][32]); q / attention / SwiGLU operands [32][*]; logits fp32 [32][n]
-//   step_ws            fp32 stream-K partials of the step GEMMs: [slot][tile][32 rows][128 features]
+//   decode state       residual streams x_slow / x_fast [RT][D] + their per-128-feature sums of squares
+//                      (fp32 [RT][32]); q / attention / SwiGLU operands [RT][*]; logits fp32 [max_batch][n]
+//   step_ws            fp32 stream-K partials of the step GEMMs: [slot][tile][RT rows][128 features]
+// RT = the decode row tile: 32 for max_batch <= 32 (the 32-row step GEMM), 64 above (the 64-row one).
 //   prefill workspaces [max_rows][*] operands + ws fp32 [max_rows][N]
 //
 // One decode frame (inference.py:96-181) = embed, 36 x {qkv GEMM (norm on load), attention (finishes qkv: bias /
@@ -33,7 +34,6 @@ using namespace fsb;
 namespace {
 
 typedef __nv_bfloat16 bf16;
-constexpr int kDecRows = kStepRows;  // decode GEMM N tile: up to 32 sequences per step
 constexpr int kStepStages = 4;       // ring depth the step GEMM plans start from (step_plan_init may shrink it)
 
 struct LayerW {
@@ -58,8 +58,8 @@ struct Stack {
     bf16 *kcache = nullptr, *vcache = nullptr;
     const bf16* freqs = nullptr;
     size_t cache_layer_stride = 0;
-    bf16* xres = nullptr;  // decode residual stream [32][D]
-    float* ssq = nullptr;  // its per-tile sums of squares [32][kSsqStride]
+    bf16* xres = nullptr;  // decode residual stream [RT][D]
+    float* ssq = nullptr;  // its per-tile sums of squares [RT][kSsqStride]
 };
 
 }  // namespace
@@ -77,6 +77,7 @@ struct fsb_lm {
     fsb_lm_config cfg;
     int num_sms = 0;
     int step_ctas = 0;
+    int rt = kStepRows;  // decode row tile: 32 or 64 rows (kStepRowsMax) per step GEMM
     Stack slow, fast;
     const bf16 *emb = nullptr, *cb_emb = nullptr, *norm_w = nullptr, *head_w = nullptr;
     const bf16 *fast_emb = nullptr, *fast_norm_w = nullptr, *fast_out_w = nullptr;
@@ -176,7 +177,8 @@ int make_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, int 
                    const Stack* norm_of = nullptr) {
     const bool norm = act == nullptr;
     if (norm) act = norm_of->xres;
-    return step_plan_init(plan, w, n_out, K, act, norm, h->step_ctas, kStepStages, h->step_ws, h->step_ws_floats);
+    return step_plan_init(plan, w, n_out, K, act, norm, h->rt, h->step_ctas, kStepStages, h->step_ws,
+                          h->step_ws_floats);
 }
 
 void bind_norm_on_load(StepGemmPlan* plan, const Stack& s, const bf16* norm_w, float eps) {
@@ -389,7 +391,7 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
             er.rows = rows; er.D = f.D; er.eps = c.norm_eps;
             FSB_TRY(launch_rows(er, st));
         }
-        FSB_TRY(run_stack_decode(h, f, rows, slots, h->fpos + p * kDecRows, p == 0, st,
+        FSB_TRY(run_stack_decode(h, f, rows, slots, h->fpos + p * h->rt, p == 0, st,
                                  (p == 0 && h->has_proj) ? &h->fast_qkv0_proj : nullptr));
         if (p == 0) continue;
         FSB_TRY(launch_step(h->fast_out_plan, rows, st));
@@ -434,9 +436,9 @@ int decode_one_frame(fsb_lm* h, int batch, const fsb_sampling& sp, cudaStream_t 
     return run_frame_tail(h, batch, nullptr, true, nullptr, nullptr, sp, st);
 }
 
-size_t step_ws_bound(int n_out, int ctas) {
+size_t step_ws_bound(int n_out, int ctas, int rt) {
     const int tiles = cdiv(n_out, 128);
-    return static_cast<size_t>(tiles) * (cdiv(ctas, tiles) + 2) * 128 * 32;
+    return static_cast<size_t>(tiles) * (cdiv(ctas, tiles) + 2) * 128 * rt;
 }
 
 }  // namespace
@@ -445,7 +447,7 @@ extern "C" {
 
 int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** out) {
     FSB_CHECK(cfg && w && out, "fsb_lm_create: null argument");
-    FSB_CHECK(cfg->max_batch >= 1 && cfg->max_batch <= kDecRows, "max_batch must be in [1,32]");
+    FSB_CHECK(cfg->max_batch >= 1 && cfg->max_batch <= kStepRowsMax, "max_batch must be in [1,%d]", kStepRowsMax);
     FSB_CHECK(cfg->dim % 8 == 0 && cfg->fast_dim % 8 == 0 && cfg->intermediate % 16 == 0 &&
                   cfg->fast_intermediate % 16 == 0,
               "dims must be multiples of 8, intermediate sizes of 16 (TMA 16-byte strides, SwiGLU interleave)");
@@ -473,6 +475,9 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
         return 1;
     }
     h->step_ctas = h->num_sms * 2;  // two step-GEMM CTAs per SM
+    // engines of up to 32 slots keep the 32-row tile; more slots take the 64-row one (same bits per row)
+    h->rt = cfg->max_batch <= kStepRows ? kStepRows : kStepRowsMax;
+    const int RT = h->rt;
 
     auto B16 = [](const void* p) { return reinterpret_cast<const bf16*>(p); };
     h->emb = B16(w->d_embeddings);
@@ -516,7 +521,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     h->ws_floats = static_cast<size_t>(R) * std::max({Nqkv_s, s.n13, s.D});
     h->step_ws_floats = 0;
     for (int n : {Nqkv_s, Nqkv_f, s.n13, f.n13, s.D, f.D, h->head_rows, cfg->codebook_size})
-        h->step_ws_floats = std::max(h->step_ws_floats, step_ws_bound(n, h->step_ctas));
+        h->step_ws_floats = std::max(h->step_ws_floats, step_ws_bound(n, h->step_ctas, RT));
 #define TRYC(x)                  \
     do {                         \
         if ((x) != 0) {          \
@@ -526,14 +531,14 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     } while (0)
     TRYC(dalloc(h, &h->ws, h->ws_floats));
     TRYC(dalloc(h, &h->step_ws, h->step_ws_floats));
-    TRYC(dalloc(h, &s.xres, static_cast<size_t>(kDecRows) * s.D, "x_slow"));
-    TRYC(dalloc(h, &s.ssq, static_cast<size_t>(kDecRows) * kSsqStride, "ssq_slow"));
-    TRYC(dalloc(h, &f.xres, static_cast<size_t>(kDecRows) * f.D, "x_fast"));
-    TRYC(dalloc(h, &f.ssq, static_cast<size_t>(kDecRows) * kSsqStride, "ssq_fast"));
-    TRYC(dalloc(h, &h->hid_d, static_cast<size_t>(kDecRows) * Dm));
-    TRYC(dalloc(h, &h->q_d, static_cast<size_t>(kDecRows) * Qm));
-    TRYC(dalloc(h, &h->attn_d, static_cast<size_t>(kDecRows) * Qm, "attn"));
-    TRYC(dalloc(h, &h->h_d, static_cast<size_t>(kDecRows) * Im, "ffn_h"));
+    TRYC(dalloc(h, &s.xres, static_cast<size_t>(RT) * s.D, "x_slow"));
+    TRYC(dalloc(h, &s.ssq, static_cast<size_t>(RT) * kSsqStride, "ssq_slow"));
+    TRYC(dalloc(h, &f.xres, static_cast<size_t>(RT) * f.D, "x_fast"));
+    TRYC(dalloc(h, &f.ssq, static_cast<size_t>(RT) * kSsqStride, "ssq_fast"));
+    TRYC(dalloc(h, &h->hid_d, static_cast<size_t>(RT) * Dm));
+    TRYC(dalloc(h, &h->q_d, static_cast<size_t>(RT) * Qm));
+    TRYC(dalloc(h, &h->attn_d, static_cast<size_t>(RT) * Qm, "attn"));
+    TRYC(dalloc(h, &h->h_d, static_cast<size_t>(RT) * Im, "ffn_h"));
     TRYC(dalloc(h, &h->xres_p, static_cast<size_t>(R) * s.D));
     TRYC(dalloc(h, &h->xn_p, static_cast<size_t>(R) * s.D));
     TRYC(dalloc(h, &h->q_p, static_cast<size_t>(R) * s.H * s.Dh));
@@ -548,7 +553,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &h->cur_tok, static_cast<size_t>(cfg->max_batch) * (C + 1), "cur_tok"));
     TRYC(dalloc(h, &h->out_tokens, static_cast<size_t>(cfg->max_batch) * (C + 1) * cfg->max_frames, "out_tokens"));
     TRYC(dalloc(h, &h->n_out, cfg->max_batch, "n_out"));
-    TRYC(dalloc(h, &h->pos, kDecRows, "pos"));
+    TRYC(dalloc(h, &h->pos, RT, "pos"));
     TRYC(dalloc(h, &h->finished, cfg->max_batch, "finished"));
     TRYC(dalloc(h, &h->ras_window, static_cast<size_t>(cfg->max_batch) * 10, "ras_window"));
     TRYC(dalloc(h, &h->slot_state, cfg->max_batch, "slot_state"));
@@ -557,18 +562,18 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &h->slot_top_p, cfg->max_batch, "slot_top_p"));
     TRYC(dalloc(h, &h->slot_top_k, cfg->max_batch, "slot_top_k"));
     TRYC(dalloc(h, &h->slot_seed, cfg->max_batch, "slot_seed"));
-    TRYC(dalloc(h, &h->iota, kDecRows));
-    TRYC(dalloc(h, &h->fpos, static_cast<size_t>(C) * kDecRows));
+    TRYC(dalloc(h, &h->iota, RT));
+    TRYC(dalloc(h, &h->fpos, static_cast<size_t>(C) * RT));
     TRYC(dalloc(h, &h->step, 1));
     if (cfg->debug) {
         TRYC(dalloc(h, &h->slow_logits, static_cast<size_t>(cfg->max_batch) * h->head_rows, "slow_logits"));
         TRYC(dalloc(h, &h->fast_logits, static_cast<size_t>(C) * cfg->max_batch * cfg->codebook_size, "fast_logits"));
     }
     {
-        std::vector<int> io(kDecRows), fp(static_cast<size_t>(C) * kDecRows);
-        for (int i = 0; i < kDecRows; ++i) io[i] = i;
+        std::vector<int> io(RT), fp(static_cast<size_t>(C) * RT);
+        for (int i = 0; i < RT; ++i) io[i] = i;
         for (int p = 0; p < C; ++p)
-            for (int i = 0; i < kDecRows; ++i) fp[p * kDecRows + i] = p;
+            for (int i = 0; i < RT; ++i) fp[p * RT + i] = p;
         if (cudaMemcpy(h->iota, io.data(), io.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
             cudaMemcpy(h->fpos, fp.data(), fp.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
             set_error("fsb_lm_create: state upload failed");
@@ -658,7 +663,7 @@ int fsb_lm_reset(fsb_lm* h, void* stream) {
     FSB_CUDA(cudaMemsetAsync(h->finished, 0, c.max_batch * 4, st));
     FSB_CUDA(cudaMemsetAsync(h->slot_state, 0, c.max_batch * 4, st));
     FSB_CUDA(cudaMemsetAsync(h->ras_window, 0, static_cast<size_t>(c.max_batch) * 10 * 4, st));
-    FSB_CUDA(cudaMemsetAsync(h->pos, 0, kDecRows * 4, st));
+    FSB_CUDA(cudaMemsetAsync(h->pos, 0, h->rt * 4, st));
     FSB_CUDA(cudaMemsetAsync(h->step, 0, 8, st));
     return 0;
 }

@@ -13,15 +13,18 @@ namespace fsb {
 
 namespace {
 
-constexpr int kBN = kStepRows;
-constexpr int kBTileBytes = kBN * kBlockK * 2;  // 4 KB
-constexpr int kStageBytes = kATileBytes + kBTileBytes;
+// operand-X tile of RT rows (4 KB at 32 rows, 8 KB at 64) and one ring stage (weight tile + operand tile)
+template <int RT>
+constexpr int kBTileBytesOf = RT * kBlockK * 2;
+template <int RT>
+constexpr int kStageBytesOf = kATileBytes + kBTileBytesOf<RT>;
+constexpr int kHalfBTileBytes = kBTileBytesOf<kStepRows>;  // one 32-row half of the 64-row operand tile
 constexpr int kEpiThreads = 128;
 constexpr int kMmaThreads = 128;  // one warpgroup
 constexpr int kProducerWarp = kMmaThreads / 32;
 constexpr int kStepThreads = kMmaThreads + 32;  // + the TMA producer warp
 constexpr int kLoaderThreads = 128;  // four normaliser warps: two 16-byte cells per thread and k-block
-constexpr int kScratchBytes = 1024;  // r_s[32] | spare
+constexpr int kScratchBytes = 1024;  // r_s[RT] | spare
 
 __device__ __forceinline__ void bar_sync(int id, int n) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
@@ -47,15 +50,16 @@ __device__ __forceinline__ void rows_warp_sums(const float (&sq)[R], float* red,
     red[quad * 32 + lane] = keep;
 }
 
-// Slot-ordered sums of the previous GEMM's partials; up to 32 independent loads in flight per thread.
-template <int R, int UQ>  // UQ = partials fetched per round
+// Slot-ordered sums of the previous GEMM's partials; up to 32 independent loads in flight per thread. RT = the row
+// tile of the previous GEMM (p.prev.rt), a template parameter so that the 32-row finalize keeps its constant strides.
+template <int R, int UQ, int RT>  // UQ = partials fetched per round
 __device__ __forceinline__ void prev_sums(const StepGemmParams& p, int tile, int tid, int j0, float (&acc)[R]) {
     const int np = __ldg(p.prev.nparts + tile);
     const int maxp = p.prev.max_parts;  // loads are bounded by the launch constant, see step_partial_sum
 #pragma unroll
     for (int r = 0; r < R; ++r) acc[r] = 0.f;
-    const float* src = p.prev.ws + (static_cast<size_t>(tile) * 32 + j0) * 128 + tid;
-    const size_t sstride = static_cast<size_t>(p.prev.tiles) * 32 * 128;
+    const float* src = p.prev.ws + (static_cast<size_t>(tile) * RT + j0) * 128 + tid;
+    const size_t sstride = static_cast<size_t>(p.prev.tiles) * RT * 128;
     for (int q0 = 0; q0 < maxp; q0 += UQ) {
         float t[UQ][R];
 #pragma unroll
@@ -74,7 +78,7 @@ __device__ __forceinline__ void prev_sums(const StepGemmParams& p, int tile, int
 }
 
 // llama.py:842-845 / 944-946: y = Linear(...) (bf16), x = x + y (bf16); plus sum_i x^2 of this tile per row
-template <int R>
+template <int R, int RT>
 __device__ __forceinline__ void pro_resid(const StepGemmParams& p, int tile, int tid, int j0, float* red) {
     const int quad = tid >> 5, lane = tid & 31;
     const int i = tile * 128 + tid;
@@ -87,7 +91,7 @@ __device__ __forceinline__ void pro_resid(const StepGemmParams& p, int tile, int
         xin[r] = (p.resid != nullptr && ok && j0 + r < p.rows) ? bf2f(p.resid[static_cast<size_t>(j0 + r) * n + i]) : 0.f;
     const float b = (p.bias != nullptr && ok) ? bf2f(p.bias[i]) : 0.f;
     float acc[R], sq[R];
-    prev_sums<R, 32 / R>(p, tile, tid, j0, acc);
+    prev_sums<R, 32 / R, RT>(p, tile, tid, j0, acc);
 #pragma unroll
     for (int r = 0; r < R; ++r) {
         const float y = p.bias != nullptr ? rbf(acc[r] + b) : rbf(acc[r]);
@@ -104,13 +108,13 @@ __device__ __forceinline__ void pro_resid(const StepGemmParams& p, int tile, int
 }
 
 // llama.py:979-987: h = silu(w1 x) * w3 x, every intermediate a bf16 tensor
-template <int R>
+template <int R, int RT>
 __device__ __forceinline__ void pro_swiglu(const StepGemmParams& p, int tile, int tid, int j0) {
     const int quad = tid >> 5, lane = tid & 31;
     const bool hi = (lane & 16) != 0;  // lanes 16..31 hold the w3 ("up") rows of the features lanes 0..15 gate
     const int f = tile * 64 + quad * 16 + (lane & 15);
     float acc[R];
-    prev_sums<R, 32 / R>(p, tile, tid, j0, acc);
+    prev_sums<R, 32 / R, RT>(p, tile, tid, j0, acc);
 #pragma unroll
     for (int r = 0; r < R; ++r) {
         const float up = __shfl_xor_sync(0xffffffffu, acc[r], 16);
@@ -130,7 +134,7 @@ constexpr int kFinalizeRows = PRO == PRO_SWIGLU ? 8 : 4;
 
 // step_finalize: finishes the GEMM that produced the next GEMM's operand (one unit = R batch rows x one 128-feature
 // tile per CTA); launched between the two GEMMs, so the consumer GEMM finds its operand complete.
-template <int PRO>
+template <int PRO, int RT>
 __global__ void __launch_bounds__(kEpiThreads) step_finalize_kernel(const __grid_constant__ StepGemmParams p) {
     constexpr int R = kFinalizeRows<PRO>;
     __shared__ float red[4 * 32];
@@ -139,15 +143,18 @@ __global__ void __launch_bounds__(kEpiThreads) step_finalize_kernel(const __grid
     const int units = p.prev.tiles * ((p.rows + R - 1) / R);
     for (int u = blockIdx.x; u < units; u += gridDim.x) {
         const int tile = u % p.prev.tiles, j0 = (u / p.prev.tiles) * R;
-        if (PRO == PRO_RESID) pro_resid<R>(p, tile, threadIdx.x, j0, red);
-        else pro_swiglu<R>(p, tile, threadIdx.x, j0);
+        if (PRO == PRO_RESID) pro_resid<R, RT>(p, tile, threadIdx.x, j0, red);
+        else pro_swiglu<R, RT>(p, tile, threadIdx.x, j0);
     }
 }
 
-template <int NORM>
+template <int NORM, int RT>
 __global__ void __launch_bounds__(kStepThreads + (NORM ? kLoaderThreads : 0), 2)
 step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ StepGemmParams p) {
+    static_assert(RT == kStepRows || RT == kStepRowsMax, "row tile: 32 or 64");
+    constexpr int kStageBytes = kStageBytesOf<RT>;
+    constexpr int kBTileBytes = kBTileBytesOf<RT>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t tiles = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
@@ -159,7 +166,7 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint8_t* gen = smem_raw + (tiles - raw);
     uint8_t* bar_gen = gen + static_cast<size_t>(stages) * kStageBytes;
     float* scratch = reinterpret_cast<float*>(bar_gen + scratch_off);
-    float* r_s = scratch;       // [32] per-row rsqrt (normalisers)
+    float* r_s = scratch;       // [RT] per-row rsqrt (normalisers)
     uint4* normw_s = reinterpret_cast<uint4*>(bar_gen + scratch_off + kScratchBytes);  // [kblocks*8] norm weights
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -236,9 +243,9 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int ch = t; ch < nchunks; ch += kLoaderThreads)
                 normw_s[ch] = ch * 8 < p.K ? __ldg(reinterpret_cast<const uint4*>(p.norm_w + ch * 8)) : make_uint4(0, 0, 0, 0);
             pdl_wait();
-            if (t < 32) {
+            if (t < RT) {
                 // rsqrt(mean(x^2) + eps) of row t: the producer's per-tile sums, added in tile order (all loads in flight)
-                // (16-byte loads: every CTA of the grid reads these same 32 lines right after the grid-wide arrival)
+                // (16-byte loads: every CTA of the grid reads these same RT lines right after the grid-wide arrival)
                 const float4* q = reinterpret_cast<const float4*>(p.x_ssq + t * kSsqStride);
                 float4 a[kSsqStride / 4];
 #pragma unroll
@@ -254,8 +261,8 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 r_s[t] = rsqrtf(tot / static_cast<float>(p.K) + p.eps);
             }
             bar_sync(2, kLoaderThreads);
-            // 32 rows x 8 sixteen-byte chunks per k-block; thread t owns chunk (t & 7) of rows (t >> 3) + 16e
-            constexpr int kCells = 256 / kLoaderThreads;
+            // RT rows x 8 sixteen-byte chunks per k-block; thread t owns chunk (t & 7) of rows (t >> 3) + 16e
+            constexpr int kCells = RT * 8 / kLoaderThreads;
             const int c = t & 7, rb = t >> 3;
             float rr[kCells];
             uint32_t off[kCells];
@@ -299,16 +306,18 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
         }
     } else {
-        // ===== warpgroup 0: wgmma over the ring (rows [0, 64) and [64, 128) of the weight tile), then the fp32
-        // partial stores straight from the accumulator registers =====
+        // ===== warpgroup 0: wgmma over the ring (rows [0, 64) and [64, 128) of the weight tile; at RT = 64 each once
+        // per 32-row half of the operand tile, with the wgmma of the 32-row tile), then the fp32 partial stores
+        // straight from the accumulator registers =====
         pdl_wait();
         int it = 0;
         for (int n = item_begin; n < item_end; ++n) {
             const int4 w = p.sched[n];
             const int tile = w.x, slot = w.w;
-            float d0[kBN / 2], d1[kBN / 2];
+            // d0 / d1: weight rows [0, 64) / [64, 128); entries [16h, 16h + 16) hold operand rows [32h, 32h + 32)
+            float d0[RT / 2], d1[RT / 2];
 #pragma unroll
-            for (int e = 0; e < kBN / 2; ++e) d0[e] = d1[e] = 0.f;
+            for (int e = 0; e < RT / 2; ++e) d0[e] = d1[e] = 0.f;
             for (int kb = w.y; kb < w.z; ++kb, ++it) {
                 const int s = it % stages;
                 mbar_wait(full0 + 8u * s, static_cast<uint32_t>(it / stages) & 1u);
@@ -318,8 +327,12 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < kBlockK / 16; ++k) {
-                    wgmma_bf16<kBN>(d0, a0 + 2u * k, bd + 2u * k, 1);
-                    wgmma_bf16<kBN>(d1, a1 + 2u * k, bd + 2u * k, 1);
+#pragma unroll
+                    for (int hh = 0; hh < RT / kStepRows; ++hh) {
+                        const uint64_t bh = hh == 0 ? bd : make_gdesc(a_src + kATileBytes + hh * kHalfBTileBytes);
+                        wgmma_bf16<kStepRows>(d0 + 16 * hh, a0 + 2u * k, bh + 2u * k, 1);
+                        wgmma_bf16<kStepRows>(d1 + 16 * hh, a1 + 2u * k, bh + 2u * k, 1);
+                    }
                 }
                 wgmma_commit();
                 // release the slot as soon as its own MMAs retire: the producer refills it while the next k-block
@@ -329,10 +342,10 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 if (lane == 0) mbar_arrive(empty0 + 8u * s);
             }
             // accumulator element (feature i, batch row j) -> ws[slot][tile][j][i]
-            float* dst = p.ws + ((static_cast<size_t>(slot) * p.tiles + tile) * 32) * 128;
+            float* dst = p.ws + ((static_cast<size_t>(slot) * p.tiles + tile) * RT) * 128;
             const int i0 = warp * 16 + (lane >> 2);
 #pragma unroll
-            for (int b = 0; b < kBN / 8; ++b)
+            for (int b = 0; b < RT / 8; ++b)
 #pragma unroll
                 for (int r = 0; r < 4; ++r) {
                     const int j = 8 * b + 2 * (lane & 3) + (r & 1);
@@ -346,15 +359,19 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
 }
 
-template <int NORM>
+template <int NORM, int RT>
 int launch_t(const StepGemmPlan& plan, cudaStream_t st) {
-    auto k = step_gemm_kernel<NORM>;
+    auto k = step_gemm_kernel<NORM, RT>;
     FSB_LAUNCH(k, plan.grid, dim3(kStepThreads + (NORM ? kLoaderThreads : 0)), plan.smem, st, plan.tmA, plan.tmB, plan.p);
     return 0;
 }
 
-const void* kernel_of(int norm) {
-    return norm ? reinterpret_cast<const void*>(step_gemm_kernel<1>) : reinterpret_cast<const void*>(step_gemm_kernel<0>);
+const void* kernel_of(int norm, int rt) {
+    if (rt == kStepRowsMax)
+        return norm ? reinterpret_cast<const void*>(step_gemm_kernel<1, kStepRowsMax>)
+                    : reinterpret_cast<const void*>(step_gemm_kernel<0, kStepRowsMax>);
+    return norm ? reinterpret_cast<const void*>(step_gemm_kernel<1, kStepRows>)
+                : reinterpret_cast<const void*>(step_gemm_kernel<0, kStepRows>);
 }
 
 }  // namespace
@@ -362,32 +379,35 @@ const void* kernel_of(int norm) {
 int step_gemm_init() {
     static bool done = false;
     if (done) return 0;
-#define FSB_STEP_ATTR(B_)                                                                                          \
-    FSB_CUDA(cudaFuncSetAttribute(step_gemm_kernel<B_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-    FSB_CUDA(cudaFuncSetAttribute(step_gemm_kernel<B_>, cudaFuncAttributePreferredSharedMemoryCarveout,            \
+#define FSB_STEP_ATTR(B_, RT_)                                                                                          \
+    FSB_CUDA(cudaFuncSetAttribute(step_gemm_kernel<B_, RT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+    FSB_CUDA(cudaFuncSetAttribute(step_gemm_kernel<B_, RT_>, cudaFuncAttributePreferredSharedMemoryCarveout,            \
                                   cudaSharedmemCarveoutMaxShared));
-    FSB_STEP_ATTR(1) FSB_STEP_ATTR(0)
+    FSB_STEP_ATTR(1, kStepRows) FSB_STEP_ATTR(0, kStepRows) FSB_STEP_ATTR(1, kStepRowsMax) FSB_STEP_ATTR(0, kStepRowsMax)
 #undef FSB_STEP_ATTR
     done = true;
     return 0;
 }
 
 int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K, const __nv_bfloat16* act,
-                   bool norm_on_load, int num_ctas, int stages, float* ws, size_t ws_floats) {
+                   bool norm_on_load, int row_tile, int num_ctas, int stages, float* ws, size_t ws_floats) {
     memset(plan, 0, sizeof(*plan));
     FSB_CHECK(K % 8 == 0, "step GEMM: K=%d must be a multiple of 8", K);
     FSB_CHECK(act != nullptr, "step GEMM: operand X missing");
+    FSB_CHECK(row_tile == kStepRows || row_tile == kStepRowsMax, "step GEMM: row tile %d is not %d or %d", row_tile,
+              kStepRows, kStepRowsMax);
     const int norm = norm_on_load ? 1 : 0;
-    const void* kernel = kernel_of(norm);
+    const void* kernel = kernel_of(norm, row_tile);
     FSB_TRY(step_gemm_init());
     GemmOperand A{w, K, n_out, 1, K, static_cast<long long>(n_out) * K};
     FSB_TRY(gemm_make_tmap(&plan->tmA, A, kBlockM));
-    GemmOperand B{act, K, kStepRows, 1, K, static_cast<long long>(kStepRows) * K};
-    FSB_TRY(gemm_make_tmap(&plan->tmB, B, kBN));
+    GemmOperand B{act, K, row_tile, 1, K, static_cast<long long>(row_tile) * K};
+    FSB_TRY(gemm_make_tmap(&plan->tmB, B, row_tile));
     const int tiles = cdiv(n_out, kBlockM), kblocks = cdiv(K, kBlockK);
     const int normw_bytes = norm ? kblocks * 128 : 0;
+    const size_t stage_bytes = row_tile == kStepRowsMax ? kStageBytesOf<kStepRowsMax> : kStageBytesOf<kStepRows>;
     auto smem_of = [&](int st) {
-        return static_cast<size_t>(1024) + static_cast<size_t>(st) * kStageBytes + ((24 * st + 15) / 16) * 16 +
+        return static_cast<size_t>(1024) + static_cast<size_t>(st) * stage_bytes + ((24 * st + 15) / 16) * 16 +
                kScratchBytes + normw_bytes;
     };
     while (stages > 2 && 2 * (smem_of(stages) + 1024) > 228 * 1024) --stages;  // two CTAs per SM
@@ -422,7 +442,7 @@ int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K,
     int maxp = 0;
     for (int t = 0; t < tiles; ++t) maxp = std::max(maxp, nparts[t]);
     plan->max_parts = maxp;
-    FSB_CHECK(static_cast<size_t>(maxp) * tiles * 128 * 32 <= ws_floats, "step GEMM: partial workspace too small");
+    FSB_CHECK(static_cast<size_t>(maxp) * tiles * 128 * row_tile <= ws_floats, "step GEMM: partial workspace too small");
     FSB_CUDA(cudaMalloc(&plan->sched_dev, items.size() * sizeof(int4)));
     FSB_CUDA(cudaMemcpy(plan->sched_dev, items.data(), items.size() * sizeof(int4), cudaMemcpyHostToDevice));
     FSB_CUDA(cudaMalloc(&plan->cta_items_dev, cta_items.size() * sizeof(int)));
@@ -436,7 +456,7 @@ int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K,
     p.stages = stages;
     p.n_out = n_out;
     p.K = K;
-    p.rows = kStepRows;
+    p.rows = row_tile;
     p.a_hint = kEvictFirst;  // weights are streamed once per step (>> L2)
     p.b_hint = kEvictLast;   // the activation tile is re-read by every CTA
     p.ws = ws;
@@ -444,6 +464,7 @@ int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K,
     plan->smem = smem_of(stages);
     plan->pro = PRO_NONE;
     plan->norm = norm;
+    plan->rt = row_tile;
     plan->weight_bytes = static_cast<double>(n_out) * K * 2;
     return 0;
 }
@@ -455,6 +476,7 @@ StepPartials step_plan_partials(const StepGemmPlan& plan) {
     P.tiles = plan.p.tiles;
     P.n_out = plan.p.n_out;
     P.max_parts = plan.max_parts;
+    P.rt = plan.rt;
     return P;
 }
 
@@ -472,23 +494,28 @@ void step_plan_free(StepGemmPlan* plan) {
     plan->nparts_dev = nullptr;
 }
 
+namespace {
+template <int PRO, int RT>
+int finalize_t(const StepGemmParams& p, cudaStream_t st) {
+    const dim3 units(p.prev.tiles * cdiv(p.rows, kFinalizeRows<PRO>));
+    FSB_LAUNCH((step_finalize_kernel<PRO, RT>), units, dim3(kEpiThreads), 0, st, p);
+    return 0;
+}
+}  // namespace
+
 int step_finalize_launch(const StepGemmPlan& consumer, cudaStream_t st) {
     // `consumer`'s finalize fields (prev, bias / resid / x_out / ssq_out or h / I, rows) describe the work; one unit per CTA
     const int pro = consumer.pro;
     if (pro == PRO_NONE) return 0;
     const StepGemmParams& p = consumer.p;
-    if (pro == PRO_RESID) {
-        const dim3 units(p.prev.tiles * cdiv(p.rows, kFinalizeRows<PRO_RESID>));
-        FSB_LAUNCH(step_finalize_kernel<PRO_RESID>, units, dim3(kEpiThreads), 0, st, p);
-    } else {
-        const dim3 units(p.prev.tiles * cdiv(p.rows, kFinalizeRows<PRO_SWIGLU>));
-        FSB_LAUNCH(step_finalize_kernel<PRO_SWIGLU>, units, dim3(kEpiThreads), 0, st, p);
-    }
-    return 0;
+    if (p.prev.rt == kStepRowsMax)
+        return pro == PRO_RESID ? finalize_t<PRO_RESID, kStepRowsMax>(p, st) : finalize_t<PRO_SWIGLU, kStepRowsMax>(p, st);
+    return pro == PRO_RESID ? finalize_t<PRO_RESID, kStepRows>(p, st) : finalize_t<PRO_SWIGLU, kStepRows>(p, st);
 }
 
 int step_gemm_launch(const StepGemmPlan& plan, cudaStream_t st) {
-    return plan.norm ? launch_t<1>(plan, st) : launch_t<0>(plan, st);
+    if (plan.rt == kStepRowsMax) return plan.norm ? launch_t<1, kStepRowsMax>(plan, st) : launch_t<0, kStepRowsMax>(plan, st);
+    return plan.norm ? launch_t<1, kStepRows>(plan, st) : launch_t<0, kStepRows>(plan, st);
 }
 
 }  // namespace fsb

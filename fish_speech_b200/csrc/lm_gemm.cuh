@@ -2,9 +2,13 @@
 // inference.py:96-181 one frame).
 //
 //   D[i][j] = sum_k W[i][k] * X[j][k]        i = output feature (128 per tile: two wgmma of 64 rows)
-//                                            j = sequence slot of the batch (<= 32, the wgmma N)
+//                                            j = sequence slot of the batch (< RT, the row tile: 32 or 64)
 //
 // Life of one launch (one CTA = 5 warps + 4 normaliser warps, two CTAs per SM, the whole grid in one wave):
+// The row tile RT is chosen per engine: 32 rows (one wgmma.m64n32k16 per 64 weight rows and k16 step) up to 32
+// sequences, 64 rows (the same wgmma issued once per 32-row half of the operand tile, its descriptor 4 KB further)
+// up to 64. Every output element sees the same MMA sequence at either tile, so its bits do not depend on RT.
+//
 //   1. The TMA producer requests the first ring-full of weight tiles at once -- before griddepcontrol.wait, i.e.
 //      while the previous kernels are still finishing: weights do not depend on anything.
 //   2. Main loop: weights HBM -> shared memory by TMA (SWIZZLE_128B, EVICT_FIRST), operand X by TMA from L2; where X
@@ -31,17 +35,19 @@ namespace fsb {
 
 enum StepPro { PRO_NONE = 0, PRO_RESID = 1, PRO_SWIGLU = 2 };
 
-constexpr int kStepRows = 32;   // batch rows per step = wgmma N
+constexpr int kStepRows = 32;     // batch rows of the 32-row tile = wgmma N
+constexpr int kStepRowsMax = 64;  // the 64-row tile: two wgmma N=32 halves
 constexpr int kSsqStride = 32;  // floats per row of a sum-of-squares array: one per 128-feature tile (D <= 4096)
 
 // fp32 stream-K partials of one step GEMM:
-//   value(row j, feature i) = sum_{q < nparts[i/128]} ws[((q*tiles + i/128)*32 + j)*128 + i%128]
+//   value(row j, feature i) = sum_{q < nparts[i/128]} ws[((q*tiles + i/128)*rt + j)*128 + i%128]
 struct StepPartials {
     const float* ws;
     const int* nparts;  // [tiles]
     int tiles;
     int n_out;      // output features (rows of the weight matrix)
     int max_parts;  // max over tiles of nparts: slots [0, max_parts) exist in ws for every tile
+    int rt;         // row tile of the GEMM (32 or 64): rows per (slot, tile) block of ws
 };
 
 #ifdef __CUDACC__
@@ -49,8 +55,8 @@ struct StepPartials {
 __device__ __forceinline__ float step_partial_sum(const StepPartials& P, int row, int feat) {
     const int tile = feat >> 7;
     const int np = __ldg(P.nparts + tile);
-    const float* p = P.ws + (static_cast<size_t>(tile) * 32 + row) * 128 + (feat & 127);
-    const size_t ss = static_cast<size_t>(P.tiles) * 32 * 128;
+    const float* p = P.ws + (static_cast<size_t>(tile) * P.rt + row) * 128 + (feat & 127);
+    const size_t ss = static_cast<size_t>(P.tiles) * P.rt * 128;
     float s = 0.f;
     // The loads are bounded by max_parts (a launch constant), not by this tile's count: they leave together with
     // the load of the count instead of one round trip behind it; slots >= np hold stale data and are not added.
@@ -69,14 +75,14 @@ __device__ __forceinline__ float step_partial_sum(const StepPartials& P, int row
 template <int N>
 __device__ __forceinline__ void step_partial_sums(const StepPartials& P, int row, const int (&feat)[N], const bool (&ok)[N],
                                                   float (&out)[N]) {
-    const size_t ss = static_cast<size_t>(P.tiles) * 32 * 128;
+    const size_t ss = static_cast<size_t>(P.tiles) * P.rt * 128;
     int np[N];
     const float* p[N];
 #pragma unroll
     for (int k = 0; k < N; ++k) {
         const int f = ok[k] ? feat[k] : 0;
         np[k] = ok[k] ? __ldg(P.nparts + (f >> 7)) : 0;
-        p[k] = P.ws + (static_cast<size_t>(f >> 7) * 32 + row) * 128 + (f & 127);
+        p[k] = P.ws + (static_cast<size_t>(f >> 7) * P.rt + row) * 128 + (f & 127);
         out[k] = 0.f;
     }
     for (int q = 0; q < P.max_parts; q += 8) {  // bounded by the launch constant: see step_partial_sum
@@ -101,19 +107,19 @@ struct StepGemmParams {
     const int* cta_items;   // [grid + 1]
     int tiles, stages;
     int n_out, K;           // output features, reduction length
-    int rows;               // live batch rows (<= 32)
+    int rows;               // live batch rows (<= the row tile RT)
     unsigned long long a_hint, b_hint;
-    float* ws;              // out: [slot][tile][32 rows][128 features] fp32 partials
+    float* ws;              // out: [slot][tile][RT rows][128 features] fp32 partials
     // ---- step_finalize of the GEMM that produces this one's operand (pro != PRO_NONE) ----
     StepPartials prev;
     const __nv_bfloat16* bias;    // PRO_RESID: [prev.n_out] or null
-    const __nv_bfloat16* resid;   // PRO_RESID: [32][prev.n_out]; may alias x_out; null => no add
-    __nv_bfloat16* x_out;         // PRO_RESID: [32][prev.n_out] new residual stream
-    float* ssq_out;               // PRO_RESID: [32][kSsqStride]
-    __nv_bfloat16* h;             // PRO_SWIGLU: [32][I]; prev tile t = features [64t, 64t+64): lanes 32w+l (l < 16) =
+    const __nv_bfloat16* resid;   // PRO_RESID: [RT][prev.n_out]; may alias x_out; null => no add
+    __nv_bfloat16* x_out;         // PRO_RESID: [RT][prev.n_out] new residual stream
+    float* ssq_out;               // PRO_RESID: [RT][kSsqStride]
+    __nv_bfloat16* h;             // PRO_SWIGLU: [RT][I]; prev tile t = features [64t, 64t+64): lanes 32w+l (l < 16) =
     int I;                        //             w1 row, lanes 32w+16+l = w3 row
     // ---- operand X by normalise-on-load (NORM = 1) ----
-    const float* x_ssq;           // [32][kSsqStride] per-tile sum of squares of x
+    const float* x_ssq;           // [RT][kSsqStride] per-tile sum of squares of x
     const __nv_bfloat16* norm_w;  // [K]
     int x_nt;                     // tiles per row in x_ssq
     float eps;
@@ -125,6 +131,7 @@ struct StepGemmPlan {
     dim3 grid;
     size_t smem;
     int pro, norm;
+    int rt;  // row tile: 32 or 64
     void* sched_dev;
     int* cta_items_dev;
     int* nparts_dev;
@@ -132,10 +139,10 @@ struct StepGemmPlan {
     double weight_bytes;
 };
 
-// Operand X = act [32][K], fetched by TMA; norm_on_load: act is the un-normalised residual stream (the caller fills
-// p.x_ssq / p.norm_w / p.x_nt / p.eps).
+// Operand X = act [row_tile][K] (row_tile 32 or 64), fetched by TMA; norm_on_load: act is the un-normalised residual
+// stream (the caller fills p.x_ssq / p.norm_w / p.x_nt / p.eps).
 int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K, const __nv_bfloat16* act,
-                   bool norm_on_load, int num_ctas, int stages, float* ws, size_t ws_floats);
+                   bool norm_on_load, int row_tile, int num_ctas, int stages, float* ws, size_t ws_floats);
 // the partials `plan` produces, as a consumer sees them
 StepPartials step_plan_partials(const StepGemmPlan& plan);
 // `plan`'s operand is the output of `prev` finished with `pro` (PRO_RESID / PRO_SWIGLU): records what

@@ -10,7 +10,14 @@ import torch
 
 from . import _lib
 
-MAX_DECODE_BATCH = 32
+STEP_ROWS = 32  # row tile of the decode step GEMM for engines of up to 32 slots
+MAX_DECODE_BATCH = 64  # sequences per engine: above 32 the decode step runs its 64-row tile
+
+
+def decode_row_tile(max_batch: int) -> int:
+    """Rows of the decode step's GEMM tile and decode-state buffers for an engine of `max_batch` slots: 32 up to
+    32 slots, 64 above. A sequence's bits do not depend on it (include/fishb200.h, fsb_lm_config.max_batch)."""
+    return STEP_ROWS if max_batch <= STEP_ROWS else MAX_DECODE_BATCH
 
 
 class _DevView:
@@ -70,6 +77,7 @@ class LmEngine:
         kv_len = min(kv_len, config.max_seq_len)
         max_frames = int(max_frames or kv_len)
         self.max_batch, self.kv_len, self.max_rows, self.max_frames = max_batch, kv_len, max_rows, max_frames
+        self.row_tile = decode_row_tile(max_batch)
         self._keep = []  # device tensors the library points into
         dev = self.device
 
@@ -167,10 +175,11 @@ class LmEngine:
         _lib.check(self.lib.fsb_lm_buffer(self.h, name.encode(), C.byref(ptr), C.byref(nbytes)))
         c = self.cfg
         C1 = c.num_codebooks + 1
+        rt = self.row_tile
         shapes = {
             "out_tokens": ((self.max_batch, C1, self.max_frames), "<i4"),
             "n_out": ((self.max_batch,), "<i4"),
-            "pos": ((32,), "<i4"),
+            "pos": ((self.row_tile,), "<i4"),
             "finished": ((self.max_batch,), "<i4"),
             "cur_tok": ((self.max_batch, C1), "<i4"),
             "ras_window": ((self.max_batch, 10), "<i4"),
@@ -182,14 +191,14 @@ class LmEngine:
             "slot_seed": ((self.max_batch,), "<i8"),
             "slow_logits": ((self.max_batch, self.head_rows), "<f4"),
             "fast_logits": ((c.num_codebooks, self.max_batch, c.codebook_size), "<f4"),
-            # decode state (include/fishb200.h fsb_lm_test_layer_gemms); "attn" / "ffn_h" are flat: the rows of the
-            # stack being run sit at stride H*Dh / I of that stack
-            "x_slow": ((MAX_DECODE_BATCH, c.dim), "<u2"),
-            "x_fast": ((MAX_DECODE_BATCH, c.fast_dim), "<u2"),
-            "ssq_slow": ((MAX_DECODE_BATCH, 32), "<f4"),
-            "ssq_fast": ((MAX_DECODE_BATCH, 32), "<f4"),
-            "attn": ((MAX_DECODE_BATCH * max(c.n_head * c.head_dim, c.fast_n_head * c.fast_head_dim),), "<u2"),
-            "ffn_h": ((MAX_DECODE_BATCH * max(c.intermediate_size, c.fast_intermediate_size),), "<u2"),
+            # decode state (include/fishb200.h fsb_lm_test_layer_gemms), row_tile rows; "attn" / "ffn_h" are flat:
+            # the rows of the stack being run sit at stride H*Dh / I of that stack
+            "x_slow": ((rt, c.dim), "<u2"),
+            "x_fast": ((rt, c.fast_dim), "<u2"),
+            "ssq_slow": ((rt, 32), "<f4"),
+            "ssq_fast": ((rt, 32), "<f4"),
+            "attn": ((rt * max(c.n_head * c.head_dim, c.fast_n_head * c.fast_head_dim),), "<u2"),
+            "ffn_h": ((rt * max(c.intermediate_size, c.fast_intermediate_size),), "<u2"),
         }
         shape, ts = shapes[name]
         with torch.cuda.device(self.device):

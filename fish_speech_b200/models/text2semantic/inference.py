@@ -3,7 +3,7 @@
 Same entry points and semantics (`init_model`, `decode_one_token_ar`, `decode_n_tokens`, `generate`,
 `generate_long`, `launch_thread_safe_queue`, `load_codec_model`, `encode_audio`, `decode_to_audio`, the
 click `main`), with the per-frame math executed by the CUDA engine.  New on top of the reference:
-`generate_batch` — up to 32 independent utterances decoded in lock-step on one GPU (the reference is
+`generate_batch` — up to 64 independent utterances decoded in lock-step on one GPU (the reference is
 batch-1 only: inference.py:87, 284-288).
 
 The CPU-side prompt builder (Conversation / ContentSequence / tokenizer) is the reference's own code
@@ -23,6 +23,7 @@ from typing import Callable, Literal, Optional, Sequence, Union
 import numpy as np
 import torch
 
+from ...engine import MAX_DECODE_BATCH
 from .llama import IM_END_TOKEN, DualARTransformer
 
 try:  # loguru is what the reference logs with; fall back to stdlib logging if absent
@@ -179,7 +180,7 @@ def generate_batch(
     audio_parts: Optional[torch.Tensor] = None,
     **sampling_kwargs,
 ) -> list[torch.Tensor]:
-    """`generate` for up to 32 independent utterances at once (one KV slot each). Every sequence sees
+    """`generate` for up to 64 independent utterances at once (one KV slot each). Every sequence sees
     exactly the computation it would see alone: the kernels are batch-invariant, so the result for a
     prompt does not depend on its batch neighbours. `reuse_prefix=True` (sampling_kwargs) prefills only the
     rows whose K/V is not already in the cache (LmEngine.prefill_reusing): same tokens, less work."""
@@ -187,8 +188,8 @@ def generate_batch(
         raise NotImplementedError("audio_parts is not supported (nor by the reference model, llama.py:423-433)")
     cfg = model.config
     B = len(prompts)
-    if B < 1 or B > 32:
-        raise ValueError("generate_batch handles 1..32 prompts per call")
+    if B < 1 or B > MAX_DECODE_BATCH:
+        raise ValueError(f"generate_batch handles 1..{MAX_DECODE_BATCH} prompts per call")
     T_max = max(int(p.size(1)) for p in prompts)
     for p in prompts:
         if p.size(1) >= cfg.max_seq_len:
@@ -588,22 +589,47 @@ def serve_requests(model, input_queue: "queue.Queue", max_slots: int, frames_per
             logger.error(traceback.format_exc())
 
 
+def slow_kv_bytes_per_position(config) -> int:
+    """Bytes of slow-stack K and V cache one sequence slot holds per position (bf16): 147 456 at S2-Pro geometry."""
+    return 2 * config.n_layer * config.n_local_heads * config.head_dim * 2
+
+
+def check_serve_kv_fits(slots: int, kv_len: int, config, free_bytes: int) -> None:
+    """Raise a ValueError naming FSB_SERVE_KV_LEN when `slots` slow KV caches of `kv_len` positions do not fit in
+    `free_bytes` of device memory (64 slots x 8192 positions need 77 GB at S2-Pro geometry)."""
+    need = slots * kv_len * slow_kv_bytes_per_position(config)
+    if need > free_bytes:
+        fit = free_bytes // max(1, slots * slow_kv_bytes_per_position(config))
+        raise ValueError(f"{slots} slots x {kv_len} KV positions need {need / 1e9:.1f} GB of slow KV cache, but only "
+                         f"{free_bytes / 1e9:.1f} GB of device memory is free: lower FSB_SERVE_KV_LEN (at most "
+                         f"{fit} fits) or FSB_SERVE_SLOTS")
+
+
 def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool = False):
     """inference.py:736-799: the model lives in ONE daemon worker thread fed by a queue; `None` shuts
     it down; errors are returned as WrappedGenerateResponse(status="error", response=exc).
 
-    FSB_SERVE_SLOTS=n (2..32) makes the worker a slot scheduler that runs up to n requests concurrently
+    FSB_SERVE_SLOTS=n (2..64) makes the worker a slot scheduler that runs up to n requests concurrently
     (`serve_requests`), each with a KV cache of FSB_SERVE_KV_LEN positions (default 8192; a slot costs
-    147 456 B per position at the S2-Pro geometry). Unset / 1: the reference's one-at-a-time loop."""
+    147 456 B per position at the S2-Pro geometry). Unset / 1: the reference's one-at-a-time loop. If the slots'
+    KV caches do not fit in free device memory, this raises a ValueError naming FSB_SERVE_KV_LEN."""
     input_queue = queue.Queue()
     init_event = threading.Event()
-    slots = max(1, min(32, int(os.environ.get("FSB_SERVE_SLOTS", "1"))))
+    init_error: list = []
+    slots = max(1, min(MAX_DECODE_BATCH, int(os.environ.get("FSB_SERVE_SLOTS", "1"))))
 
     def worker():
         model, decode_one_token = init_model(checkpoint_path, device, precision, compile=compile)
         if slots > 1:
             kv = min(int(os.environ.get("FSB_SERVE_KV_LEN", "8192")), model.config.max_seq_len)
-            model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype)
+            try:
+                if torch.device(device).type == "cuda":
+                    check_serve_kv_fits(slots, kv, model.config, torch.cuda.mem_get_info(torch.device(device))[0])
+                model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype)
+            except Exception as e:
+                init_error.append(e)
+                init_event.set()
+                return
             init_event.set()
             serve_requests(model, input_queue, slots)
             return
@@ -629,6 +655,8 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
 
     threading.Thread(target=worker, daemon=True).start()
     init_event.wait()
+    if init_error:
+        raise init_error[0]
     return input_queue
 
 

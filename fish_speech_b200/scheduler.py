@@ -16,7 +16,7 @@ from typing import Callable, Optional
 
 import torch
 
-from .engine import bf16_round
+from .engine import MAX_DECODE_BATCH, bf16_round
 
 
 @dataclass(eq=False)  # identity semantics: requests hold tensors
@@ -52,8 +52,8 @@ class ContinuousBatcher:
         all weights for the new rows only, so grouping them trades admission latency for throughput."""
         from .models.text2semantic.inference import _ensure_engine
 
-        if not 1 <= max_slots <= 32:
-            raise ValueError("max_slots must be in 1..32")
+        if not 1 <= max_slots <= MAX_DECODE_BATCH:
+            raise ValueError(f"max_slots must be in 1..{MAX_DECODE_BATCH}")
         self.model = model
         self.cfg = model.config
         self.eng = _ensure_engine(model, max_slots)
@@ -200,7 +200,7 @@ class ContinuousBatcher:
             self._len[s] += k
         self.eng.set_context_bound_exact(min(max(self._len.values()) + 1, self.eng.kv_len))
         # every slot row is decoded: idle and frozen rows cost one attention position and nothing else
-        # (the GEMMs stream the weights once for 32 activation rows whatever the number of live ones)
+        # (the GEMMs stream the weights once for the engine's 32- or 64-row tile whatever the number of live rows)
         self.eng.decode(self.max_slots, k, None, use_graph=True)
         self.frames_run += k
         self.slot_frames += k * len(self.active)

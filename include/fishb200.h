@@ -52,7 +52,8 @@ typedef struct {
     int qk_norm, fast_qk_norm;           /* attention_qk_norm / fast_attention_qk_norm */
     int scale_codebook_embeddings;       /* llama.py:416-420 */
     int norm_fastlayer_input;            /* llama.py:459-461 */
-    int max_batch;                       /* resident sequences ("slots"), <= 32 */
+    int max_batch;                       /* resident sequences ("slots"), <= 64; above 32 the decode step runs
+                                            its 64-row tile (RT = 64), else the 32-row one (RT = 32) */
     int kv_len;                          /* KV-cache positions per sequence */
     int max_rows;                        /* token rows per prefill pass */
     int max_frames;                      /* generated frames kept per sequence */
@@ -152,14 +153,14 @@ int fsb_lm_set_slot_control(fsb_lm* h, int enable);
 int fsb_lm_reset(fsb_lm* h, void* stream);
 
 /* Named device buffers of the handle, for reading results and for tests:
- *   "out_tokens" int32 [max_batch][C+1][max_frames], "n_out" int32 [max_batch], "pos" int32 [max_batch],
+ *   "out_tokens" int32 [max_batch][C+1][max_frames], "n_out" int32 [max_batch], "pos" int32 [RT],
  *   "finished" int32 [max_batch], "cur_tok" int32 [max_batch][C+1], "ras_window" int32 [max_batch][10],
  *   the slot-control arrays listed at fsb_lm_set_slot_control,
  *   debug only: "slow_logits" f32 [max_batch][head_rows], "fast_logits" f32 [C][max_batch][codebook_size];
- *   the decode state (for fsb_lm_test_layer_gemms): "x_slow" / "x_fast" bf16 [32][dim] / [32][fast_dim] residual
- *   streams, "ssq_slow" / "ssq_fast" f32 [32][32] their per-128-feature sums of squares, "attn" bf16 [32 * max H*Dh]
- *   (the wo operand: rows of the stack being run at stride H*Dh), "ffn_h" bf16 [32 * max I] (the w2 operand:
- *   rows at stride I of the stack being run) */
+ *   the decode state (for fsb_lm_test_layer_gemms), RT = the decode row tile (32 for max_batch <= 32, else 64):
+ *   "x_slow" / "x_fast" bf16 [RT][dim] / [RT][fast_dim] residual streams, "ssq_slow" / "ssq_fast" f32 [RT][32] their
+ *   per-128-feature sums of squares, "attn" bf16 [RT * max H*Dh] (the wo operand: rows of the stack being run at
+ *   stride H*Dh), "ffn_h" bf16 [RT * max I] (the w2 operand: rows at stride I of the stack being run) */
 int fsb_lm_buffer(fsb_lm* h, const char* name, void** d_ptr, size_t* bytes);
 
 /* Measurement hook for bench.py: launch every weight-streaming step GEMM of one decode frame `reps` times
@@ -260,6 +261,11 @@ int fsb_op_gemm(const void* d_a, const void* d_b, float* d_out, int m, int n, in
  * that ran. Synchronises `stream`. */
 int fsb_op_step_gemm(const void* d_w, int n_out, int K, const void* d_x, int rows, const void* d_norm_w,
                      const float* d_x_ssq, float eps, int num_ctas, int stages, float* d_out, int* info, void* stream);
+/* The same for either row tile of the decode step: row_tile 32 or 64; X bf16 [row_tile][K], all row_tile rows
+ * readable; d_x_ssq f32 [row_tile][32]; rows in [1, row_tile]. fsb_op_step_gemm is this with row_tile = 32. */
+int fsb_op_step_gemm_tile(const void* d_w, int n_out, int K, const void* d_x, int row_tile, int rows,
+                          const void* d_norm_w, const float* d_x_ssq, float eps, int num_ctas, int stages, float* d_out,
+                          int* info, void* stream);
 
 /* Runs the step GEMMs of decode layer `layer` of the slow (fast = 0) or fast (fast = 1) stack for `rows` batch rows
  * exactly as fsb_lm_decode does (the handle's own plans, launch order and partial workspace), without attention:

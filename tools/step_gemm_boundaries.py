@@ -9,10 +9,10 @@ per-launch weight bytes over the four kinds:
 t0 is the fixed cost of a boundary, BW the streaming rate inside a GEMM. For reference it also times the frame's whole
 step GEMM chain (the replay line of bench.py) and decode frames.
 
-    python tools/step_gemm_boundaries.py [--min-s 0.5]
+    python tools/step_gemm_boundaries.py [--min-s 0.5] [--batch 32]
 
 Prints one JSON object, with the card's name, power limit and maximum SM clock. Needs a GPU; S2-Pro geometry with
-synthetic weights, batch 32.
+synthetic weights, batch 32 by default (an engine of --batch slots: above 32 it runs the 64-row step GEMM).
 """
 from __future__ import annotations
 
@@ -31,7 +31,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 KINDS = ("qkv", "wo", "w13", "w2")
-B, T_PROMPT = 32, 64
+T_PROMPT = 64
 
 
 def card() -> dict:
@@ -75,7 +75,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--min-s", type=float, default=0.5, help="least length of each timed window")
     ap.add_argument("--frames", type=int, default=64, help="decode frames timed")
+    ap.add_argument("--batch", type=int, default=32, help="engine slots = rows of every step (1..64)")
     args = ap.parse_args()
+    B = args.batch
 
     from bench import make_prompts, s2pro_cfg
     from fish_speech_b200 import _lib, synthetic

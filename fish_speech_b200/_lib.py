@@ -20,7 +20,7 @@ class LmConfig(C.Structure):
         "semantic_begin_id", "semantic_end_id", "im_end_id")] + [("norm_eps", C.c_float)] + [
         (n, C.c_int) for n in (
             "qk_norm", "fast_qk_norm", "scale_codebook_embeddings", "norm_fastlayer_input",
-            "max_batch", "kv_len", "max_rows", "max_frames", "debug")]
+            "max_batch", "kv_len", "max_rows", "max_frames", "debug", "kv_pages")]
 
 
 class LmLayer(C.Structure):
@@ -81,6 +81,7 @@ def lib() -> C.CDLL:
     L.fsb_lm_buffer.argtypes = [vp, C.c_char_p, C.POINTER(vp), C.POINTER(C.c_size_t)]
     L.fsb_lm_set_sampler_noise.argtypes = [vp, vp, i32, i32]
     L.fsb_lm_copy_kv.argtypes = [vp, i32, i32, i32, vp]
+    L.fsb_lm_copy_kv_page.argtypes = [vp, i32, i32, i32, vp]
     L.fsb_lm_bench_gemms.argtypes = [vp, i32, C.POINTER(C.c_double), C.POINTER(i32), vp]
     L.fsb_lm_bench_step_kind.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_double), C.POINTER(i32), vp]
     f32p, i32p, ll = C.c_void_p, C.POINTER(C.c_int), C.c_longlong

@@ -81,11 +81,21 @@ __global__ void __launch_bounds__(kAtThreads) attn_tile_kernel(AttnArgs a, float
 #pragma unroll
         for (int e = 0; e < 4; ++e) o[nt][e] = 0.f;
 
-    auto load_tile = [&](int buf, const __nv_bfloat16* kbase, const __nv_bfloat16* vbase, int kt, int hi) {
+    // K/V tile of positions kt .. kt + 63 of sequence `seq`: contiguous, or exactly one (mapped) page of a paged cache
+    auto load_tile = [&](int buf, int seq, int kt, int hi) {
+        size_t tbase;
+        if (a.kv_page != nullptr) {
+            const int pg = a.kv_page[static_cast<size_t>(seq) * a.kv_page_ld + kt / kKvPage];
+            tbase = (static_cast<size_t>(pg) * a.Hkv + g) * kKvPage * DH;
+        } else {
+            tbase = ((static_cast<size_t>(seq) * a.Hkv + g) * a.S + kt) * DH;
+        }
+        const __nv_bfloat16* kbase = a.kcache + tbase;
+        const __nv_bfloat16* vbase = a.vcache + tbase;
         for (int e = tid; e < kTK * CH; e += kAtThreads) {
             const int i = e / CH, c = e - i * CH;
             const bool ok = kt + i <= hi;
-            const size_t off = static_cast<size_t>(ok ? kt + i : 0) * DH + c * 8;
+            const size_t off = static_cast<size_t>(ok ? i : 0) * DH + c * 8;
             const uint32_t d = buf * TILEB + i * ROWB + ((c ^ (i & 7)) << 4);
             cp_async16(sK + d, kbase + off, ok);
             cp_async16(sV + d, vbase + off, ok);
@@ -102,20 +112,25 @@ __global__ void __launch_bounds__(kAtThreads) attn_tile_kernel(AttnArgs a, float
             // ---- one run: rows [start, end) = positions p0 .. p0 + (end - start) - 1 of sequence `seq` ----
             const int hi = min(p0 + (end - start) - 1, a.S - 1);
             const int lo = a.window > 0 ? max(0, p0 - a.window + 1) : 0;
-            const size_t cbase = (static_cast<size_t>(seq) * a.Hkv + g) * a.S * DH;
-            const __nv_bfloat16* kbase = a.kcache + cbase;
-            const __nv_bfloat16* vbase = a.vcache + cbase;
             const bool v0 = qi0 >= start && qi0 < end, v1 = qi1 >= start && qi1 < end;
             const int pq0 = p0 + (qi0 - start), pq1 = p0 + (qi1 - start);
             const int lo0 = a.window > 0 ? pq0 - a.window + 1 : 0, lo1 = a.window > 0 ? pq1 - a.window + 1 : 0;
             const int kt0 = (lo / kTK) * kTK;
             int buf = 0;
-            __syncthreads();  // the previous run's last tile has been consumed
-            load_tile(0, kbase, vbase, kt0, hi);
+            bool unmapped = false;  // a page of the run's history is not mapped: its rows attend to nothing (zeros)
+            if (a.kv_page != nullptr)
+                for (int j = kt0 / kKvPage + tid; j <= hi / kKvPage; j += kAtThreads)
+                    unmapped |= a.kv_page[static_cast<size_t>(seq) * a.kv_page_ld + j] < 0;
+            // (also: the previous run's last tile has been consumed)
+            if (__syncthreads_or(unmapped)) {
+                start = end;
+                continue;
+            }
+            load_tile(0, seq, kt0, hi);
             for (int kt = kt0; kt <= hi; kt += kTK) {
                 const bool more = kt + kTK <= hi;
                 if (more) {
-                    load_tile(buf ^ 1, kbase, vbase, kt + kTK, hi);
+                    load_tile(buf ^ 1, seq, kt + kTK, hi);
                     cp_async_wait<1>();
                 } else {
                     cp_async_wait<0>();
@@ -239,6 +254,7 @@ int launch_t(const AttnArgs& a, cudaStream_t st) {
 }  // namespace
 
 bool attn_tile_supported(const AttnArgs& a) {
+    static_assert(kTK == kKvPage, "one K/V tile is one page of a paged cache");
     return a.bf16_math == 0 && (a.Dh == 64 || a.Dh == 128) && a.H % a.Hkv == 0;
 }
 

@@ -4,7 +4,8 @@
 // HBM layout (all bf16 unless noted)
 //   weights            caller-owned, row-major [out, in] as in the checkpoint (TMA-ready, K-major); the fused
 //                      w1|w3 matrix has its rows interleaved per 128-row tile (lm_gemm.cuh, w13_gate_row)
-//   slow KV cache      [n_layer][max_batch][Hkv][kv_len][Dh]   x2 (K, V)
+//   slow KV cache      [n_layer][kv_pages][Hkv][64][Dh]   x2 (K, V): a pool of 64-position pages; page table "kv_page"
+//                      int32 [max_batch][ceil(kv_len / 64)] maps a sequence's positions to pages (-1: not mapped)
 //   fast KV cache      [n_fast_layer][max_batch][fHkv][num_codebooks][fDh]  x2
 //   decode state       residual streams x_slow / x_fast [RT][D] + their per-128-feature sums of squares
 //                      (fp32 [RT][32]); q / attention / SwiGLU operands [RT][*]; logits fp32 [max_batch][n]
@@ -56,6 +57,8 @@ struct Stack {
     std::vector<StepLayer> dec;     // decode: fused step GEMMs
     std::vector<PrefillLayer> pf;   // prefill: BN=128 tiles, fp32 result + consumer kernels (slow only)
     bf16 *kcache = nullptr, *vcache = nullptr;
+    int* kv_page = nullptr;  // slow stack: page table [max_batch][kv_page_ld] of the paged cache; fast stack: contiguous
+    int kv_page_ld = 0, n_pages = 0;
     const bf16* freqs = nullptr;
     size_t cache_layer_stride = 0;
     bf16* xres = nullptr;  // decode residual stream [RT][D]
@@ -238,6 +241,8 @@ int run_stack_decode(fsb_lm* h, Stack& s, int rows, const int* row_seq, const in
         aa.freqs = s.freqs;
         aa.kcache = s.kcache + l * s.cache_layer_stride;
         aa.vcache = s.vcache + l * s.cache_layer_stride;
+        aa.kv_page = s.kv_page;
+        aa.kv_page_ld = s.kv_page_ld;
         aa.row_seq = row_seq;
         aa.row_pos = row_pos;
         aa.out = h->attn_d;
@@ -275,6 +280,8 @@ int run_stack_prefill(fsb_lm* h, Stack& s, int rows, const int* row_seq, const i
         qa.q = h->q_p;
         qa.kcache = s.kcache + l * s.cache_layer_stride;
         qa.vcache = s.vcache + l * s.cache_layer_stride;
+        qa.kv_page = s.kv_page;
+        qa.kv_page_ld = s.kv_page_ld;
         qa.rows = rows; qa.H = s.H; qa.Hkv = s.Hkv; qa.Dh = s.Dh; qa.S = s.S;
         qa.eps = eps;
         FSB_TRY(launch_qkv_prep(qa, st));
@@ -282,6 +289,8 @@ int run_stack_prefill(fsb_lm* h, Stack& s, int rows, const int* row_seq, const i
         aa.q = h->q_p;
         aa.kcache = qa.kcache;
         aa.vcache = qa.vcache;
+        aa.kv_page = s.kv_page;
+        aa.kv_page_ld = s.kv_page_ld;
         aa.row_seq = row_seq;
         aa.row_pos = row_pos;
         aa.out = h->attn_p;
@@ -455,6 +464,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     FSB_CHECK((cfg->head_dim == 64 || cfg->head_dim == 128) && (cfg->fast_head_dim == 64 || cfg->fast_head_dim == 128),
               "head_dim must be 64 or 128");
     FSB_CHECK(w->head_rows == cfg->semantic_end_id - cfg->semantic_begin_id + 2, "head_rows mismatch");
+    FSB_CHECK(cfg->kv_len >= 1 && cfg->kv_pages >= 0, "kv_len must be >= 1 and kv_pages >= 0");
     fsb_lm* h = new fsb_lm();
     h->cfg = *cfg;
     int dev = 0;
@@ -544,12 +554,20 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &h->q_p, static_cast<size_t>(R) * s.H * s.Dh));
     TRYC(dalloc(h, &h->attn_p, static_cast<size_t>(R) * s.H * s.Dh));
     TRYC(dalloc(h, &h->h_p, static_cast<size_t>(R) * s.I));
-    s.cache_layer_stride = static_cast<size_t>(cfg->max_batch) * s.Hkv * s.S * s.Dh;
+    s.kv_page_ld = cdiv(s.S, kKvPage);
+    s.n_pages = cfg->kv_pages > 0 ? cfg->kv_pages : cfg->max_batch * s.kv_page_ld;
+    s.cache_layer_stride = static_cast<size_t>(s.n_pages) * s.Hkv * kKvPage * s.Dh;
     f.cache_layer_stride = static_cast<size_t>(cfg->max_batch) * f.Hkv * f.S * f.Dh;
     TRYC(dalloc(h, &s.kcache, s.cache_layer_stride * s.nl));
     TRYC(dalloc(h, &s.vcache, s.cache_layer_stride * s.nl));
     TRYC(dalloc(h, &f.kcache, f.cache_layer_stride * f.nl));
     TRYC(dalloc(h, &f.vcache, f.cache_layer_stride * f.nl));
+    TRYC(dalloc(h, &s.kv_page, static_cast<size_t>(cfg->max_batch) * s.kv_page_ld, "kv_page"));
+    if (cudaMemset(s.kv_page, 0xff, static_cast<size_t>(cfg->max_batch) * s.kv_page_ld * 4) != cudaSuccess) {
+        set_error("fsb_lm_create: page table init failed");  // every entry -1: nothing mapped
+        fsb_lm_destroy(h);
+        return 1;
+    }
     TRYC(dalloc(h, &h->cur_tok, static_cast<size_t>(cfg->max_batch) * (C + 1), "cur_tok"));
     TRYC(dalloc(h, &h->out_tokens, static_cast<size_t>(cfg->max_batch) * (C + 1) * cfg->max_frames, "out_tokens"));
     TRYC(dalloc(h, &h->n_out, cfg->max_batch, "n_out"));
@@ -857,9 +875,25 @@ int fsb_lm_copy_kv(fsb_lm* h, int src_slot, int dst_slot, int n_pos, void* strea
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     FSB_CHECK(h != nullptr, "copy_kv: null handle");
     Stack& s = h->slow;
+    const int B = h->cfg.max_batch;
     FSB_CHECK(n_pos >= 0 && n_pos <= s.S, "copy_kv: n_pos=%d outside the KV cache (%d)", n_pos, s.S);
-    FSB_TRY(launch_kv_copy(s.kcache, s.nl, h->cfg.max_batch, s.Hkv, s.S, s.Dh, src_slot, dst_slot, n_pos, st));
-    FSB_TRY(launch_kv_copy(s.vcache, s.nl, h->cfg.max_batch, s.Hkv, s.S, s.Dh, src_slot, dst_slot, n_pos, st));
+    FSB_CHECK(src_slot >= 0 && src_slot < B && dst_slot >= 0 && dst_slot < B, "copy_kv: slot outside [0, %d)", B);
+    if (src_slot == dst_slot) return 0;
+    const int* src = s.kv_page + static_cast<size_t>(src_slot) * s.kv_page_ld;
+    const int* dst = s.kv_page + static_cast<size_t>(dst_slot) * s.kv_page_ld;
+    FSB_TRY(launch_kv_copy(s.kcache, s.nl, s.n_pages, s.Hkv, s.Dh, src, 0, dst, 0, n_pos, st));
+    FSB_TRY(launch_kv_copy(s.vcache, s.nl, s.n_pages, s.Hkv, s.Dh, src, 0, dst, 0, n_pos, st));
+    return 0;
+}
+
+int fsb_lm_copy_kv_page(fsb_lm* h, int src_page, int dst_page, int n_pos, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(h != nullptr, "copy_kv_page: null handle");
+    Stack& s = h->slow;
+    FSB_CHECK(n_pos >= 0 && n_pos <= kKvPage, "copy_kv_page: n_pos=%d outside [0, %d]", n_pos, kKvPage);
+    if (src_page == dst_page) return 0;
+    FSB_TRY(launch_kv_copy(s.kcache, s.nl, s.n_pages, s.Hkv, s.Dh, nullptr, src_page, nullptr, dst_page, n_pos, st));
+    FSB_TRY(launch_kv_copy(s.vcache, s.nl, s.n_pages, s.Hkv, s.Dh, nullptr, src_page, nullptr, dst_page, n_pos, st));
     return 0;
 }
 

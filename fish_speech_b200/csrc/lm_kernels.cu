@@ -268,10 +268,8 @@ __global__ void qkv_prep_kernel(QkvPrepArgs a) {
     } else if (pos >= 0 && pos < a.S) {
         const int g = kind == 1 ? head - a.H : head - a.H - a.Hkv;
         __nv_bfloat16* cache = kind == 1 ? a.kcache : a.vcache;
-        const int b = a.row_seq[row];
-        uint32_t* dst = reinterpret_cast<uint32_t*>(
-            cache + ((static_cast<size_t>(b) * a.Hkv + g) * a.S + pos) * Dh);
-        dst[t] = packed;
+        const long long off = kv_offset(a.kv_page, a.kv_page_ld, a.row_seq[row], g, pos, a.Hkv, a.S, Dh);
+        if (off >= 0) reinterpret_cast<uint32_t*>(cache + off)[t] = packed;
     }
 }
 
@@ -336,7 +334,8 @@ __global__ void __launch_bounds__(kQkvRowThreads) qkv_prep_row_kernel(QkvPrepArg
             } else if (pos >= 0 && pos < a.S) {
                 const int g = kind == 1 ? head - a.H : head - a.H - a.Hkv;
                 __nv_bfloat16* cache = kind == 1 ? a.kcache : a.vcache;
-                reinterpret_cast<uint32_t*>(cache + ((static_cast<size_t>(b) * a.Hkv + g) * a.S + pos) * DH)[t] = packed;
+                const long long off = kv_offset(a.kv_page, a.kv_page_ld, b, g, pos, a.Hkv, a.S, DH);
+                if (off >= 0) reinterpret_cast<uint32_t*>(cache + off)[t] = packed;
             }
         }
     }
@@ -354,10 +353,13 @@ constexpr int kAttnPrefetchPos = 2048;  // positions of K/V history the decode a
 // one is walked in chunks of lcap three times -- maximum, sum of exponentials, weighted values -- recomputing the
 // scores each time.  Chunk boundaries are multiples of 32, so every lane and every warp accumulates exactly the
 // sequence of terms it would in one pass: the result is bit-identical to the unchunked kernel, whatever lcap is.
+// Row p of the history: kc + pt[p / kKvPage] * page_stride + (p % kKvPage) * DH, with `pt` the row's page-table entries
+// in shared memory. A paged cache: kc / vc at this KV head's offset inside a page, page_stride elements between pages
+// (kv_offset). A contiguous one: pt[j] = j and page_stride = kKvPage * DH, one code path for both.
 template <int DH, int G>
 __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, const __nv_bfloat16* kc,
-                                       const __nv_bfloat16* vc, int L, int lcap, float scale, int bf16_math,
-                                       __nv_bfloat16* out) {
+                                       const __nv_bfloat16* vc, const int* pt, size_t page_stride, int L, int lcap,
+                                       float scale, int bf16_math, __nv_bfloat16* out) {
     static_assert(G <= kAttnWarps, "one warp per query head in the softmax");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     constexpr int LPR = DH / 8;    // lanes per cache row (16-byte loads)
@@ -371,15 +373,18 @@ __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, c
 #pragma unroll
         for (int e = 0; e < 8; ++e) qr[gg][e] = qs[gg * DH + li * 8 + e];
 
+    auto at = [&](const __nv_bfloat16* base, int p) {
+        return base + static_cast<size_t>(pt[p / kKvPage]) * page_stride + (p % kKvPage) * DH;
+    };
     auto scores = [&](int c0, int n) {  // sc[gg][p - c0] for p in [c0, c0 + n)
-        const __nv_bfloat16* kcc = kc + static_cast<size_t>(c0) * DH;
         for (int pb = warp * RPW * UNR; pb < n; pb += kAttnWarps * RPW * UNR) {
             uint4 u[UNR];
+            const __nv_bfloat16* kp = at(kc, c0 + pb);  // RPW * UNR positions from a multiple of 8: one page
 #pragma unroll
             for (int j = 0; j < UNR; ++j) {
                 const int p = pb + j * RPW + sub;
                 u[j] = make_uint4(0, 0, 0, 0);
-                if (p < n) u[j] = *reinterpret_cast<const uint4*>(kcc + static_cast<size_t>(p) * DH + li * 8);
+                if (p < n) u[j] = *reinterpret_cast<const uint4*>(kp + (j * RPW + sub) * DH + li * 8);
             }
 #pragma unroll
             for (int j = 0; j < UNR; ++j) {
@@ -458,8 +463,8 @@ __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, c
             }
             __syncthreads();
         }
-        const __nv_bfloat16* vcc = vc + static_cast<size_t>(c0) * DH;
         for (int pb = warp; pb < n; pb += kAttnWarps * UNR) {
+            const __nv_bfloat16* vp = at(vc, c0 + pb);  // positions pb + 8 j, inside a run of 32 from a multiple of 32: one page
             float vf[UNR][DPL];
 #pragma unroll
             for (int j = 0; j < UNR; ++j) {
@@ -468,10 +473,10 @@ __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, c
                 for (int e = 0; e < DPL; ++e) vf[j][e] = 0.f;
                 if (p < n) {
                     if (DPL == 4) {
-                        const uint2 u2 = *reinterpret_cast<const uint2*>(vcc + static_cast<size_t>(p) * DH + lane * 4);
+                        const uint2 u2 = *reinterpret_cast<const uint2*>(vp + (j * kAttnWarps) * DH + lane * 4);
                         vf[j][0] = bf_lo(u2.x); vf[j][1] = bf_hi(u2.x); vf[j][2 % DPL] = bf_lo(u2.y); vf[j][3 % DPL] = bf_hi(u2.y);
                     } else {
-                        const uint32_t u1 = *reinterpret_cast<const uint32_t*>(vcc + static_cast<size_t>(p) * DH + lane * 2);
+                        const uint32_t u1 = *reinterpret_cast<const uint32_t*>(vp + (j * kAttnWarps) * DH + lane * 2);
                         vf[j][0] = bf_lo(u1); vf[j][1] = bf_hi(u1);
                     }
                 }
@@ -521,20 +526,30 @@ __global__ void __launch_bounds__(kAttnThreads) attn_kernel(AttnArgs a, float sc
             a.out[(static_cast<size_t>(row) * a.H + blockIdx.x * G) * DH + e] = f2bf(0.f);
         return;
     }
-    const int lo = (a.window > 0 && pos - a.window + 1 > 0) ? pos - a.window + 1 : 0;
+    const int lo = (a.window > 0 && pos - a.window + 1 > 0) ? pos - a.window + 1 : 0;  // 0 when paged
     const int L = pos - lo + 1;
-    const size_t cache_base = ((static_cast<size_t>(b) * a.Hkv + g) * a.S + lo) * DH;
-    const __nv_bfloat16* kc = a.kcache + cache_base;
-    const __nv_bfloat16* vc = a.vcache + cache_base;
+    int* pt = reinterpret_cast<int*>(red + kAttnWarps * G * DH);  // [pages of positions lo..pos]
+    bool unmapped = false;
+    for (int j = threadIdx.x; j <= (L - 1) / kKvPage; j += kAttnThreads) {
+        pt[j] = a.kv_page ? a.kv_page[static_cast<size_t>(b) * a.kv_page_ld + j] : j;
+        unmapped |= pt[j] < 0;
+    }
+    const size_t cache_base = a.kv_page ? static_cast<size_t>(g) * kKvPage * DH
+                                        : ((static_cast<size_t>(b) * a.Hkv + g) * a.S + lo) * DH;
+    const size_t page_stride = static_cast<size_t>(a.kv_page ? a.Hkv : 1) * kKvPage * DH;
 
     for (int e = threadIdx.x; e < G * DH; e += kAttnThreads) {
         const int gg = e / DH, d = e - gg * DH;
         qs[e] = bf2f(a.q[(static_cast<size_t>(row) * a.H + g * G + gg) * DH + d]);
     }
-    __syncthreads();
+    if (__syncthreads_or(unmapped)) {  // part of the history is not mapped: attend to nothing, like an idle row
+        for (int e = threadIdx.x; e < G * DH; e += kAttnThreads)
+            a.out[(static_cast<size_t>(row) * a.H + blockIdx.x * G) * DH + e] = f2bf(0.f);
+        return;
+    }
 
-    attend<DH, G>(qs, sc, red, kc, vc, L, lcap, scale, a.bf16_math,
-                  a.out + (static_cast<size_t>(row) * a.H + g * G) * DH);
+    attend<DH, G>(qs, sc, red, a.kcache + cache_base, a.vcache + cache_base, pt, page_stride, L, lcap, scale,
+                  a.bf16_math, a.out + (static_cast<size_t>(row) * a.H + g * G) * DH);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -545,19 +560,34 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
     pdl_launch_dependents();
     const int row = blockIdx.y, g = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // ---- before the qkv GEMM has finished: pull this row's K/V history towards L2.  The cache lines of positions
-    // < pos were written frames ago; the position read here may be one frame stale (it only steers prefetch hints,
-    // the real one is read after the dependency wait).  The scores / values loops then find L2 hits instead of paying
-    // the HBM latency while the next GEMM's weight prefetch keeps the memory queues full. ----
+    extern __shared__ float sm[];
+    float* qs = sm;                      // [G][DH]
+    float* sc = qs + G * DH;             // [G][lcap]
+    float* red = sc + G * lcap;          // [kAttnWarps][G][DH]
+    int* pt = reinterpret_cast<int*>(red + kAttnWarps * G * DH);  // this row's pages (attend()); identity if contiguous
+    // ---- before the qkv GEMM has finished: this row's page-table entries into registers, and its K/V history towards
+    // L2.  The cache lines of positions < pos were written frames ago; the position read here may be one frame stale
+    // (it only steers how many entries are loaded early and the prefetch hints; the real one is read after the
+    // dependency wait, and the page table does not change during a decode call).  The scores / values loops then find
+    // L2 hits instead of paying the HBM latency while the next GEMM's weight prefetch keeps the memory queues full. ----
+    const size_t cache_base = a.kv_page ? static_cast<size_t>(g) * kKvPage * DH
+                                        : (static_cast<size_t>(a.row_seq[row]) * a.Hkv + g) * a.S * DH;
+    const size_t page_stride = static_cast<size_t>(a.kv_page ? a.Hkv : 1) * kKvPage * DH;
+    const int* ptab = a.kv_page ? a.kv_page + static_cast<size_t>(a.row_seq[row]) * a.kv_page_ld : nullptr;
+    const int pp = min(max(a.row_pos[row], 0), a.S - 1);
+    // entry j < npre of the row's page table is held by thread j from here on (one load, off the critical path)
+    const int npre = min(min(pp / kKvPage + 2, (a.S + kKvPage - 1) / kKvPage), kAttnThreads);
+    const int pg_pre = threadIdx.x < npre ? (ptab ? ptab[threadIdx.x] : static_cast<int>(threadIdx.x)) : -1;
     {
-        const int pb = a.row_seq[row];
-        const int pp = min(max(a.row_pos[row], 0), a.S - 1);
         const int n = min(pp + 1, kAttnPrefetchPos);
-        const size_t base = (static_cast<size_t>(pb) * a.Hkv + g) * a.S * DH;
-        const int lines = n * DH * 2 / 128;  // 128-byte lines of K (and as many of V)
+        const int lines = n * DH * 2 / 128;  // 128-byte lines of K (and as many of V); a page is whole lines
+        constexpr int kLinesPerPage = kKvPage * DH * 2 / 128;
         for (int i = threadIdx.x; i < lines; i += kAttnThreads) {
-            prefetch_l2(reinterpret_cast<const char*>(a.kcache + base) + static_cast<size_t>(i) * 128);
-            prefetch_l2(reinterpret_cast<const char*>(a.vcache + base) + static_cast<size_t>(i) * 128);
+            const int pg = ptab ? ptab[i / kLinesPerPage] : i / kLinesPerPage;
+            if (pg < 0) continue;
+            const size_t byte = (cache_base + pg * page_stride) * 2 + static_cast<size_t>(i % kLinesPerPage) * 128;
+            prefetch_l2(reinterpret_cast<const char*>(a.kcache) + byte);
+            prefetch_l2(reinterpret_cast<const char*>(a.vcache) + byte);
         }
     }
     // what the front end needs besides the GEMM result (static data): requested before the wait as well
@@ -577,14 +607,9 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
         normw_r[r] = (nw != nullptr && hh < NH) ? bf2f(nw[d]) : 0.f;
     }
     pdl_wait();
-    extern __shared__ float sm[];
-    float* qs = sm;                      // [G][DH]
-    float* sc = qs + G * DH;             // [G][lcap]
-    float* red = sc + G * lcap;          // [kAttnWarps][G][DH]
     __shared__ float wred[NR][kAttnWarps];
     // ---- finish the qkv GEMM for this row's heads: q heads g*G .. g*G+G-1, then k, then v of KV group g.  The
     // partials are requested before the row's position is looked at (they do not depend on it) ----
-    const int b = a.row_seq[row];
     const int rpos = a.row_pos[row];
     float vsum[NR];
     {
@@ -604,6 +629,12 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
         return;
     }
     const int wpos = min(rpos, a.S - 1);
+    bool unmapped = false;
+    for (int j = threadIdx.x; j <= wpos / kKvPage; j += kAttnThreads) {  // entries the early load did not cover
+        pt[j] = j < npre ? pg_pre : (ptab ? ptab[j] : j);  // j < npre: j == threadIdx.x
+        unmapped |= pt[j] < 0;
+    }
+    if (__syncthreads_or(unmapped)) return;  // unmapped history: nothing is written, nothing attended
     // (cos, sin) of this lane's rotary pair at the row's position: the same for q and k
     const uint32_t cs = *reinterpret_cast<const uint32_t*>(a.freqs + (static_cast<size_t>(wpos) * (DH / 2) + (d >> 1)) * 2);
     // bias, the GEMM output's bf16 rounding, and per-head nn.RMSNorm (fp32 math, weight multiply included, ONE
@@ -651,21 +682,16 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
                 qs[hh * DH + d] = x;
             } else if (rpos < a.S) {
                 __nv_bfloat16* cache = kind == 1 ? a.kcache : a.vcache;
-                cache[((static_cast<size_t>(b) * a.Hkv + g) * a.S + rpos) * DH + d] = f2bf(x);
+                cache[cache_base + pt[rpos / kKvPage] * page_stride + (rpos % kKvPage) * DH + d] = f2bf(x);
             }
         }
     }
     if (a.kv_only) return;
     __syncthreads();  // q in shared memory, this row's new K/V visible to the whole CTA
 
-    const int pos = wpos;
-    const int L = pos + 1;
-    const size_t cache_base = (static_cast<size_t>(b) * a.Hkv + g) * a.S * DH;
-    const __nv_bfloat16* kc = a.kcache + cache_base;
-    const __nv_bfloat16* vc = a.vcache + cache_base;
-
-    attend<DH, G>(qs, sc, red, kc, vc, L, lcap, scale, a.bf16_math,
-                  a.out + (static_cast<size_t>(row) * a.H + g * G) * DH);
+    const int L = wpos + 1;
+    attend<DH, G>(qs, sc, red, a.kcache + cache_base, a.vcache + cache_base, pt, page_stride, L, lcap, scale,
+                  a.bf16_math, a.out + (static_cast<size_t>(row) * a.H + g * G) * DH);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -964,15 +990,20 @@ __global__ void frame_end_kernel(FrameEndArgs a) {
             a.pos[slot] = a.pos[slot] + 1;
     }
 }
-// 16-byte copies of one (layer, KV head) run of n_pos positions per CTA column
-__global__ void kv_copy_kernel(uint4* cache, size_t slot_stride16, size_t head_stride16, size_t layer_stride16, int src,
-                               int dst, int n16) {
+// 16-byte copies of positions [0, n_pos) of one (layer, KV head) per CTA row, page by page
+__global__ void kv_copy_kernel(uint4* cache, size_t layer16, size_t page16, size_t head16, const int* src_tab,
+                               int src0, const int* dst_tab, int dst0, int n16) {
     pdl_launch_dependents();
     pdl_wait();
-    const size_t base = blockIdx.z * layer_stride16 + blockIdx.y * head_stride16;
-    const uint4* s = cache + base + src * slot_stride16;
-    uint4* d = cache + base + dst * slot_stride16;
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n16; e += gridDim.x * blockDim.x) d[e] = s[e];
+    const int per_page = static_cast<int>(head16);  // 16-byte units of one (page, head) block
+    uint4* base = cache + blockIdx.z * layer16 + blockIdx.y * head16;
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n16; e += gridDim.x * blockDim.x) {
+        const int j = e / per_page;
+        const int sp = src_tab ? src_tab[j] : src0 + j, dp = dst_tab ? dst_tab[j] : dst0 + j;
+        if (sp < 0 || dp < 0 || sp == dp) continue;
+        const int w = e - j * per_page;
+        base[dp * page16 + w] = base[sp * page16 + w];
+    }
 }
 
 __global__ void step_inc_kernel(unsigned long long* step) {
@@ -1023,15 +1054,16 @@ static int g_attn_chunk = 0;
 static bool g_attn_per_row = false;  // tests: launch_attn uses the per-row kernel (the decode kernel's attention core)
 void attn_set_score_chunk(int positions) { g_attn_chunk = positions > 0 ? (positions + 31) / 32 * 32 : 0; }
 void attn_force_per_row(bool on) { g_attn_per_row = on; }
+// `pages`: page-table entries of one row kept in shared memory
 template <int DH, int G>
-static size_t attn_smem_bytes(int lcap) {
+static size_t attn_smem_bytes(int lcap, int pages) {
     return (static_cast<size_t>(G) * DH + static_cast<size_t>(G) * lcap + static_cast<size_t>(kAttnWarps) * G * DH) *
-           sizeof(float);
+               sizeof(float) + static_cast<size_t>(pages) * sizeof(int);
 }
 template <int DH, int G>
-static int attn_score_chunk(int need) {
+static int attn_score_chunk(int need, int pages) {
     int lcap = (need + 31) / 32 * 32;
-    const int fit = static_cast<int>((200 * 1024 - attn_smem_bytes<DH, G>(0)) / (sizeof(float) * G)) / 32 * 32;
+    const int fit = static_cast<int>((200 * 1024 - attn_smem_bytes<DH, G>(0, pages)) / (sizeof(float) * G)) / 32 * 32;
     if (lcap > fit) lcap = fit;
     if (g_attn_chunk > 0 && g_attn_chunk < lcap) lcap = g_attn_chunk;
     return lcap;
@@ -1041,8 +1073,9 @@ template <int DH, int G>
 static int launch_attn_t(const AttnArgs& a, cudaStream_t st) {
     int lcap = a.window > 0 && a.window < a.S ? a.window : a.S;
     if (a.lcap > 0 && a.lcap < lcap) lcap = a.lcap;
-    lcap = attn_score_chunk<DH, G>(lcap);
-    const size_t smem = attn_smem_bytes<DH, G>(lcap);
+    const int pages = cdiv(a.S, kKvPage);  // page-table entries of one row (the identity when contiguous)
+    lcap = attn_score_chunk<DH, G>(lcap, pages);
+    const size_t smem = attn_smem_bytes<DH, G>(lcap, pages);
     const float scale = 1.0f / sqrtf(static_cast<float>(DH));
     FSB_LAUNCH((attn_kernel<DH, G>), dim3(a.Hkv, a.rows), dim3(kAttnThreads), smem, st, a, scale, lcap);
     return 0;
@@ -1065,8 +1098,9 @@ template <int DH, int G>
 static int launch_attn_decode_t(const AttnDecodeArgs& a, cudaStream_t st) {
     int lcap = a.S;
     if (a.lcap > 0 && a.lcap < lcap) lcap = a.lcap;
-    lcap = attn_score_chunk<DH, G>(lcap);
-    const size_t smem = attn_smem_bytes<DH, G>(lcap);
+    const int pages = cdiv(a.S, kKvPage);  // page-table entries of one row (the identity when contiguous)
+    lcap = attn_score_chunk<DH, G>(lcap, pages);
+    const size_t smem = attn_smem_bytes<DH, G>(lcap, pages);
     const float scale = 1.0f / sqrtf(static_cast<float>(DH));
     FSB_LAUNCH((attn_decode_kernel<DH, G>), dim3(a.Hkv, a.rows), dim3(kAttnThreads), smem, st, a, scale, lcap);
     return 0;
@@ -1087,6 +1121,7 @@ int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st) {
 
 int launch_attn(const AttnArgs& a, cudaStream_t st) {
     if (a.rows <= 0) return 0;
+    FSB_CHECK(a.kv_page == nullptr || a.window <= 0, "attention: a paged KV cache takes no window");
     // one kernel whatever the number of rows: a sequence must get the same bits alone, in a batch or in pieces
     if (!g_attn_per_row && attn_tile_supported(a)) return launch_attn_tile(a, st);
     const int G = a.H / a.Hkv;
@@ -1116,15 +1151,16 @@ int launch_sample(const SampleArgs& a, cudaStream_t st) {
     return 0;
 }
 
-int launch_kv_copy(__nv_bfloat16* cache, int layers, int slots, int Hkv, int S, int Dh, int src, int dst, int n_pos,
-                   cudaStream_t st) {
-    if (n_pos <= 0 || src == dst) return 0;
-    FSB_CHECK(src >= 0 && src < slots && dst >= 0 && dst < slots && n_pos <= S, "kv_copy: bad slot / length");
+int launch_kv_copy(__nv_bfloat16* cache, int layers, int n_pages, int Hkv, int Dh, const int* src_tab, int src0,
+                   const int* dst_tab, int dst0, int n_pos, cudaStream_t st) {
+    if (n_pos <= 0) return 0;
     FSB_CHECK(Dh % 8 == 0, "kv_copy: head_dim %d", Dh);
-    const size_t head16 = static_cast<size_t>(S) * Dh / 8, slot16 = head16 * Hkv, layer16 = slot16 * slots;
+    FSB_CHECK(src_tab != nullptr || (src0 >= 0 && src0 < n_pages && dst0 >= 0 && dst0 < n_pages && n_pos <= kKvPage),
+              "kv_copy: page %d -> %d (%d positions) outside the pool of %d pages", src0, dst0, n_pos, n_pages);
+    const size_t head16 = static_cast<size_t>(kKvPage) * Dh / 8, page16 = head16 * Hkv, layer16 = page16 * n_pages;
     const int n16 = n_pos * (Dh / 8);
     FSB_LAUNCH(kv_copy_kernel, dim3(cdiv(n16, 256 * 4), Hkv, layers), dim3(256), 0, st,
-               reinterpret_cast<uint4*>(cache), slot16, head16, layer16, src, dst, n16);
+               reinterpret_cast<uint4*>(cache), layer16, page16, head16, src_tab, src0, dst_tab, dst0, n16);
     return 0;
 }
 

@@ -59,8 +59,22 @@ struct ResidNormArgs {
 };
 int launch_resid_norm(const ResidNormArgs& a, cudaStream_t st);
 
+// KV cache addressing. kv_page == nullptr: one contiguous block per sequence, [seqs][Hkv][S][Dh] (codec, fast stack).
+// Otherwise a pool of pages of kKvPage positions, [n_pages][Hkv][kKvPage][Dh], and position p of sequence b lives in
+// page kv_page[b * kv_page_ld + p / kKvPage]; -1 = not mapped, neither read nor written. A page is one K tile of
+// attn_tile.cu and a whole number of attend()'s 32-position score chunks, so the paged walk sums the same terms in the
+// same order as the contiguous one.
+constexpr int kKvPage = 64;
+// Element offset of (sequence b, KV head g, position pos) in one layer's cache, or -1 when its page is not mapped.
+__device__ __forceinline__ long long kv_offset(const int* kv_page, int kv_page_ld, int b, int g, int pos, int Hkv,
+                                               int S, int Dh) {
+    if (kv_page == nullptr) return ((static_cast<long long>(b) * Hkv + g) * S + pos) * Dh;
+    const int pg = kv_page[static_cast<size_t>(b) * kv_page_ld + pos / kKvPage];
+    return pg < 0 ? -1 : ((static_cast<long long>(pg) * Hkv + g) * kKvPage + pos % kKvPage) * Dh;
+}
+
 // q,k,v = rbf(y [+bias]); optional per-head nn.RMSNorm (single rounding); interleaved RoPE in
-// fp32 with bf16 tables; q -> qbuf[row][H][Dh]; k,v -> cache[b][hkv][pos][Dh].
+// fp32 with bf16 tables; q -> qbuf[row][H][Dh]; k,v -> the cache at (row_seq, row_pos) (see kv_offset).
 struct QkvPrepArgs {
     const float* y;  // [rows][ld]
     int ld;
@@ -71,20 +85,25 @@ struct QkvPrepArgs {
     const int* row_seq;          // [rows] cache slot of each row
     const int* row_pos;          // [rows] position of each row
     __nv_bfloat16* q;            // [rows, H, Dh]
-    __nv_bfloat16* kcache;       // [Bslots, Hkv, S, Dh]
+    __nv_bfloat16* kcache;       // one layer's cache (see kv_offset)
     __nv_bfloat16* vcache;
+    const int* kv_page;          // page table or null (contiguous)
+    int kv_page_ld;
     int rows, H, Hkv, Dh, S;
     float eps;
 };
 int launch_qkv_prep(const QkvPrepArgs& a, cudaStream_t st);
 
 // out[row][h][:] = softmax(q.k^T * scale over cache positions [max(0,pos-window+1), pos]) . v
+// A row whose history includes an unmapped page attends to nothing: its output row is zero, as for an idle row.
 // bf16_math = 1 reproduces the fast-AR hand-rolled attention (llama.py:948-976): scores, scaled
 // scores, probabilities and the output are each rounded to bf16.
 struct AttnArgs {
     const __nv_bfloat16* q;  // [rows, H, Dh]
     const __nv_bfloat16* kcache;
     const __nv_bfloat16* vcache;
+    const int* kv_page;  // page table or null (contiguous, see kv_offset); paged caches take no window
+    int kv_page_ld;
     const int* row_seq;
     const int* row_pos;
     __nv_bfloat16* out;  // [rows, H*Dh]
@@ -106,15 +125,17 @@ void attn_force_per_row(bool on);          // tests: launch_attn runs the per-ro
 // GEMM for its own (G + 2) heads -- slot-ordered sum of the stream-K partials, bias, per-head nn.RMSNorm, interleaved
 // RoPE (llama.py:891-908) -- appends K/V to the cache (KVCache.update, llama.py:196-214), then attends over the cache
 // with q still in shared memory. kv_only: stop after the append (fast pass 0 of a frame, inference.py:147).
-// A row parked at position -1 (idle slot) is skipped.
+// A row parked at position -1 (idle slot), or whose pages are not all mapped, is skipped.
 struct AttnDecodeArgs {
     StepPartials qkv;
     const __nv_bfloat16* bias;    // [(H+2Hkv)*Dh] or null
     const __nv_bfloat16* q_norm;  // [Dh] or null
     const __nv_bfloat16* k_norm;
     const __nv_bfloat16* freqs;   // [S, Dh/2, 2] bf16 (cos, sin)
-    __nv_bfloat16* kcache;        // [slots, Hkv, S, Dh]
+    __nv_bfloat16* kcache;        // one layer's cache (see kv_offset)
     __nv_bfloat16* vcache;
+    const int* kv_page;           // page table or null (contiguous)
+    int kv_page_ld;
     const int* row_seq;
     const int* row_pos;
     __nv_bfloat16* out;  // [rows, H*Dh]
@@ -207,9 +228,10 @@ struct FrameEndArgs {
 };
 int launch_frame_end(const FrameEndArgs& a, cudaStream_t st);
 
-// Prefix reuse: cache[layer][dst][g][0..n_pos) = cache[layer][src][g][0..n_pos) for every layer and KV head of one
-// cache tensor laid out [layers][slots][Hkv][S][Dh].
-int launch_kv_copy(__nv_bfloat16* cache, int layers, int slots, int Hkv, int S, int Dh, int src, int dst, int n_pos,
-                   cudaStream_t st);
+// Copy positions [0, n_pos) between pages of a paged cache [layers][n_pages][Hkv][kKvPage][Dh], every layer and KV
+// head. Page j of the run is src_tab[j] / dst_tab[j] when the table is given (a slot's row of the page table), else
+// src0 + j / dst0 + j. Unmapped or identical pages are skipped.
+int launch_kv_copy(__nv_bfloat16* cache, int layers, int n_pages, int Hkv, int Dh, const int* src_tab, int src0,
+                   const int* dst_tab, int dst0, int n_pos, cudaStream_t st);
 
 }  // namespace fsb

@@ -6,6 +6,7 @@ import ctypes as C
 import math
 from typing import Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -61,12 +62,149 @@ def bf16_round(v: float) -> float:
     return float(torch.tensor(v, dtype=torch.bfloat16).float())
 
 
+KV_PAGE = 64  # positions per page of the slow KV cache (include/fishb200.h, fsb_lm_config.kv_pages)
+
+
+def kv_pages_for(n_positions: int) -> int:
+    return -(-int(n_positions) // KV_PAGE)
+
+
+class KvPagePool:
+    """Host side of the paged slow KV cache: which pool page holds each 64-position block of each slot.
+
+    `table[slot, j]` is the page of positions [64 j, 64 j + 64) of the slot, -1 when none is mapped. A page can be
+    mapped by several slots (a shared prompt prefix); `ref[page]` counts them and a page returns to the free list when
+    the count drops to 0. A slot is live (reserved for a request that may still write) or retired: a retired slot keeps
+    its pages mapped, as a prefix later requests may reuse, until an allocation needs them; retired slots are then
+    released least recently retired first, and `on_reclaim(slot)` lets the owner forget what the slot held.
+
+    Device effects are callbacks, so that the rules can run without a GPU: `copy_page(src, dst, n)` copies positions
+    [0, n) of a page, stream-ordered before the writes that follow."""
+
+    def __init__(self, slots: int, pages_per_slot: int, n_pages: int, copy_page=None, on_reclaim=None):
+        if n_pages < 1:
+            raise ValueError(f"kv_pages must be >= 1, got {n_pages}")
+        self.slots, self.pages_per_slot, self.n_pages = slots, pages_per_slot, n_pages
+        self.table = np.full((slots, pages_per_slot), -1, dtype=np.int32)
+        self.ref = np.zeros(n_pages, dtype=np.int32)
+        self.free = list(range(n_pages - 1, -1, -1))  # popped from the end: page 0 first
+        self.retired: dict[int, None] = {s: None for s in range(slots)}  # insertion order = retirement order
+        self.copy_page = copy_page or (lambda src, dst, n: None)
+        self.on_reclaim = on_reclaim or (lambda slot: None)
+        self.dirty = True
+        self.peak = 0
+
+    # ---- queries ------------------------------------------------------------------------------------------------
+    def in_use(self) -> int:
+        return self.n_pages - len(self.free)
+
+    def available(self) -> int:
+        """Pages a reservation can get: free ones plus those that only retired slots map."""
+        live = [s for s in range(self.slots) if s not in self.retired]
+        pages = self.table[live]
+        return self.n_pages - len(np.unique(pages[pages >= 0]))
+
+    # ---- mapping ------------------------------------------------------------------------------------------------
+    def _unmap(self, slot: int, first: int):
+        """Unmap pages first.. of `slot` (a row never maps one page twice)."""
+        row = self.table[slot, first:]
+        pages = row[row >= 0]
+        if len(pages):
+            row[:] = -1
+            self.ref[pages] -= 1
+            self.free.extend(pages[self.ref[pages] == 0].tolist())
+            self.dirty = True
+
+    def release(self, slot: int):
+        """Unmap every page of `slot`."""
+        self._unmap(slot, 0)
+
+    def retire(self, slot: int):
+        """`slot` will not write again until its next reservation; its pages stay mapped until needed."""
+        self.retired.setdefault(slot, None)
+
+    def hold(self, slot: int, end: int, start: int = 0):
+        """Make `slot` live without mapping anything yet, and release its pages past position `end` as well as the
+        pages from `start` on that other slots map too (they would be replaced by pages of their own, nothing kept)."""
+        self.retired.pop(slot, None)
+        n = kv_pages_for(max(int(end), 0))
+        self._unmap(slot, n)
+        row = self.table[slot]
+        for j in range(kv_pages_for(max(int(start), 0)), n):
+            p = int(row[j])
+            if p >= 0 and self.ref[p] > 1:
+                row[j] = -1
+                self.ref[p] -= 1
+                self.dirty = True
+
+    def share(self, dst: int, src: int, n_pages: int):
+        """Map the first `n_pages` pages of `src` into `dst` as well (a shared prompt prefix)."""
+        for j in range(n_pages):
+            p = int(self.table[src, j])
+            if p < 0 or p == self.table[dst, j]:
+                continue
+            old = int(self.table[dst, j])
+            if old >= 0:
+                self.ref[old] -= 1
+                if self.ref[old] == 0:
+                    self.free.append(old)
+            self.table[dst, j] = p
+            self.ref[p] += 1
+            self.dirty = True
+
+    def _take(self) -> int:
+        p = self.free.pop()
+        self.ref[p] = 1
+        self.dirty = True
+        return p
+
+    def reserve(self, slot: int, end: int, start: int = 0):
+        """Make `slot` live with private pages for every position in [start, end) it is about to write, and mapped
+        pages for [0, start). A page overlapping [start, end) that other slots map too is replaced by a private copy of
+        its positions before `start` (copy-on-write). Pages past `end` are released."""
+        end = max(int(end), 0)
+        start = min(max(int(start), 0), end)
+        n = kv_pages_for(end)
+        if n > self.pages_per_slot:
+            raise ValueError(f"{end} positions exceed the slot's KV capacity ({self.pages_per_slot * KV_PAGE})")
+        self.hold(slot, end, start)
+        row = self.table[slot]
+        first = start // KV_PAGE
+        while True:
+            head = row[first:n]
+            cow = (first + np.nonzero((head >= 0) & (self.ref[np.maximum(head, 0)] > 1))[0]).tolist()
+            missing = np.nonzero(row[:n] < 0)[0].tolist()
+            need = len(cow) + len(missing)
+            if len(self.free) >= need:
+                break
+            if not self.retired:
+                raise RuntimeError(
+                    f"KV page pool exhausted: slot {slot} needs {need} more pages of {KV_PAGE} positions for {end} "
+                    f"positions, {len(self.free)} of the pool's {self.n_pages} pages (kv_pages) are free")
+            victim = next(iter(self.retired))
+            del self.retired[victim]
+            self.release(victim)
+            self.on_reclaim(victim)
+        for j in cow:
+            old, new = int(row[j]), self._take()
+            keep = min(max(0, start - j * KV_PAGE), KV_PAGE)
+            if keep:
+                self.copy_page(old, new, keep)
+            self.ref[old] -= 1  # another slot still maps it
+            row[j] = new
+        for j in missing:
+            row[j] = self._take()
+        self.peak = max(self.peak, self.in_use())
+
+
 class LmEngine:
     """One model replica on one GPU: weights (bf16, device), KV caches and workspaces (library-owned)."""
 
     def __init__(self, config, state_dict: dict, device, im_end_id: int, max_batch: int = 1,
                  kv_len: Optional[int] = None, max_rows: int = 2048, max_frames: Optional[int] = None,
-                 debug: bool = False):
+                 debug: bool = False, kv_pages: Optional[int] = None):
+        """`kv_len`: KV positions one sequence can hold. `kv_pages`: size of the slow KV cache's page pool (pages of
+        64 positions); None = room for every slot at full capacity, so that no reservation can fail."""
         if not torch.cuda.is_available():
             raise _lib.FsbError("fish_speech_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.lib = _lib.lib()
@@ -142,6 +280,8 @@ class LmEngine:
         K.scale_codebook_embeddings = int(c.scale_codebook_embeddings)
         K.norm_fastlayer_input = int(getattr(c, "norm_fastlayer_input", False))
         K.max_batch, K.kv_len, K.max_rows, K.max_frames, K.debug = max_batch, kv_len, max_rows, max_frames, int(debug)
+        pages_per_slot = kv_pages_for(kv_len)
+        K.kv_pages = int(kv_pages) if kv_pages else max_batch * pages_per_slot
         self._K, self._W = K, W
         h = C.c_void_p()
         with torch.cuda.device(self.device):
@@ -154,6 +294,10 @@ class LmEngine:
         self._slot_tokens: dict = {}  # slot -> token rows [C+1, T] (CPU int32) whose K/V positions [0, T) are valid
         self.rows_reused = 0
         self.rows_prefilled = 0
+        self.kv_pool = KvPagePool(max_batch, pages_per_slot, K.kv_pages, copy_page=self._copy_page,
+                                  on_reclaim=self._forget_slot)
+        self._wfrom: dict = {}  # slot -> lowest position the next decode frames write (copy-on-write bound)
+        self._covered: dict = {}  # slot -> pages [0, n) its last reservation mapped (decode skips what is covered)
 
     def close(self):
         if getattr(self, "h", None):
@@ -189,6 +333,7 @@ class LmEngine:
             "slot_top_p": ((self.max_batch,), "<f4"),
             "slot_top_k": ((self.max_batch,), "<i4"),
             "slot_seed": ((self.max_batch,), "<i8"),
+            "kv_page": ((self.max_batch, self.kv_pool.pages_per_slot), "<i4"),
             "slow_logits": ((self.max_batch, self.head_rows), "<f4"),
             "fast_logits": ((c.num_codebooks, self.max_batch, c.codebook_size), "<f4"),
             # decode state (include/fishb200.h fsb_lm_test_layer_gemms), row_tile rows; "attn" / "ffn_h" are flat:
@@ -246,14 +391,88 @@ class LmEngine:
         self._noise = u
         _lib.check(self.lib.fsb_lm_set_sampler_noise(self.h, u.data_ptr(), u.shape[1], u.shape[2]))
 
+    # ---- paged slow KV cache (KvPagePool) --------------------------------------------------------------------------
+    def _forget_slot(self, slot: int):
+        """The pool reclaimed the slot's pages: its prefix record and reservation are gone."""
+        self._slot_tokens.pop(slot, None)
+        self._covered.pop(slot, None)
+
+    def _copy_page(self, src: int, dst: int, n: int):
+        _lib.check(self.lib.fsb_lm_copy_kv_page(self.h, src, dst, n, _stream()))
+
+    def _reserve(self, items):
+        """items: (slot, end, start) -- map pages for positions [0, end) of each slot, private from `start` on. Every
+        slot is first made live and trimmed to its end, so that none of them is reclaimed for another; the page table
+        then reaches the device with one stream-ordered copy."""
+        pool = self.kv_pool
+        with torch.cuda.device(self.device):
+            for s, end, start in items:
+                pool.hold(int(s), end, start)
+            for s, end, start in items:
+                pool.reserve(int(s), end, start)
+                self._covered[int(s)] = kv_pages_for(end)
+            if pool.dirty:
+                table = torch.from_numpy(pool.table.copy()).pin_memory()
+                self.buffer("kv_page").copy_(table, non_blocking=True)
+                pool.dirty = False
+
+    def reserve(self, slot: int, n_positions: int, start: int = 0):
+        """Pages for every position < n_positions of `slot`, before it writes [start, n_positions): for callers that
+        decode at explicit positions (decode_one_token_ar / decode_n_tokens)."""
+        n_positions = min(int(n_positions), self.kv_len)
+        self._reserve([(slot, n_positions, start)])
+        self._wfrom[int(slot)] = int(start)
+
+    def retire_slot(self, slot: int):
+        """The slot's request is done: its pages stay mapped as a reusable prefix until the pool needs them."""
+        self.kv_pool.retire(int(slot))
+
+    def release_kv(self):
+        """Forget every slot's K/V: all pages return to the pool."""
+        self._slot_tokens.clear()
+        self._covered.clear()
+        for s in range(self.max_batch):
+            self.kv_pool.release(s)
+            self.kv_pool.retire(s)
+        self._reserve([])
+
+    def _donor(self, prompt: torch.Tensor, slot: int, busy) -> tuple[int, int]:
+        """(rows, slot) of the longest prefix of `prompt` whose K/V a slot holds: its own, or one not in `busy`."""
+        best, donor = 0, slot
+        for d, toks in self._slot_tokens.items():
+            if d != slot and d in busy:
+                continue
+            n = self._common_prefix(prompt, toks)
+            if n > best:
+                best, donor = n, d
+        best = min(best, prompt.shape[1] - 1)  # at least the last row is computed: its logits are sampled
+        return (best, donor) if best >= self.MIN_REUSE else (0, slot)
+
+    def kv_pages_needed(self, prompt: torch.Tensor, n_positions: int, slot: int, busy=(), reuse: bool = False) -> int:
+        """Pages a request in `slot` adds to those live slots map: all of [0, n_positions), less the whole pages of a
+        prefix it shares with a live slot (prefill_reusing). `prompt`: the request's token rows on the host."""
+        need = kv_pages_for(min(int(n_positions), self.kv_len))
+        if reuse:
+            best, donor = self._donor(prompt, int(slot), set(busy) | {int(slot)})
+            if donor != slot and donor not in self.kv_pool.retired:
+                need -= best // KV_PAGE
+        return need
+
+    def kv_pages_available(self) -> int:
+        return self.kv_pool.available()
+
     def reset(self):
+        for s in range(self.max_batch):
+            self.kv_pool.retire(s)  # their K/V stays mapped for prefix reuse until the pool needs the pages
         self._ctx_bound = 0
         with torch.cuda.device(self.device):
             _lib.check(self.lib.fsb_lm_reset(self.h, _stream()))
 
     def prefill(self, prompts: Sequence[torch.Tensor], slots: Sequence[int], sp: Optional[_lib.Sampling],
-                start_pos: Optional[Sequence[int]] = None, do_sample: bool = True) -> None:
-        """prompts[k]: integer tensor [C+1, T_k] (row 0 token ids, rows 1..C codes) for slot slots[k]."""
+                start_pos: Optional[Sequence[int]] = None, do_sample: bool = True,
+                kv_end: Optional[Sequence[int]] = None) -> None:
+        """prompts[k]: integer tensor [C+1, T_k] (row 0 token ids, rows 1..C codes) for slot slots[k]. `kv_end[k]`:
+        reserve KV pages up to that position (prompt + frames to come) instead of the prompt alone."""
         C1 = self.cfg.num_codebooks + 1
         start_pos = list(start_pos) if start_pos is not None else [0] * len(prompts)
         for p, s0 in zip(prompts, start_pos):
@@ -283,6 +502,12 @@ class LmEngine:
         for k, s0 in enumerate(start_pos):
             if s0 == 0:
                 self._slot_tokens.pop(int(slots[k]), None)  # overwritten from position 0: the old record is void
+        ends = [s0 + p.shape[1] for p, s0 in zip(prompts, start_pos)]
+        if kv_end is not None:
+            ends = [max(e, min(int(k), self.kv_len)) for e, k in zip(ends, kv_end)]
+        self._reserve([(int(s), e, s0) for s, e, s0 in zip(slots, ends, start_pos)])
+        for p, s, s0 in zip(prompts, slots, start_pos):
+            self._wfrom[int(s)] = s0 + p.shape[1]
         self._grow_bound(max(s0 + p.shape[1] for p, s0 in zip(prompts, start_pos)) + 1)
         with torch.cuda.device(dev):
             for grp in groups:
@@ -322,35 +547,30 @@ class LmEngine:
         return int(diff[0]) if len(diff) else n
 
     def prefill_reusing(self, prompts: Sequence[torch.Tensor], slots: Sequence[int], sp: Optional[_lib.Sampling],
-                        do_sample: bool = True) -> list[int]:
+                        do_sample: bool = True, kv_end: Optional[Sequence[int]] = None) -> list[int]:
         """`prefill` of full prompts that skips every row whose K/V the cache already holds: the longest prefix
         a prompt shares with what its own slot was last prefilled with, or with another slot that is not being
-        re-prefilled in this call (copied over with fsb_lm_copy_kv). The reference re-prefills the whole growing
-        conversation for every chunk of `generate_long` (inference.py:611-721); prefill is row-independent, so
-        the reused K/V is bit-identical to what a full prefill would write. Returns the reused length per prompt."""
+        re-prefilled in this call (its whole pages are mapped by reference; a partly shared last page is copied).
+        The reference re-prefills the whole growing conversation for every chunk of `generate_long`
+        (inference.py:611-721); prefill is row-independent, so the reused K/V is bit-identical to what a full
+        prefill would write. Returns the reused length per prompt."""
         host = [p.detach().to("cpu", torch.int32) for p in prompts]
         busy = set(int(s) for s in slots)
-        reused, pieces, starts = [], [], []
-        with torch.cuda.device(self.device):
-            for p, s in zip(host, slots):
-                s = int(s)
-                best, donor = 0, s
-                for d, toks in self._slot_tokens.items():
-                    if d != s and d in busy:
-                        continue
-                    n = self._common_prefix(p, toks)
-                    if n > best:
-                        best, donor = n, d
-                best = min(best, p.shape[1] - 1)  # at least the last row is computed: its logits are sampled
-                if best < self.MIN_REUSE:
-                    best = 0
-                elif donor != s:
-                    _lib.check(self.lib.fsb_lm_copy_kv(self.h, donor, s, best, _stream()))
-                reused.append(best)
-                starts.append(best)
-            for p, b in zip(prompts, reused):
-                pieces.append(p[:, b:])
-        self.prefill(pieces, slots, sp, start_pos=starts, do_sample=do_sample)
+        ends = [p.shape[1] if kv_end is None else max(p.shape[1], min(int(e), self.kv_len))
+                for p, e in zip(host, kv_end if kv_end is not None else host)]
+        for s, e in zip(slots, ends):
+            self.kv_pool.hold(int(s), e, e)  # no slot of this call is reclaimed for another
+        reused, pieces = [], []
+        for p, s in zip(host, slots):  # every prefix is mapped before any page is allocated: the pages the slots
+            s = int(s)                 # held before (maybe shared among them) are released first
+            best, donor = self._donor(p, s, busy)
+            if donor != s:
+                self.kv_pool.share(s, donor, kv_pages_for(best))
+            reused.append(best)
+        self._reserve([(int(s), e, b) for s, e, b in zip(slots, ends, reused)])
+        for p, b in zip(prompts, reused):
+            pieces.append(p[:, b:])
+        self.prefill(pieces, slots, sp, start_pos=reused, do_sample=do_sample, kv_end=ends)
         for p, s in zip(host, slots):
             self._slot_tokens[int(s)] = p
         self.rows_reused += sum(reused)
@@ -358,9 +578,17 @@ class LmEngine:
         return reused
 
     def decode(self, batch: int, nframes: int, sp: Optional[_lib.Sampling], use_graph: bool = True) -> None:
+        """Under slot control the scheduler reserved every request's pages at admission; otherwise the frames'
+        positions are reserved here, before the call."""
         if not self.slot_control and self._ctx_bound - 1 + nframes > self.kv_len:
             raise ValueError(f"decode: {nframes} more frames from position {self._ctx_bound - 1} run past the KV "
                              f"cache ({self.kv_len} positions)")
+        if not self.slot_control:
+            end = self._ctx_bound - 1 + nframes
+            n = kv_pages_for(min(end, self.kv_len))
+            retired = self.kv_pool.retired
+            if any(self._covered.get(s, -1) < n or s in retired for s in range(batch)):  # new pages every 64 frames
+                self._reserve([(s, end, self._wfrom.get(s, 0)) for s in range(batch)])
         self._grow_bound(self._ctx_bound + nframes)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.fsb_lm_decode(self.h, batch, nframes, C.byref(sp) if sp is not None else None,

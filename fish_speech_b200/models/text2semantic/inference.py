@@ -23,7 +23,7 @@ from typing import Callable, Literal, Optional, Sequence, Union
 import numpy as np
 import torch
 
-from ...engine import MAX_DECODE_BATCH
+from ...engine import KV_PAGE, MAX_DECODE_BATCH
 from .llama import IM_END_TOKEN, DualARTransformer
 
 try:  # loguru is what the reference logs with; fall back to stdlib logging if absent
@@ -84,6 +84,7 @@ def decode_one_token_ar(
             raise ValueError(f"input_pos {p0} is outside the KV cache ({eng.kv_len} positions)")
         eng.buffer("cur_tok")[0].copy_(x[0, :, 0].to(torch.int32))
         eng.buffer("pos")[0:1].copy_(input_pos.to(torch.int32).view(1))
+        eng.reserve(0, p0 + 1, start=p0)
         eng.set_context_bound(p0 + 1)
         win = eng.buffer("ras_window")
         if previous_tokens is not None:
@@ -120,6 +121,7 @@ def decode_n_tokens(
     eng.buffer("finished").zero_()
     eng.buffer("ras_window").zero_()
     start = int(input_pos.view(-1)[0].item())
+    eng.reserve(0, start + 1, start=start)
     eng.set_context_bound(start + 1)
     num_new_tokens = min(int(num_new_tokens), eng.max_frames, eng.kv_len - start)  # never write past the KV cache
     n = _run_frames(eng, 1, num_new_tokens, sp, first_frame_from_prefill=False)[0]
@@ -605,6 +607,24 @@ def check_serve_kv_fits(slots: int, kv_len: int, config, free_bytes: int) -> Non
                          f"{fit} fits) or FSB_SERVE_SLOTS")
 
 
+def kv_page_bytes(config) -> int:
+    """Bytes of one page of the slow KV cache: 64 positions of every slow layer, K and V (9.44 MB at S2-Pro)."""
+    return KV_PAGE * slow_kv_bytes_per_position(config)
+
+
+def serve_kv_pool_pages(gb: float, config, free_bytes: int) -> int:
+    """Pages in a slow KV pool of `gb` GB (FSB_SERVE_KV_GB); a ValueError naming FSB_SERVE_KV_GB when that pool
+    does not fit in `free_bytes` of device memory or holds no page."""
+    pages = int(float(gb) * 1e9 // kv_page_bytes(config))
+    if pages < 1:
+        raise ValueError(f"FSB_SERVE_KV_GB={gb} is smaller than one KV page ({kv_page_bytes(config) / 1e9:.3f} GB)")
+    need = pages * kv_page_bytes(config)
+    if need > free_bytes:
+        raise ValueError(f"FSB_SERVE_KV_GB={gb}: a pool of {pages} KV pages needs {need / 1e9:.1f} GB, but only "
+                         f"{free_bytes / 1e9:.1f} GB of device memory is free: lower FSB_SERVE_KV_GB")
+    return pages
+
+
 def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool = False):
     """inference.py:736-799: the model lives in ONE daemon worker thread fed by a queue; `None` shuts
     it down; errors are returned as WrappedGenerateResponse(status="error", response=exc).
@@ -612,7 +632,10 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
     FSB_SERVE_SLOTS=n (2..64) makes the worker a slot scheduler that runs up to n requests concurrently
     (`serve_requests`), each with a KV cache of FSB_SERVE_KV_LEN positions (default 8192; a slot costs
     147 456 B per position at the S2-Pro geometry). Unset / 1: the reference's one-at-a-time loop. If the slots'
-    KV caches do not fit in free device memory, this raises a ValueError naming FSB_SERVE_KV_LEN."""
+    KV caches do not fit in free device memory, this raises a ValueError naming FSB_SERVE_KV_LEN.
+    FSB_SERVE_KV_GB=g (with FSB_SERVE_SLOTS > 1) instead gives the slots one shared pool of g GB of KV pages, each
+    slot a capacity of FSB_SERVE_KV_LEN (default: the model's max_seq_len) positions, and a request is admitted when
+    its pages fit; a pool that does not fit in free device memory raises a ValueError naming FSB_SERVE_KV_GB."""
     input_queue = queue.Queue()
     init_event = threading.Event()
     init_error: list = []
@@ -621,11 +644,19 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
     def worker():
         model, decode_one_token = init_model(checkpoint_path, device, precision, compile=compile)
         if slots > 1:
-            kv = min(int(os.environ.get("FSB_SERVE_KV_LEN", "8192")), model.config.max_seq_len)
+            gb = os.environ.get("FSB_SERVE_KV_GB")
+            default_kv = str(model.config.max_seq_len) if gb else "8192"
+            kv = min(int(os.environ.get("FSB_SERVE_KV_LEN", default_kv)), model.config.max_seq_len)
             try:
-                if torch.device(device).type == "cuda":
-                    check_serve_kv_fits(slots, kv, model.config, torch.cuda.mem_get_info(torch.device(device))[0])
-                model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype)
+                cuda = torch.device(device).type == "cuda"
+                if gb:
+                    free = torch.cuda.mem_get_info(torch.device(device))[0] if cuda else float("inf")
+                    pages = serve_kv_pool_pages(float(gb), model.config, free)
+                    model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype, kv_pages=pages)
+                else:
+                    if cuda:
+                        check_serve_kv_fits(slots, kv, model.config, torch.cuda.mem_get_info(torch.device(device))[0])
+                    model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype)
             except Exception as e:
                 init_error.append(e)
                 init_event.set()

@@ -208,6 +208,7 @@ class DualARTransformer:
         self.engine: Optional[LmEngine] = None
         self.max_batch_size = -1
         self.max_seq_len = -1
+        self.kv_pages: Optional[int] = None
         self._cache_setup_done = False
         self.debug = False
         self.max_rows = 2048
@@ -228,17 +229,21 @@ class DualARTransformer:
             self.device = torch.device(device)
         return self
 
-    def setup_caches(self, max_batch_size: int, max_seq_len: int, dtype: torch.dtype = torch.bfloat16):
-        """llama.py:307-325 — (re)create the engine when more capacity is asked for."""
-        if self.max_seq_len >= max_seq_len and self.max_batch_size >= max_batch_size:
+    def setup_caches(self, max_batch_size: int, max_seq_len: int, dtype: torch.dtype = torch.bfloat16,
+                     kv_pages: Optional[int] = None):
+        """llama.py:307-325 — (re)create the engine when more capacity is asked for. `kv_pages`: the slow KV
+        cache's page pool (64 positions per page) when it should be smaller than every slot at full capacity."""
+        if (self.max_seq_len >= max_seq_len and self.max_batch_size >= max_batch_size
+                and kv_pages == self.kv_pages):
             return
         max_seq_len = find_multiple(max_seq_len, 8)
         if self.engine is not None:
             self.engine.close()
         im_end = self.tokenizer.get_token_id(IM_END_TOKEN)
         self.engine = LmEngine(self.config, self._state, self.device, im_end, max_batch=max_batch_size,
-                               kv_len=max_seq_len, max_rows=self.max_rows, debug=self.debug)
+                               kv_len=max_seq_len, max_rows=self.max_rows, debug=self.debug, kv_pages=kv_pages)
         self.max_seq_len = max_seq_len
+        self.kv_pages = kv_pages
         self.max_batch_size = max_batch_size
 
     @staticmethod

@@ -16,7 +16,7 @@ from typing import Callable, Optional
 
 import torch
 
-from .engine import MAX_DECODE_BATCH, bf16_round
+from .engine import MAX_DECODE_BATCH, bf16_round, kv_pages_for
 
 
 @dataclass(eq=False)  # identity semantics: requests hold tensors
@@ -42,6 +42,7 @@ class SlotRequest:
     slot: int = -1
     _limit: int = 0
     _emitted: int = 0
+    _host_prompt: Optional[torch.Tensor] = None  # the prompt on the host, for page-limited admission with reuse
 
 
 class ContinuousBatcher:
@@ -68,6 +69,8 @@ class ContinuousBatcher:
         eng = self.eng
         eng.reset()
         getattr(eng, "_slot_tokens", {}).clear()  # idle rows of the frames below write position 0 of unused slots
+        if hasattr(eng, "release_kv"):
+            eng.release_kv()  # paged KV: unused slots map no page, so those writes go nowhere
         eng.set_slot_control(True)
         self._state = eng.buffer("slot_state")
         self._limit = eng.buffer("slot_limit")
@@ -111,6 +114,10 @@ class ContinuousBatcher:
         n = min(n, cfg.max_seq_len - T, self.eng.max_frames, self.eng.kv_len - T)
         if n < 1:
             raise ValueError("no room for new tokens")
+        pool = getattr(self.eng, "kv_pool", None)
+        if pool is not None and kv_pages_for(T + n) > pool.n_pages:
+            raise ValueError(f"{T} prompt rows + {n} frames need {kv_pages_for(T + n)} KV pages, more than the "
+                             f"engine's whole pool of {pool.n_pages} (kv_pages)")
         req._limit = n
         self.waiting.append(req)
         return req
@@ -126,16 +133,32 @@ class ContinuousBatcher:
             return
         batch, slots = [], []
         budget = self.eng.max_rows  # one prefill pass worth of rows per step keeps decode latency bounded
+        pool = getattr(self.eng, "kv_pool", None)
+        # a pool with room for every slot at full capacity never runs out: no page accounting needed
+        paged = pool is not None and pool.n_pages < pool.slots * pool.pages_per_slot
+        pages = self.eng.kv_pages_available() if paged else 0
         while free and self.waiting:
-            T = int(self.waiting[0].prompt.size(1))
+            head = self.waiting[0]
+            T = int(head.prompt.size(1))
             if batch and T > budget:
                 break
+            if paged:
+                # FIFO: the head of the queue waits until its pages fit, and nothing overtakes it
+                if head.reuse_prefix and head._host_prompt is None:  # one device -> host copy per request
+                    head._host_prompt = head.prompt.detach().to("cpu", torch.int32)
+                need = self.eng.kv_pages_needed(head._host_prompt, T + head._limit, free[0], busy=slots,
+                                                reuse=head.reuse_prefix)
+                if need > pages:
+                    break
+                pages -= need
             req = self.waiting.pop(0)
             s = free.pop(0)
             req.slot = s
             batch.append(req)
             slots.append(s)
             budget -= T
+        if not batch:
+            return
         idx = torch.tensor(slots, dtype=torch.long, device=self._state.device)
 
         def put(buf, vals, dtype):
@@ -153,10 +176,12 @@ class ContinuousBatcher:
             self.active[r.slot] = r
             self._len[r.slot] = int(r.prompt.size(1)) + 1
         self.eng.set_context_bound_exact(max(self._len.values()) + 1)
+        # paged KV: every request's pages (prompt + budget) are reserved before its prefill
+        kw = dict(kv_end=[int(r.prompt.size(1)) + r._limit for r in batch]) if pool is not None else {}
         if any(r.reuse_prefix for r in batch) and hasattr(self.eng, "prefill_reusing"):
-            self.eng.prefill_reusing([r.prompt for r in batch], slots, None, do_sample=True)
+            self.eng.prefill_reusing([r.prompt for r in batch], slots, None, do_sample=True, **kw)
         else:
-            self.eng.prefill([r.prompt for r in batch], slots, None, do_sample=True)
+            self.eng.prefill([r.prompt for r in batch], slots, None, do_sample=True, **kw)
 
     def _retire(self) -> list[SlotRequest]:
         st = torch.stack([self._state.to(torch.int32), self._n_out]).cpu()  # one small D2H copy (synchronises)
@@ -184,6 +209,9 @@ class ContinuousBatcher:
             self._state[idx] = 0
             self._pos[idx] = -1  # parked: the decode frames neither attend for this row nor touch its K/V (which a
             #                      later request with the same prompt prefix may reuse)
+            for r in finished:
+                if hasattr(self.eng, "retire_slot"):
+                    self.eng.retire_slot(r.slot)  # its pages stay a reusable prefix until the pool needs them
         for req in finished:
             req.done.set()
             if req.on_done is not None:

@@ -54,10 +54,15 @@ typedef struct {
     int norm_fastlayer_input;            /* llama.py:459-461 */
     int max_batch;                       /* resident sequences ("slots"), <= 64; above 32 the decode step runs
                                             its 64-row tile (RT = 64), else the 32-row one (RT = 32) */
-    int kv_len;                          /* KV-cache positions per sequence */
+    int kv_len;                          /* KV-cache positions per sequence (its capacity) */
     int max_rows;                        /* token rows per prefill pass */
     int max_frames;                      /* generated frames kept per sequence */
     int debug;                           /* keep logits / per-layer activations for tests */
+    int kv_pages;                        /* slow KV cache pool, in pages of 64 positions (every slow layer, K and V:
+                                            64 x 2 x n_layer x n_kv_head x head_dim x 2 B); 0 = max_batch x
+                                            ceil(kv_len / 64), room for every slot at full capacity. Sequences map
+                                            pages through the "kv_page" table (fsb_lm_buffer), which the caller
+                                            fills: a position whose page is not mapped is neither written nor read */
 } fsb_lm_config;
 
 /* One TransformerBlock (llama.py:831-987). bf16, row-major [out_features, in_features]. */
@@ -131,6 +136,15 @@ int fsb_lm_decode(fsb_lm* h, int batch, int nframes, const fsb_sampling* s, int 
  * prompt with another slot. Prefill is row-independent, so reused K/V is bit-identical to recomputed K/V. */
 int fsb_lm_copy_kv(fsb_lm* h, int src_slot, int dst_slot, int n_pos, void* stream);
 
+/* With the paged slow cache (fsb_lm_config.kv_pages), fsb_lm_copy_kv copies page by page through the "kv_page" table:
+ * dst_slot must already map pages of its own (mapped by no other slot) for positions [0, n_pos). A block whose source
+ * or destination page is not mapped is skipped; a page both slots map is left as it is. */
+
+/* Copy-on-write of a partly shared page: positions [0, n_pos) (n_pos <= 64) of page `src_page` into page `dst_page`,
+ * every slow layer, K and V. fsb_lm_copy_kv above copies through the page table the same way, page by page; both
+ * are stream-ordered with the prefill / decode calls. */
+int fsb_lm_copy_kv_page(fsb_lm* h, int src_page, int dst_page, int n_pos, void* stream);
+
 /* Upper bound of (position + 1) over all slots for the calls that follow (prompt length + frames decoded so
  * far). Sizes the attention score buffer; must be set before prefill / decode whenever it grows. */
 int fsb_lm_set_context_bound(fsb_lm* h, int max_positions);
@@ -155,7 +169,9 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
 /* Named device buffers of the handle, for reading results and for tests:
  *   "out_tokens" int32 [max_batch][C+1][max_frames], "n_out" int32 [max_batch], "pos" int32 [RT],
  *   "finished" int32 [max_batch], "cur_tok" int32 [max_batch][C+1], "ras_window" int32 [max_batch][10],
- *   the slot-control arrays listed at fsb_lm_set_slot_control,
+ *   the slot-control arrays listed at fsb_lm_set_slot_control, "kv_page" int32 [max_batch][ceil(kv_len / 64)]
+ *   (page of each 64-position block of each slot, -1 = not mapped; read by the kernels at run time, so a captured
+ *   decode graph stays valid when the caller remaps pages between calls),
  *   debug only: "slow_logits" f32 [max_batch][head_rows], "fast_logits" f32 [C][max_batch][codebook_size];
  *   the decode state (for fsb_lm_test_layer_gemms), RT = the decode row tile (32 for max_batch <= 32, else 64):
  *   "x_slow" / "x_fast" bf16 [RT][dim] / [RT][fast_dim] residual streams, "ssq_slow" / "ssq_fast" f32 [RT][32] their

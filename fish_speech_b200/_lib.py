@@ -106,6 +106,7 @@ def lib() -> C.CDLL:
     L.fsb_op_step_gemm.argtypes = [vp, i32, i32, vp, i32, vp, vp, C.c_float, i32, i32, vp, i32p, vp]
     L.fsb_op_step_gemm_tile.argtypes = [vp, i32, i32, vp, i32, i32, vp, vp, C.c_float, i32, i32, vp, i32p, vp]
     L.fsb_lm_test_layer_gemms.argtypes = [vp, i32, i32, i32, i32, vp]
+    L.fsb_lm_test_layer_attn.argtypes = [vp, i32, i32, i32, i32, vp]
     _lib = L
     return L
 

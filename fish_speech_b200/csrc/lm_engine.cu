@@ -222,37 +222,44 @@ int launch_step(const StepGemmPlan& plan, int rows, cudaStream_t st, bool finali
     return finalize_only ? 0 : step_gemm_launch(q, st);
 }
 
+// Arguments of layer l's decode attention over `rows` batch rows, the consumer of the qkv GEMM `qkv` ran: one place
+// for run_stack_decode and fsb_lm_test_layer_attn, so that the test hook launches exactly what decode launches.
+AttnDecodeArgs decode_attn_args(const fsb_lm* h, const Stack& s, int l, const StepGemmPlan& qkv, int rows,
+                                const int* row_seq, const int* row_pos, bool kv_only) {
+    const LayerW& w = s.w[l];
+    AttnDecodeArgs aa{};
+    aa.qkv = step_plan_partials(qkv);
+    aa.bias = w.bqkv;
+    aa.q_norm = s.qk_norm ? w.q_norm : nullptr;
+    aa.k_norm = s.qk_norm ? w.k_norm : nullptr;
+    aa.freqs = s.freqs;
+    aa.kcache = s.kcache + l * s.cache_layer_stride;
+    aa.vcache = s.vcache + l * s.cache_layer_stride;
+    aa.kv_page = s.kv_page;
+    aa.kv_page_ld = s.kv_page_ld;
+    aa.row_seq = row_seq;
+    aa.row_pos = row_pos;
+    aa.out = h->attn_d;
+    aa.rows = rows; aa.H = s.H; aa.Hkv = s.Hkv; aa.Dh = s.Dh; aa.S = s.S;
+    aa.lcap = (s.bf16_math == 0) ? h->ctx_lcap : 0;  // slow stack: bounded by the live context, not the capacity
+    aa.bf16_math = s.bf16_math;
+    aa.kv_only = kv_only ? 1 : 0;
+    aa.eps = h->cfg.norm_eps;
+    return aa;
+}
+
 // ---- decode: one transformer stack over the batch rows, five kernels per layer. `first_qkv`: the plan of layer 0's
 // qkv GEMM when its operand is produced by a GEMM (fast_project_in) instead of a row kernel. After the last layer the
 // residual stream is complete only once the NEXT step GEMM (head / fast_output) has run its prologue. ----
 int run_stack_decode(fsb_lm* h, Stack& s, int rows, const int* row_seq, const int* row_pos, bool stop_after_kv,
                      cudaStream_t st, const StepGemmPlan* first_qkv = nullptr) {
-    const float eps = h->cfg.norm_eps;
     for (int l = 0; l < s.nl; ++l) {
         StepLayer& P = s.dec[l];
-        const LayerW& w = s.w[l];
         const StepGemmPlan& qkv = (l == 0 && first_qkv) ? *first_qkv : P.qkv;
         FSB_TRY(launch_step(qkv, rows, st));
-        AttnDecodeArgs aa{};
-        aa.qkv = step_plan_partials(qkv);
-        aa.bias = w.bqkv;
-        aa.q_norm = s.qk_norm ? w.q_norm : nullptr;
-        aa.k_norm = s.qk_norm ? w.k_norm : nullptr;
-        aa.freqs = s.freqs;
-        aa.kcache = s.kcache + l * s.cache_layer_stride;
-        aa.vcache = s.vcache + l * s.cache_layer_stride;
-        aa.kv_page = s.kv_page;
-        aa.kv_page_ld = s.kv_page_ld;
-        aa.row_seq = row_seq;
-        aa.row_pos = row_pos;
-        aa.out = h->attn_d;
-        aa.rows = rows; aa.H = s.H; aa.Hkv = s.Hkv; aa.Dh = s.Dh; aa.S = s.S;
-        aa.lcap = (s.bf16_math == 0) ? h->ctx_lcap : 0;  // slow stack: bounded by the live context, not the capacity
-        aa.bf16_math = s.bf16_math;
-        aa.kv_only = (stop_after_kv && l == s.nl - 1) ? 1 : 0;  // fast pass 0 only fills the KV cache (inference.py:147)
-        aa.eps = eps;
-        FSB_TRY(launch_attn_decode(aa, st));
-        if (aa.kv_only) return 0;
+        const bool kv_only = stop_after_kv && l == s.nl - 1;  // fast pass 0 only fills the KV cache (inference.py:147)
+        FSB_TRY(launch_attn_decode(decode_attn_args(h, s, l, qkv, rows, row_seq, row_pos, kv_only), st));
+        if (kv_only) return 0;
         FSB_TRY(launch_step(P.wo, rows, st));
         FSB_TRY(launch_step(P.w13, rows, st));
         FSB_TRY(launch_step(P.w2, rows, st));
@@ -558,10 +565,10 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     s.n_pages = cfg->kv_pages > 0 ? cfg->kv_pages : cfg->max_batch * s.kv_page_ld;
     s.cache_layer_stride = static_cast<size_t>(s.n_pages) * s.Hkv * kKvPage * s.Dh;
     f.cache_layer_stride = static_cast<size_t>(cfg->max_batch) * f.Hkv * f.S * f.Dh;
-    TRYC(dalloc(h, &s.kcache, s.cache_layer_stride * s.nl));
-    TRYC(dalloc(h, &s.vcache, s.cache_layer_stride * s.nl));
-    TRYC(dalloc(h, &f.kcache, f.cache_layer_stride * f.nl));
-    TRYC(dalloc(h, &f.vcache, f.cache_layer_stride * f.nl));
+    TRYC(dalloc(h, &s.kcache, s.cache_layer_stride * s.nl, "k_slow"));
+    TRYC(dalloc(h, &s.vcache, s.cache_layer_stride * s.nl, "v_slow"));
+    TRYC(dalloc(h, &f.kcache, f.cache_layer_stride * f.nl, "k_fast"));
+    TRYC(dalloc(h, &f.vcache, f.cache_layer_stride * f.nl, "v_fast"));
     TRYC(dalloc(h, &s.kv_page, static_cast<size_t>(cfg->max_batch) * s.kv_page_ld, "kv_page"));
     if (cudaMemset(s.kv_page, 0xff, static_cast<size_t>(cfg->max_batch) * s.kv_page_ld * 4) != cudaSuccess) {
         set_error("fsb_lm_create: page table init failed");  // every entry -1: nothing mapped
@@ -869,6 +876,18 @@ int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, 
     const StepGemmPlan* seq[4] = {&P.wo, &P.w13, &P.w2, next};
     for (int k = 0; k < upto; ++k) FSB_TRY(launch_step(*seq[k], rows, st));
     return launch_step(*seq[upto], rows, st, /*finalize_only=*/true);
+}
+
+int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(h != nullptr, "test_layer_attn: null handle");
+    Stack& s = fast ? h->fast : h->slow;
+    FSB_CHECK(layer >= 0 && layer < s.nl, "test_layer_attn: layer=%d outside [0, %d)", layer, s.nl);
+    FSB_CHECK(rows >= 1 && rows <= h->cfg.max_batch, "test_layer_attn: rows=%d outside [1, %d]", rows, h->cfg.max_batch);
+    // the GEMM alone: its operand is the residual stream as the caller left it, normalised on load
+    const StepGemmPlan& qkv = s.dec[layer].qkv;
+    FSB_TRY(launch_step(qkv, rows, st, /*finalize_only=*/false, /*finalize=*/false));
+    return launch_attn_decode(decode_attn_args(h, s, layer, qkv, rows, h->iota, h->pos, kv_only != 0), st);
 }
 
 int fsb_lm_copy_kv(fsb_lm* h, int src_slot, int dst_slot, int n_pos, void* stream) {

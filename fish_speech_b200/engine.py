@@ -344,6 +344,11 @@ class LmEngine:
             "ssq_fast": ((rt, 32), "<f4"),
             "attn": ((rt * max(c.n_head * c.head_dim, c.fast_n_head * c.fast_head_dim),), "<u2"),
             "ffn_h": ((rt * max(c.intermediate_size, c.fast_intermediate_size),), "<u2"),
+            # KV caches (include/fishb200.h fsb_lm_test_layer_attn): the slow page pool, the fast stack per slot
+            "k_slow": ((c.n_layer, self._K.kv_pages, c.n_local_heads, KV_PAGE, c.head_dim), "<u2"),
+            "v_slow": ((c.n_layer, self._K.kv_pages, c.n_local_heads, KV_PAGE, c.head_dim), "<u2"),
+            "k_fast": ((c.n_fast_layer, self.max_batch, c.fast_n_local_heads, c.num_codebooks, c.fast_head_dim), "<u2"),
+            "v_fast": ((c.n_fast_layer, self.max_batch, c.fast_n_local_heads, c.num_codebooks, c.fast_head_dim), "<u2"),
         }
         shape, ts = shapes[name]
         with torch.cuda.device(self.device):

@@ -176,7 +176,10 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
  *   the decode state (for fsb_lm_test_layer_gemms), RT = the decode row tile (32 for max_batch <= 32, else 64):
  *   "x_slow" / "x_fast" bf16 [RT][dim] / [RT][fast_dim] residual streams, "ssq_slow" / "ssq_fast" f32 [RT][32] their
  *   per-128-feature sums of squares, "attn" bf16 [RT * max H*Dh] (the wo operand: rows of the stack being run at
- *   stride H*Dh), "ffn_h" bf16 [RT * max I] (the w2 operand: rows at stride I of the stack being run) */
+ *   stride H*Dh), "ffn_h" bf16 [RT * max I] (the w2 operand: rows at stride I of the stack being run);
+ *   the KV caches (for fsb_lm_test_layer_attn and the copy tests): "k_slow" / "v_slow" bf16
+ *   [n_layer][kv_pages][n_kv_head][64][head_dim] (the page pool), "k_fast" / "v_fast" bf16
+ *   [n_fast_layer][max_batch][fast_n_kv_head][num_codebooks][fast_head_dim] (one contiguous block per slot) */
 int fsb_lm_buffer(fsb_lm* h, const char* name, void** d_ptr, size_t* bytes);
 
 /* Measurement hook for bench.py: launch every weight-streaming step GEMM of one decode frame `reps` times
@@ -292,6 +295,18 @@ int fsb_op_step_gemm_tile(const void* d_w, int n_out, int K, const void* d_x, in
  * Inputs and outputs are the fsb_lm_buffer arrays "x_slow" / "x_fast", "ssq_slow" / "ssq_fast", "attn" and "ffn_h".
  * rows in [1, max_batch]. */
 int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, void* stream);
+
+/* Runs the qkv step GEMM of decode layer `layer` and the decode attention after it (csrc/lm_kernels.cu
+ * attn_decode_kernel: the GEMM's fix-up -- bias, qk-norm, RoPE --, the K/V append and the attention) for `rows` batch
+ * rows, with the arguments fsb_lm_decode gives them: the handle's own plan and partial workspace, the "kv_page" table,
+ * the context bound (fsb_lm_set_context_bound) and the score chunk (fsb_op_attn_score_chunk). The GEMM runs without
+ * the finalize in front of it, so its operand is "x_slow" / "x_fast" exactly as the caller wrote them, normalised on
+ * load with "ssq_slow" / "ssq_fast". Row i is slot i at position "pos"[i] in both stacks (decode gives the fast stack
+ * its codebook positions instead); -1 parks a row. kv_only != 0 stops after the append, as the fast stack's pass 0
+ * does. The fast stack's layer 0 runs the plan of passes >= 1: its operand is the residual stream, not
+ * fast_project_in's output. Outputs: "attn" (rows at stride H*Dh) and the caches "k_*" / "v_*". rows in
+ * [1, max_batch]. */
+int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only, void* stream);
 
 /* Attention keeps one fp32 score per position and head in shared memory; contexts longer than the buffer are walked
  * in chunks, bit-identically (csrc/lm_kernels.cu attend()).  positions > 0 forces a smaller chunk; 0 = automatic. */

@@ -183,7 +183,6 @@ int fsb_op_step_gemm_tile(const void* d_w, int n_out, int K, const void* d_x, in
     }
     if (rc == 0) {
         plan.p.ws = ws;
-        plan.p.rows = rows;
         if (norm) {
             plan.p.x_ssq = d_x_ssq;
             plan.p.norm_w = reinterpret_cast<const __nv_bfloat16*>(d_norm_w);
@@ -197,7 +196,7 @@ int fsb_op_step_gemm_tile(const void* d_w, int n_out, int K, const void* d_x, in
             rc = 1;
         }
     }
-    if (rc == 0) rc = step_gemm_launch(plan, st);
+    if (rc == 0) rc = step_gemm_launch(plan, rows, st);
     if (rc == 0) {
         const StepPartials P = step_plan_partials(plan);
         step_sum_kernel<<<dim3(cdiv(cdiv(n_out, 4), 128), rows), 128, 0, st>>>(P, rows, d_out);

@@ -16,7 +16,7 @@
 // One decode frame (inference.py:96-181) = embed, 36 x {qkv GEMM (norm on load), attention (finishes qkv: bias /
 // qk-norm / RoPE / KV append), wo GEMM, finalize (residual add), w1|w3 GEMM (norm on load), finalize (SwiGLU), w2 GEMM,
 // finalize (residual add)}, head GEMM + sampler, then 10 fast passes of 4 such layers each: ~640 kernels, eight per
-// layer; every GEMM only stores fp32 partials, its consumer finishes it (lm_gemm.cuh).
+// layer; every GEMM only stores fp32 partials, the kernel launched right after it finishes it (lm_gemm.cuh).
 //
 // Reference: fish_speech/models/text2semantic/llama.py:390-466 (slow step), :799-817 (fast step),
 // fish_speech/models/text2semantic/inference.py:96-181 (one frame), :184-238 (frame loop).
@@ -42,6 +42,7 @@ struct LayerW {
 };
 struct StepLayer {
     StepGemmPlan qkv, wo, w13, w2;
+    StepFinalize wo_out, w13_out, w2_out;  // residual add (+ bo), SwiGLU, residual add
 };
 struct PrefillLayer {
     GemmPlan qkv, wo, w13, w2;
@@ -86,7 +87,8 @@ struct fsb_lm {
     const bf16 *fast_emb = nullptr, *fast_norm_w = nullptr, *fast_out_w = nullptr;
     const bf16 *fast_proj_w = nullptr, *fast_proj_b = nullptr;
     int head_rows = 0;
-    StepGemmPlan head_plan, head_plan_direct, fast_out_plan, proj_plan, fast_qkv0_proj;  // *_direct: operand already final
+    StepGemmPlan head_plan, fast_out_plan, proj_plan;
+    StepFinalize proj_out;  // fast_project_in's bias, no residual add, into the fast residual stream
     bool has_proj = false;
     // decode workspaces
     bf16 *q_d = nullptr, *attn_d = nullptr, *h_d = nullptr, *hid_d = nullptr;
@@ -174,30 +176,21 @@ int launch_rows_of(const GemmPlan& plan, const GemmPlan& wide, int rows, cudaStr
     return (rows >= 512 && tiles_wide >= 2 * sms) ? launch_rows_of(wide, rows, st) : launch_rows_of(plan, rows, st);
 }
 
-// Step GEMM over the weight `w` [n_out, K]. act != null: operand X = act, used as it is; act == null: operand X = the
-// stack's residual stream, normalised on load (bind_norm_on_load supplies the norm).
-int make_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, int K, const bf16* act,
-                   const Stack* norm_of = nullptr) {
-    const bool norm = act == nullptr;
-    if (norm) act = norm_of->xres;
-    return step_plan_init(plan, w, n_out, K, act, norm, h->rt, h->step_ctas, kStepStages, h->step_ws,
+// Step GEMM over the weight `w` [n_out, K]; operand X = act, used as it is.
+int make_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, int K, const bf16* act) {
+    return step_plan_init(plan, w, n_out, K, act, false, h->rt, h->step_ctas, kStepStages, h->step_ws,
                           h->step_ws_floats);
 }
 
-void bind_norm_on_load(StepGemmPlan* plan, const Stack& s, const bf16* norm_w, float eps) {
+// Step GEMM over the weight `w` [n_out, s.D]; operand X = stack s's residual stream, RMSNorm'd with norm_w on load.
+int make_norm_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, const Stack& s, const bf16* norm_w) {
+    FSB_TRY(step_plan_init(plan, w, n_out, s.D, s.xres, true, h->rt, h->step_ctas, kStepStages, h->step_ws,
+                           h->step_ws_floats));
     plan->p.x_ssq = s.ssq;
     plan->p.norm_w = norm_w;
     plan->p.x_nt = cdiv(s.D, 128);
-    plan->p.eps = eps;
-}
-
-// `plan` reads the residual stream of stack s after `prev` (a Linear) has been added to it: PRO_RESID finalize of prev
-void bind_resid(StepGemmPlan* plan, const StepGemmPlan& prev, const Stack& s, const bf16* bias, bool add_residual) {
-    step_plan_set_prev(plan, PRO_RESID, prev);
-    plan->p.bias = bias;
-    plan->p.resid = add_residual ? s.xres : nullptr;
-    plan->p.x_out = s.xres;
-    plan->p.ssq_out = s.ssq;
+    plan->p.eps = h->cfg.norm_eps;
+    return 0;
 }
 
 SlotCtl slot_ctl(const fsb_lm* h) {
@@ -211,15 +204,6 @@ SlotCtl slot_ctl(const fsb_lm* h) {
     c.seed = h->slot_seed;
     c.n_out = h->n_out;
     return c;
-}
-
-// One step GEMM over `rows` batch rows: first finish the producer of its operand (residual add / SwiGLU), then the GEMM
-// (only the finish when finalize_only; only the GEMM when !finalize).
-int launch_step(const StepGemmPlan& plan, int rows, cudaStream_t st, bool finalize_only = false, bool finalize = true) {
-    StepGemmPlan q = plan;
-    q.p.rows = rows;
-    if (finalize) FSB_TRY(step_finalize_launch(q, st));
-    return finalize_only ? 0 : step_gemm_launch(q, st);
 }
 
 // Arguments of layer l's decode attention over `rows` batch rows, the consumer of the qkv GEMM `qkv` ran: one place
@@ -248,21 +232,29 @@ AttnDecodeArgs decode_attn_args(const fsb_lm* h, const Stack& s, int l, const St
     return aa;
 }
 
-// ---- decode: one transformer stack over the batch rows, five kernels per layer. `first_qkv`: the plan of layer 0's
-// qkv GEMM when its operand is produced by a GEMM (fast_project_in) instead of a row kernel. After the last layer the
-// residual stream is complete only once the NEXT step GEMM (head / fast_output) has run its prologue. ----
+// The first `upto` (GEMM, finalize) pairs of a layer after its attention: wo + residual add, w1|w3 + SwiGLU,
+// w2 + residual add.
+int run_layer_gemms(const StepLayer& P, int rows, int upto, cudaStream_t st) {
+    const StepGemmPlan* gemm[3] = {&P.wo, &P.w13, &P.w2};
+    const StepFinalize* fin[3] = {&P.wo_out, &P.w13_out, &P.w2_out};
+    for (int k = 0; k < upto; ++k) {
+        FSB_TRY(step_gemm_launch(*gemm[k], rows, st));
+        FSB_TRY(step_finalize_launch(*fin[k], rows, st));
+    }
+    return 0;
+}
+
+// ---- decode: one transformer stack over the batch rows, eight kernels per layer: qkv GEMM, attention, then the
+// three (GEMM, finalize) pairs. ----
 int run_stack_decode(fsb_lm* h, Stack& s, int rows, const int* row_seq, const int* row_pos, bool stop_after_kv,
-                     cudaStream_t st, const StepGemmPlan* first_qkv = nullptr) {
+                     cudaStream_t st) {
     for (int l = 0; l < s.nl; ++l) {
         StepLayer& P = s.dec[l];
-        const StepGemmPlan& qkv = (l == 0 && first_qkv) ? *first_qkv : P.qkv;
-        FSB_TRY(launch_step(qkv, rows, st));
+        FSB_TRY(step_gemm_launch(P.qkv, rows, st));
         const bool kv_only = stop_after_kv && l == s.nl - 1;  // fast pass 0 only fills the KV cache (inference.py:147)
-        FSB_TRY(launch_attn_decode(decode_attn_args(h, s, l, qkv, rows, row_seq, row_pos, kv_only), st));
+        FSB_TRY(launch_attn_decode(decode_attn_args(h, s, l, P.qkv, rows, row_seq, row_pos, kv_only), st));
         if (kv_only) return 0;
-        FSB_TRY(launch_step(P.wo, rows, st));
-        FSB_TRY(launch_step(P.w13, rows, st));
-        FSB_TRY(launch_step(P.w2, rows, st));
+        FSB_TRY(run_layer_gemms(P, rows, 3, st));
     }
     return 0;
 }
@@ -336,7 +328,7 @@ int run_stack_prefill(fsb_lm* h, Stack& s, int rows, const int* row_seq, const i
 // Head + sampling + fast passes + bookkeeping for `rows` sequences whose last residual-stream rows (un-normed)
 // are in slow.xres[0..rows) with their sums of squares in slow.ssq. inference.py:114-181.
 int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const int* set_pos_rows,
-                   const int* row_pos_src, const fsb_sampling& sp, cudaStream_t st, bool x_is_final = false) {
+                   const int* row_pos_src, const fsb_sampling& sp, cudaStream_t st) {
     const fsb_lm_config& c = h->cfg;
     const int C = c.num_codebooks;
     const int* slots = row_slot ? row_slot : h->iota;
@@ -359,11 +351,9 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
         a.noise_ld = h->noise_ld;
         return a;
     };
-    // ---- slow head over the selectable rows (first the last layer's FFN output is added to the residual stream,
-    // unless the rows come from a prefill; the final norm is applied on load) ----
-    const StepGemmPlan& head = x_is_final ? h->head_plan_direct : h->head_plan;
-    FSB_TRY(launch_step(head, rows, st));
-    SampleArgs sa = sample_args(h->head_rows, head);
+    // ---- slow head over the selectable rows (the final norm is applied on load) ----
+    FSB_TRY(step_gemm_launch(h->head_plan, rows, st));
+    SampleArgs sa = sample_args(h->head_rows, h->head_plan);
     sa.slow = 1;
     sa.n_sem = h->head_rows - 1;
     sa.sem_begin = c.semantic_begin_id;
@@ -387,8 +377,8 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
     if (h->has_proj) {
         hr.y = h->hid_d;
         FSB_TRY(launch_rows(hr, st));
-        // fast_project_in; the finalize in front of layer 0's qkv GEMM adds the bias
-        FSB_TRY(launch_step(h->proj_plan, rows, st));
+        FSB_TRY(step_gemm_launch(h->proj_plan, rows, st));  // fast_project_in
+        FSB_TRY(step_finalize_launch(h->proj_out, rows, st));
     } else {
         hr.y = f.xres;
         hr.ssq = f.ssq;
@@ -407,10 +397,9 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
             er.rows = rows; er.D = f.D; er.eps = c.norm_eps;
             FSB_TRY(launch_rows(er, st));
         }
-        FSB_TRY(run_stack_decode(h, f, rows, slots, h->fpos + p * h->rt, p == 0, st,
-                                 (p == 0 && h->has_proj) ? &h->fast_qkv0_proj : nullptr));
+        FSB_TRY(run_stack_decode(h, f, rows, slots, h->fpos + p * h->rt, p == 0, st));
         if (p == 0) continue;
-        FSB_TRY(launch_step(h->fast_out_plan, rows, st));
+        FSB_TRY(step_gemm_launch(h->fast_out_plan, rows, st));
         SampleArgs fa = sample_args(c.codebook_size, h->fast_out_plan);
         fa.slow = 0;
         fa.draw_id = p;
@@ -606,8 +595,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
             return 1;
         }
     }
-    // ---- GEMM plans ----
-    const float eps = cfg->norm_eps;
+    // ---- GEMM plans, and the finalize after each GEMM whose consumer is another GEMM ----
     auto build = [&](Stack& st, bool with_prefill) -> int {
         st.dec.resize(st.nl);
         if (with_prefill) st.pf.resize(st.nl);
@@ -615,18 +603,13 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
         for (int l = 0; l < st.nl; ++l) {
             const LayerW& lw = st.w[l];
             StepLayer& P = st.dec[l];
-            // qkv: layer 0 reads a residual stream a row kernel wrote; later layers first add the previous FFN output
-            FSB_TRY(make_step_plan(h, &P.qkv, lw.wqkv, Nqkv, st.D, nullptr, &st));
-            bind_norm_on_load(&P.qkv, st, lw.attn_norm, eps);
-            if (l > 0) bind_resid(&P.qkv, st.dec[l - 1].w2, st, nullptr, true);
+            FSB_TRY(make_norm_step_plan(h, &P.qkv, lw.wqkv, Nqkv, st, lw.attn_norm));
             FSB_TRY(make_step_plan(h, &P.wo, lw.wo, st.D, st.H * st.Dh, h->attn_d));
-            FSB_TRY(make_step_plan(h, &P.w13, lw.w13, st.n13, st.D, nullptr, &st));
-            bind_norm_on_load(&P.w13, st, lw.ffn_norm, eps);
-            bind_resid(&P.w13, P.wo, st, lw.bo, true);
+            P.wo_out = step_finalize_resid(P.wo, lw.bo, st.xres, st.xres, st.ssq);
+            FSB_TRY(make_norm_step_plan(h, &P.w13, lw.w13, st.n13, st, lw.ffn_norm));
+            P.w13_out = step_finalize_swiglu(P.w13, h->h_d, st.I);
             FSB_TRY(make_step_plan(h, &P.w2, lw.w2, st.D, st.I, h->h_d));
-            step_plan_set_prev(&P.w2, PRO_SWIGLU, P.w13);
-            P.w2.p.h = h->h_d;
-            P.w2.p.I = st.I;
+            P.w2_out = step_finalize_resid(P.w2, nullptr, st.xres, st.xres, st.ssq);
             if (with_prefill) {
                 FSB_TRY(make_prefill_plan(h, &st.pf[l].qkv, lw.wqkv, Nqkv, st.D, h->xn_p, R));
                 FSB_TRY(make_prefill_plan(h, &st.pf[l].wo, lw.wo, st.D, st.H * st.Dh, h->attn_p, R));
@@ -640,21 +623,11 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     };
     TRYC(build(s, true));
     TRYC(build(f, false));
-    TRYC(make_step_plan(h, &h->head_plan, h->head_w, h->head_rows, s.D, nullptr, &s));
-    bind_norm_on_load(&h->head_plan, s, h->norm_w, eps);
-    bind_resid(&h->head_plan, s.dec[s.nl - 1].w2, s, nullptr, true);
-    TRYC(make_step_plan(h, &h->head_plan_direct, h->head_w, h->head_rows, s.D, nullptr, &s));
-    bind_norm_on_load(&h->head_plan_direct, s, h->norm_w, eps);
-    TRYC(make_step_plan(h, &h->fast_out_plan, h->fast_out_w, cfg->codebook_size, f.D, nullptr, &f));
-    bind_norm_on_load(&h->fast_out_plan, f, h->fast_norm_w, eps);
-    bind_resid(&h->fast_out_plan, f.dec[f.nl - 1].w2, f, nullptr, true);
+    TRYC(make_norm_step_plan(h, &h->head_plan, h->head_w, h->head_rows, s, h->norm_w));
+    TRYC(make_norm_step_plan(h, &h->fast_out_plan, h->fast_out_w, cfg->codebook_size, f, h->fast_norm_w));
     if (h->has_proj) {
         TRYC(make_step_plan(h, &h->proj_plan, h->fast_proj_w, f.D, s.D, h->hid_d));
-        // fast layer 0 of pass 0: its operand = fast_project_in(hidden) + bias, finished in the qkv GEMM's prologue
-        const LayerW& l0 = f.w[0];
-        TRYC(make_step_plan(h, &h->fast_qkv0_proj, l0.wqkv, (f.H + 2 * f.Hkv) * f.Dh, f.D, nullptr, &f));
-        bind_norm_on_load(&h->fast_qkv0_proj, f, l0.attn_norm, eps);
-        bind_resid(&h->fast_qkv0_proj, h->proj_plan, f, h->fast_proj_b, false);
+        h->proj_out = step_finalize_resid(h->proj_plan, h->fast_proj_b, nullptr, f.xres, f.ssq);
     }
 #undef TRYC
     *out = h;
@@ -671,12 +644,8 @@ void fsb_lm_destroy(fsb_lm* h) {
     free_plans(h->slow);
     free_plans(h->fast);
     step_plan_free(&h->head_plan);
-    step_plan_free(&h->head_plan_direct);
     step_plan_free(&h->fast_out_plan);
-    if (h->has_proj) {
-        step_plan_free(&h->proj_plan);
-        step_plan_free(&h->fast_qkv0_proj);
-    }
+    if (h->has_proj) step_plan_free(&h->proj_plan);
     for (void* p : h->owned) cudaFree(p);
     delete h;
 }
@@ -722,7 +691,7 @@ int fsb_lm_prefill(fsb_lm* h, const int32_t* d_tokens, const int32_t* d_row_slot
     g.rows = nseq; g.D = s.D; g.eps = c.norm_eps;
     FSB_TRY(launch_rows(g, st));
     // the reference resets the RAS window per generate() call and prefill uses no RAS
-    return run_frame_tail(h, nseq, d_slots, false, d_last_rows, d_row_pos, *sp, st, /*x_is_final=*/true);
+    return run_frame_tail(h, nseq, d_slots, false, d_last_rows, d_row_pos, *sp, st);
 }
 
 int fsb_lm_set_slot_control(fsb_lm* h, int enable) {
@@ -805,16 +774,17 @@ int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* l
     // Every weight-streaming step GEMM of one decode frame (36 slow layers x 4, head, 10 fast passes x
     // (4 layers x 4 + head)) back to back, without the attention / sampling kernels: the measured stream of the
     // dominant kernel for the roofline line of bench.py. Operands are whatever the workspaces hold; the
-    // epilogues run (and overwrite the decode state), so call it after the timed generation only.
+    // finalize kernels run (and overwrite the decode state), so call it after the timed generation only.
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const fsb_lm_config& c = h->cfg;
     double bytes = 0;
-    int launches = 0;
+    int launches = 0;  // GEMMs, not kernels
     const int rows = c.max_batch;
-    auto run = [&](const StepGemmPlan& p) -> int {
+    auto run = [&](const StepGemmPlan& p, const StepFinalize* fin = nullptr) -> int {
         bytes += p.weight_bytes;
         ++launches;
-        return launch_step(p, rows, st);
+        FSB_TRY(step_gemm_launch(p, rows, st));
+        return fin ? step_finalize_launch(*fin, rows, st) : 0;
     };
     for (int r = 0; r < reps; ++r) {
         bytes = 0;
@@ -823,9 +793,9 @@ int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* l
             for (int l = 0; l < s.nl; ++l) {
                 FSB_TRY(run(s.dec[l].qkv));
                 if (skip_tail && l == s.nl - 1) break;
-                FSB_TRY(run(s.dec[l].wo));
-                FSB_TRY(run(s.dec[l].w13));
-                FSB_TRY(run(s.dec[l].w2));
+                FSB_TRY(run(s.dec[l].wo, &s.dec[l].wo_out));
+                FSB_TRY(run(s.dec[l].w13, &s.dec[l].w13_out));
+                FSB_TRY(run(s.dec[l].w2, &s.dec[l].w2_out));
             }
             return 0;
         };
@@ -852,10 +822,14 @@ int fsb_lm_bench_step_kind(fsb_lm* h, int kind, int reps, int finalize, double* 
     double bytes = 0;
     for (int r = 0; r < reps; ++r) {
         bytes = 0;
-        for (StepLayer& P : h->slow.dec) {
+        for (int l = 0; l < h->slow.nl; ++l) {
+            const StepLayer& P = h->slow.dec[l];
             const StepGemmPlan* k[4] = {&P.qkv, &P.wo, &P.w13, &P.w2};
+            // what decode runs right before each kind: the finalize of the GEMM that produces its operand
+            const StepFinalize* before[4] = {l > 0 ? &h->slow.dec[l - 1].w2_out : nullptr, nullptr, &P.wo_out, &P.w13_out};
             bytes += k[kind]->weight_bytes;
-            FSB_TRY(launch_step(*k[kind], rows, st, false, finalize != 0));
+            if (finalize && before[kind]) FSB_TRY(step_finalize_launch(*before[kind], rows, st));
+            FSB_TRY(step_gemm_launch(*k[kind], rows, st));
         }
     }
     if (weight_bytes_per_rep) *weight_bytes_per_rep = bytes;
@@ -870,12 +844,7 @@ int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, 
     FSB_CHECK(layer >= 0 && layer < s.nl, "test_layer_gemms: layer=%d outside [0, %d)", layer, s.nl);
     FSB_CHECK(rows >= 1 && rows <= h->cfg.max_batch, "test_layer_gemms: rows=%d outside [1, %d]", rows, h->cfg.max_batch);
     FSB_CHECK(upto >= 1 && upto <= 3, "test_layer_gemms: upto=%d outside [1, 3]", upto);
-    StepLayer& P = s.dec[layer];
-    // the GEMMs in run_stack_decode's order, then the plan whose finalize finishes the last of them
-    const StepGemmPlan* next = layer + 1 < s.nl ? &s.dec[layer + 1].qkv : fast ? &h->fast_out_plan : &h->head_plan;
-    const StepGemmPlan* seq[4] = {&P.wo, &P.w13, &P.w2, next};
-    for (int k = 0; k < upto; ++k) FSB_TRY(launch_step(*seq[k], rows, st));
-    return launch_step(*seq[upto], rows, st, /*finalize_only=*/true);
+    return run_layer_gemms(s.dec[layer], rows, upto, st);
 }
 
 int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only, void* stream) {
@@ -884,9 +853,9 @@ int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only
     Stack& s = fast ? h->fast : h->slow;
     FSB_CHECK(layer >= 0 && layer < s.nl, "test_layer_attn: layer=%d outside [0, %d)", layer, s.nl);
     FSB_CHECK(rows >= 1 && rows <= h->cfg.max_batch, "test_layer_attn: rows=%d outside [1, %d]", rows, h->cfg.max_batch);
-    // the GEMM alone: its operand is the residual stream as the caller left it, normalised on load
+    // its operand is the residual stream as the caller left it, normalised on load
     const StepGemmPlan& qkv = s.dec[layer].qkv;
-    FSB_TRY(launch_step(qkv, rows, st, /*finalize_only=*/false, /*finalize=*/false));
+    FSB_TRY(step_gemm_launch(qkv, rows, st));
     return launch_attn_decode(decode_attn_args(h, s, layer, qkv, rows, h->iota, h->pos, kv_only != 0), st);
 }
 

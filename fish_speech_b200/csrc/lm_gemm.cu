@@ -35,7 +35,7 @@ __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
     return v;
 }
 
-// ---- step_finalize: one unit = rows [j0, j0 + R) x the 128 features of tile `tile` of the PREVIOUS GEMM's output;
+// ---- step_finalize: one unit = rows [j0, j0 + R) x the 128 features of tile `tile` of the finished GEMM's output;
 // thread tid owns feature tile*128 + tid.  `red` = shared float[4][32]. ----
 
 // Per-row sum over the 128 features of the tile: result for row r in red[q*32 + r], q = 0..3 (one per warp).
@@ -50,10 +50,10 @@ __device__ __forceinline__ void rows_warp_sums(const float (&sq)[R], float* red,
     red[quad * 32 + lane] = keep;
 }
 
-// Slot-ordered sums of the previous GEMM's partials; up to 32 independent loads in flight per thread. RT = the row
-// tile of the previous GEMM (p.prev.rt), a template parameter so that the 32-row finalize keeps its constant strides.
+// Slot-ordered sums of the finished GEMM's partials; up to 32 independent loads in flight per thread. RT = the row
+// tile of that GEMM (p.prev.rt), a template parameter so that the 32-row finalize keeps its constant strides.
 template <int R, int UQ, int RT>  // UQ = partials fetched per round
-__device__ __forceinline__ void prev_sums(const StepGemmParams& p, int tile, int tid, int j0, float (&acc)[R]) {
+__device__ __forceinline__ void prev_sums(const StepFinalize& p, int tile, int tid, int j0, float (&acc)[R]) {
     const int np = __ldg(p.prev.nparts + tile);
     const int maxp = p.prev.max_parts;  // loads are bounded by the launch constant, see step_partial_sum
 #pragma unroll
@@ -79,7 +79,7 @@ __device__ __forceinline__ void prev_sums(const StepGemmParams& p, int tile, int
 
 // llama.py:842-845 / 944-946: y = Linear(...) (bf16), x = x + y (bf16); plus sum_i x^2 of this tile per row
 template <int R, int RT>
-__device__ __forceinline__ void pro_resid(const StepGemmParams& p, int tile, int tid, int j0, float* red) {
+__device__ __forceinline__ void pro_resid(const StepFinalize& p, int tile, int tid, int j0, float* red) {
     const int quad = tid >> 5, lane = tid & 31;
     const int i = tile * 128 + tid;
     const int n = p.prev.n_out;
@@ -109,7 +109,7 @@ __device__ __forceinline__ void pro_resid(const StepGemmParams& p, int tile, int
 
 // llama.py:979-987: h = silu(w1 x) * w3 x, every intermediate a bf16 tensor
 template <int R, int RT>
-__device__ __forceinline__ void pro_swiglu(const StepGemmParams& p, int tile, int tid, int j0) {
+__device__ __forceinline__ void pro_swiglu(const StepFinalize& p, int tile, int tid, int j0) {
     const int quad = tid >> 5, lane = tid & 31;
     const bool hi = (lane & 16) != 0;  // lanes 16..31 hold the w3 ("up") rows of the features lanes 0..15 gate
     const int f = tile * 64 + quad * 16 + (lane & 15);
@@ -132,10 +132,10 @@ __device__ __forceinline__ void pro_swiglu(const StepGemmParams& p, int tile, in
 template <int PRO>
 constexpr int kFinalizeRows = PRO == PRO_SWIGLU ? 8 : 4;
 
-// step_finalize: finishes the GEMM that produced the next GEMM's operand (one unit = R batch rows x one 128-feature
-// tile per CTA); launched between the two GEMMs, so the consumer GEMM finds its operand complete.
+// step_finalize: finishes the GEMM p.prev (one unit = R batch rows x one 128-feature tile per CTA); launched right
+// after it, so the next GEMM finds its operand complete.
 template <int PRO, int RT>
-__global__ void __launch_bounds__(kEpiThreads) step_finalize_kernel(const __grid_constant__ StepGemmParams p) {
+__global__ void __launch_bounds__(kEpiThreads) step_finalize_kernel(const __grid_constant__ StepFinalize p) {
     constexpr int R = kFinalizeRows<PRO>;
     __shared__ float red[4 * 32];
     pdl_launch_dependents();
@@ -360,9 +360,9 @@ step_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 }
 
 template <int NORM, int RT>
-int launch_t(const StepGemmPlan& plan, cudaStream_t st) {
+int launch_t(const StepGemmPlan& plan, const StepGemmParams& p, cudaStream_t st) {
     auto k = step_gemm_kernel<NORM, RT>;
-    FSB_LAUNCH(k, plan.grid, dim3(kStepThreads + (NORM ? kLoaderThreads : 0)), plan.smem, st, plan.tmA, plan.tmB, plan.p);
+    FSB_LAUNCH(k, plan.grid, dim3(kStepThreads + (NORM ? kLoaderThreads : 0)), plan.smem, st, plan.tmA, plan.tmB, p);
     return 0;
 }
 
@@ -456,13 +456,11 @@ int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K,
     p.stages = stages;
     p.n_out = n_out;
     p.K = K;
-    p.rows = row_tile;
     p.a_hint = kEvictFirst;  // weights are streamed once per step (>> L2)
     p.b_hint = kEvictLast;   // the activation tile is re-read by every CTA
     p.ws = ws;
     plan->grid = dim3(static_cast<unsigned>(num_ctas), 1, 1);
     plan->smem = smem_of(stages);
-    plan->pro = PRO_NONE;
     plan->norm = norm;
     plan->rt = row_tile;
     plan->weight_bytes = static_cast<double>(n_out) * K * 2;
@@ -480,9 +478,25 @@ StepPartials step_plan_partials(const StepGemmPlan& plan) {
     return P;
 }
 
-void step_plan_set_prev(StepGemmPlan* plan, int pro, const StepGemmPlan& prev) {
-    plan->p.prev = step_plan_partials(prev);
-    plan->pro = pro;
+StepFinalize step_finalize_resid(const StepGemmPlan& src, const __nv_bfloat16* bias, const __nv_bfloat16* resid,
+                                 __nv_bfloat16* x_out, float* ssq_out) {
+    StepFinalize f{};
+    f.pro = PRO_RESID;
+    f.prev = step_plan_partials(src);
+    f.bias = bias;
+    f.resid = resid;
+    f.x_out = x_out;
+    f.ssq_out = ssq_out;
+    return f;
+}
+
+StepFinalize step_finalize_swiglu(const StepGemmPlan& src, __nv_bfloat16* h, int I) {
+    StepFinalize f{};
+    f.pro = PRO_SWIGLU;
+    f.prev = step_plan_partials(src);
+    f.h = h;
+    f.I = I;
+    return f;
 }
 
 void step_plan_free(StepGemmPlan* plan) {
@@ -496,26 +510,27 @@ void step_plan_free(StepGemmPlan* plan) {
 
 namespace {
 template <int PRO, int RT>
-int finalize_t(const StepGemmParams& p, cudaStream_t st) {
+int finalize_t(const StepFinalize& p, cudaStream_t st) {
     const dim3 units(p.prev.tiles * cdiv(p.rows, kFinalizeRows<PRO>));
     FSB_LAUNCH((step_finalize_kernel<PRO, RT>), units, dim3(kEpiThreads), 0, st, p);
     return 0;
 }
 }  // namespace
 
-int step_finalize_launch(const StepGemmPlan& consumer, cudaStream_t st) {
-    // `consumer`'s finalize fields (prev, bias / resid / x_out / ssq_out or h / I, rows) describe the work; one unit per CTA
-    const int pro = consumer.pro;
-    if (pro == PRO_NONE) return 0;
-    const StepGemmParams& p = consumer.p;
+int step_finalize_launch(const StepFinalize& fin, int rows, cudaStream_t st) {
+    StepFinalize p = fin;
+    p.rows = rows;
     if (p.prev.rt == kStepRowsMax)
-        return pro == PRO_RESID ? finalize_t<PRO_RESID, kStepRowsMax>(p, st) : finalize_t<PRO_SWIGLU, kStepRowsMax>(p, st);
-    return pro == PRO_RESID ? finalize_t<PRO_RESID, kStepRows>(p, st) : finalize_t<PRO_SWIGLU, kStepRows>(p, st);
+        return p.pro == PRO_RESID ? finalize_t<PRO_RESID, kStepRowsMax>(p, st) : finalize_t<PRO_SWIGLU, kStepRowsMax>(p, st);
+    return p.pro == PRO_RESID ? finalize_t<PRO_RESID, kStepRows>(p, st) : finalize_t<PRO_SWIGLU, kStepRows>(p, st);
 }
 
-int step_gemm_launch(const StepGemmPlan& plan, cudaStream_t st) {
-    if (plan.rt == kStepRowsMax) return plan.norm ? launch_t<1, kStepRowsMax>(plan, st) : launch_t<0, kStepRowsMax>(plan, st);
-    return plan.norm ? launch_t<1, kStepRows>(plan, st) : launch_t<0, kStepRows>(plan, st);
+int step_gemm_launch(const StepGemmPlan& plan, int rows, cudaStream_t st) {
+    StepGemmParams p = plan.p;
+    p.rows = rows;
+    if (plan.rt == kStepRowsMax)
+        return plan.norm ? launch_t<1, kStepRowsMax>(plan, p, st) : launch_t<0, kStepRowsMax>(plan, p, st);
+    return plan.norm ? launch_t<1, kStepRows>(plan, p, st) : launch_t<0, kStepRows>(plan, p, st);
 }
 
 }  // namespace fsb

@@ -21,19 +21,22 @@
 //      start step 1 while this launch drains and its consumer runs.
 // Whoever consumes the result finishes the GEMM: it sums the partials IN SLOT ORDER (deterministic, independent of
 // arrival order and of the batch) and applies what the reference does next:
-//   step_finalize (this file)  PRO_RESID   bias, residual add, new residual stream + per-128-feature sum of squares
+//   StepFinalize (this file)   PRO_RESID   bias, residual add, new residual stream + per-128-feature sum of squares
 //                                          for the next normalise-on-load                          (llama.py:842-845)
 //                              PRO_SWIGLU  silu(w1 x) * w3 x on the row-interleaved w1|w3 result   (llama.py:979-987)
 //   attention (lm_kernels.cuh) bias, per-head nn.RMSNorm, RoPE, KV append for the qkv GEMM          (llama.py:891-911)
 //   sampler (lm_kernels.cuh)   bf16 logits of the two heads                                        (llama.py:447-457)
 // The finish runs in a kernel of its own rather than in a tail of this GEMM (last-arriving CTA) or in the prologue of
-// the consumer GEMM: a tail or a prologue holds the shared memory the next GEMM's weight prefetch needs.
+// the next GEMM: a tail or a prologue holds the shared memory the next GEMM's weight prefetch needs.
+//
+// Ordering rule: all step GEMMs of an engine share one partial workspace (step_ws), so a GEMM's single consumer
+// (finalize, attention or sampler) must be launched after that GEMM and before the next step GEMM.
 #pragma once
 #include "gemm_tc.cuh"
 
 namespace fsb {
 
-enum StepPro { PRO_NONE = 0, PRO_RESID = 1, PRO_SWIGLU = 2 };
+enum StepPro { PRO_RESID = 1, PRO_SWIGLU = 2 };
 
 constexpr int kStepRows = 32;     // batch rows of the 32-row tile = wgmma N
 constexpr int kStepRowsMax = 64;  // the 64-row tile: two wgmma N=32 halves
@@ -107,17 +110,9 @@ struct StepGemmParams {
     const int* cta_items;   // [grid + 1]
     int tiles, stages;
     int n_out, K;           // output features, reduction length
-    int rows;               // live batch rows (<= the row tile RT)
+    int rows;               // live batch rows (<= the row tile RT), set by step_gemm_launch
     unsigned long long a_hint, b_hint;
     float* ws;              // out: [slot][tile][RT rows][128 features] fp32 partials
-    // ---- step_finalize of the GEMM that produces this one's operand (pro != PRO_NONE) ----
-    StepPartials prev;
-    const __nv_bfloat16* bias;    // PRO_RESID: [prev.n_out] or null
-    const __nv_bfloat16* resid;   // PRO_RESID: [RT][prev.n_out]; may alias x_out; null => no add
-    __nv_bfloat16* x_out;         // PRO_RESID: [RT][prev.n_out] new residual stream
-    float* ssq_out;               // PRO_RESID: [RT][kSsqStride]
-    __nv_bfloat16* h;             // PRO_SWIGLU: [RT][I]; prev tile t = features [64t, 64t+64): lanes 32w+l (l < 16) =
-    int I;                        //             w1 row, lanes 32w+16+l = w3 row
     // ---- operand X by normalise-on-load (NORM = 1) ----
     const float* x_ssq;           // [RT][kSsqStride] per-tile sum of squares of x
     const __nv_bfloat16* norm_w;  // [K]
@@ -125,12 +120,25 @@ struct StepGemmParams {
     float eps;
 };
 
+// The finish of one step GEMM (`prev`) by step_finalize_kernel, launched right after that GEMM.
+struct StepFinalize {
+    int pro;                      // PRO_RESID / PRO_SWIGLU
+    StepPartials prev;
+    const __nv_bfloat16* bias;    // PRO_RESID: [prev.n_out] or null
+    const __nv_bfloat16* resid;   // PRO_RESID: [RT][prev.n_out]; may alias x_out; null => no add
+    __nv_bfloat16* x_out;         // PRO_RESID: [RT][prev.n_out] new residual stream
+    float* ssq_out;               // PRO_RESID: [RT][kSsqStride]
+    __nv_bfloat16* h;             // PRO_SWIGLU: [RT][I]; prev tile t = features [64t, 64t+64): lanes 32w+l (l < 16) =
+    int I;                        //             w1 row, lanes 32w+16+l = w3 row
+    int rows;                     // live batch rows (<= prev.rt), set by step_finalize_launch
+};
+
 struct StepGemmPlan {
     CUtensorMap tmA, tmB;
     StepGemmParams p;
     dim3 grid;
     size_t smem;
-    int pro, norm;
+    int norm;
     int rt;  // row tile: 32 or 64
     void* sched_dev;
     int* cta_items_dev;
@@ -145,13 +153,14 @@ int step_plan_init(StepGemmPlan* plan, const __nv_bfloat16* w, int n_out, int K,
                    bool norm_on_load, int row_tile, int num_ctas, int stages, float* ws, size_t ws_floats);
 // the partials `plan` produces, as a consumer sees them
 StepPartials step_plan_partials(const StepGemmPlan& plan);
-// `plan`'s operand is the output of `prev` finished with `pro` (PRO_RESID / PRO_SWIGLU): records what
-// step_finalize_launch(plan) has to do before `plan` runs (the caller fills bias / resid / x_out / ssq_out or h / I)
-void step_plan_set_prev(StepGemmPlan* plan, int pro, const StepGemmPlan& prev);
 void step_plan_free(StepGemmPlan* plan);
-int step_gemm_launch(const StepGemmPlan& plan, cudaStream_t stream);
-// finish the GEMM that produces `consumer`'s operand (no-op when consumer.pro == PRO_NONE); launch it before the consumer
-int step_finalize_launch(const StepGemmPlan& consumer, cudaStream_t stream);
+int step_gemm_launch(const StepGemmPlan& plan, int rows, cudaStream_t stream);  // over `rows` (<= plan.rt) batch rows
+// PRO_RESID finish of `src`: x_out = resid + (src + bias) (resid / bias may be null), and its sums of squares
+StepFinalize step_finalize_resid(const StepGemmPlan& src, const __nv_bfloat16* bias, const __nv_bfloat16* resid,
+                                 __nv_bfloat16* x_out, float* ssq_out);
+// PRO_SWIGLU finish of the w1|w3 GEMM `src` into h [RT][I]
+StepFinalize step_finalize_swiglu(const StepGemmPlan& src, __nv_bfloat16* h, int I);
+int step_finalize_launch(const StepFinalize& fin, int rows, cudaStream_t stream);  // one unit per CTA
 int step_gemm_init();  // kernel attributes (idempotent)
 
 // Row index of the fused w1|w3 weight for SwiGLU: h feature f -> row of w1[f]; w3[f] sits 16 rows further.

@@ -183,7 +183,7 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
 int fsb_lm_buffer(fsb_lm* h, const char* name, void** d_ptr, size_t* bytes);
 
 /* Measurement hook for bench.py: launch every weight-streaming step GEMM of one decode frame `reps` times
- * (no attention / sampling kernels; the fused epilogues run and overwrite the decode state, so call it after
+ * (no attention / sampling kernels; the finalize kernels run and overwrite the decode state, so call it after
  * the timed generation); returns the algorithmic weight bytes and launch count of one repetition. */
 int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* launches_per_rep,
                        void* stream);
@@ -290,8 +290,7 @@ int fsb_op_step_gemm_tile(const void* d_w, int n_out, int K, const void* d_x, in
  * exactly as fsb_lm_decode does (the handle's own plans, launch order and partial workspace), without attention:
  *   upto = 1: wo GEMM + its residual-add finalize (x += wo(attn) + bo, and the sums of squares of x)
  *   upto = 2: + w1|w3 GEMM (normalised on load) + SwiGLU finalize (h)
- *   upto = 3: + w2 GEMM + the residual-add finalize run in front of the next consumer (next layer's qkv GEMM; the
- *             head / fast output GEMM after the last layer)
+ *   upto = 3: + w2 GEMM + its residual-add finalize
  * Inputs and outputs are the fsb_lm_buffer arrays "x_slow" / "x_fast", "ssq_slow" / "ssq_fast", "attn" and "ffn_h".
  * rows in [1, max_batch]. */
 int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, void* stream);
@@ -299,13 +298,11 @@ int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, 
 /* Runs the qkv step GEMM of decode layer `layer` and the decode attention after it (csrc/lm_kernels.cu
  * attn_decode_kernel: the GEMM's fix-up -- bias, qk-norm, RoPE --, the K/V append and the attention) for `rows` batch
  * rows, with the arguments fsb_lm_decode gives them: the handle's own plan and partial workspace, the "kv_page" table,
- * the context bound (fsb_lm_set_context_bound) and the score chunk (fsb_op_attn_score_chunk). The GEMM runs without
- * the finalize in front of it, so its operand is "x_slow" / "x_fast" exactly as the caller wrote them, normalised on
- * load with "ssq_slow" / "ssq_fast". Row i is slot i at position "pos"[i] in both stacks (decode gives the fast stack
- * its codebook positions instead); -1 parks a row. kv_only != 0 stops after the append, as the fast stack's pass 0
- * does. The fast stack's layer 0 runs the plan of passes >= 1: its operand is the residual stream, not
- * fast_project_in's output. Outputs: "attn" (rows at stride H*Dh) and the caches "k_*" / "v_*". rows in
- * [1, max_batch]. */
+ * the context bound (fsb_lm_set_context_bound) and the score chunk (fsb_op_attn_score_chunk). The GEMM's operand is
+ * "x_slow" / "x_fast" exactly as the caller wrote them, normalised on load with "ssq_slow" / "ssq_fast". Row i is
+ * slot i at position "pos"[i] in both stacks (decode gives the fast stack its codebook positions instead); -1 parks a
+ * row. kv_only != 0 stops after the append, as the fast stack's pass 0 does. Outputs: "attn" (rows at stride H*Dh)
+ * and the caches "k_*" / "v_*". rows in [1, max_batch]. */
 int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only, void* stream);
 
 /* Attention keeps one fp32 score per position and head in shared memory; contexts longer than the buffer are walked

@@ -379,9 +379,8 @@ LAYER_CASES = [pytest.param(name, fast, last, id=f"{name}-{'fast' if fast else '
 
 @pytest.mark.parametrize("name,fast,last", LAYER_CASES)
 def test_decode_layer_gemms(name, fast, last):
-    """wo + residual add, w1|w3 (normalised on load) + SwiGLU, w2 + residual add (run in front of the next layer's qkv
-    GEMM, or the head / fast output GEMM after the last layer), each stage against float64 from the kernel's own
-    output of the stage before."""
+    """wo + residual add, w1|w3 (normalised on load) + SwiGLU, w2 + residual add, each stage against float64 from the
+    kernel's own output of the stage before."""
     L = _lib()
     cfg, w, model = _model(name)
     eng = model.engine

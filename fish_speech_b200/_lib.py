@@ -102,6 +102,11 @@ def lib() -> C.CDLL:
     L.fsb_op_attn_per_row.argtypes = [i32]
     L.fsb_window_attn.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp]
     L.fsb_swiglu_f32.argtypes = [vp, i32, i32, vp, vp]
+    L.fsb_qkv_rope_ring.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]
+    L.fsb_window_attn_ring.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp]
+    L.fsb_window_fill.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    L.fsb_window_roll.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    L.fsb_dwconv_ln_window.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, C.c_float, vp, vp]
     L.fsb_op_gemm.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
     L.fsb_op_step_gemm.argtypes = [vp, i32, i32, vp, i32, vp, vp, C.c_float, i32, i32, vp, i32p, vp]
     L.fsb_op_step_gemm_tile.argtypes = [vp, i32, i32, vp, i32, i32, vp, vp, C.c_float, i32, i32, vp, i32p, vp]

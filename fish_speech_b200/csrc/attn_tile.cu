@@ -39,7 +39,9 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-template <int DH>
+// RING: the cache is a ring of S positions (kv_ring_row); S is a multiple of the tile, so the tile of absolute positions
+// kt .. kt + 63 is rows kt % S .. kt % S + 63 and the walk over absolute tiles is unchanged.
+template <int DH, bool RING>
 __global__ void __launch_bounds__(kAtThreads) attn_tile_kernel(AttnArgs a, float scale_log2e) {
     constexpr int CH = DH / 8;        // 16-byte chunks per row
     constexpr int KS = DH / 16;       // k-steps of Q K^T
@@ -84,7 +86,9 @@ __global__ void __launch_bounds__(kAtThreads) attn_tile_kernel(AttnArgs a, float
     // K/V tile of positions kt .. kt + 63 of sequence `seq`: contiguous, or exactly one (mapped) page of a paged cache
     auto load_tile = [&](int buf, int seq, int kt, int hi) {
         size_t tbase;
-        if (a.kv_page != nullptr) {
+        if (RING) {
+            tbase = static_cast<size_t>(kv_ring_row(seq, g, a.Hkv, a.S) + kt % a.S) * DH;
+        } else if (a.kv_page != nullptr) {
             const int pg = a.kv_page[static_cast<size_t>(seq) * a.kv_page_ld + kt / kKvPage];
             tbase = (static_cast<size_t>(pg) * a.Hkv + g) * kKvPage * DH;
         } else {
@@ -110,7 +114,7 @@ __global__ void __launch_bounds__(kAtThreads) attn_tile_kernel(AttnArgs a, float
         while (end < kTQ && s_seq[end] == seq && s_pos[end] == p0 + (end - start)) ++end;
         if (seq >= 0 && p0 >= 0) {
             // ---- one run: rows [start, end) = positions p0 .. p0 + (end - start) - 1 of sequence `seq` ----
-            const int hi = min(p0 + (end - start) - 1, a.S - 1);
+            const int hi = RING ? p0 + (end - start) - 1 : min(p0 + (end - start) - 1, a.S - 1);
             const int lo = a.window > 0 ? max(0, p0 - a.window + 1) : 0;
             const bool v0 = qi0 >= start && qi0 < end, v1 = qi1 >= start && qi1 < end;
             const int pq0 = p0 + (qi0 - start), pq1 = p0 + (qi1 - start);
@@ -238,16 +242,17 @@ __global__ void __launch_bounds__(kAtThreads) attn_tile_kernel(AttnArgs a, float
     }
 }
 
-template <int DH>
+template <int DH, bool RING>
 int launch_t(const AttnArgs& a, cudaStream_t st) {
     static bool attr = false;
     const size_t smem = static_cast<size_t>(kTQ + 4 * kTK) * DH * 2;
     if (!attr) {
-        FSB_CUDA(cudaFuncSetAttribute(attn_tile_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+        FSB_CUDA(cudaFuncSetAttribute(attn_tile_kernel<DH, RING>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      static_cast<int>(smem)));
         attr = true;
     }
     const float scale_log2e = 1.4426950408889634f / sqrtf(static_cast<float>(DH));
-    FSB_LAUNCH((attn_tile_kernel<DH>), dim3(cdiv(a.rows, kTQ), a.H), dim3(kAtThreads), smem, st, a, scale_log2e);
+    FSB_LAUNCH((attn_tile_kernel<DH, RING>), dim3(cdiv(a.rows, kTQ), a.H), dim3(kAtThreads), smem, st, a, scale_log2e);
     return 0;
 }
 
@@ -261,7 +266,8 @@ bool attn_tile_supported(const AttnArgs& a) {
 int launch_attn_tile(const AttnArgs& a, cudaStream_t st) {
     if (a.rows <= 0) return 0;
     FSB_CHECK(attn_tile_supported(a), "attn_tile: unsupported geometry (head_dim %d)", a.Dh);
-    return a.Dh == 64 ? launch_t<64>(a, st) : launch_t<128>(a, st);
+    if (a.ring) return a.Dh == 64 ? launch_t<64, true>(a, st) : launch_t<128, true>(a, st);
+    return a.Dh == 64 ? launch_t<64, false>(a, st) : launch_t<128, false>(a, st);
 }
 
 }  // namespace fsb

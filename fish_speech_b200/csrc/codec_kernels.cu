@@ -8,6 +8,7 @@
 //   final_conv     modded_dac.py:793-797 (Snake'd input -> conv7 C->1 -> tanh)
 //   first_conv     modded_dac.py:683 (conv7 1->C on the raw waveform)
 //   vq_encode      rvq.py:304-317 + dac/nn/quantize.py VectorQuantize.forward (10 residual VQ stages)
+#include <algorithm>
 #include <map>
 #include <mutex>
 #include <vector>
@@ -42,10 +43,11 @@ __global__ void codebook_sum_kernel(const int* __restrict__ idx, const float* co
 
 // ------------------------------------------------------------------------------------------------
 constexpr int kDwThreads = 256;
-__global__ void __launch_bounds__(kDwThreads)
-dwconv_ln_kernel(const bf16* __restrict__ x, const float* __restrict__ w /*[C][K]*/, const float* __restrict__ bias,
-                 const float* __restrict__ ln_w, const float* __restrict__ ln_b, int T, int C, int K, float eps,
-                 bf16* __restrict__ y) {
+// Output row t (blockIdx.x) of batch b reads input rows origin + t - (K-1) .. origin + t of x [B][T_in][C]; y [B][T_out][C].
+__device__ __forceinline__ void dwconv_ln_row(const bf16* __restrict__ x, const float* __restrict__ w,
+                                              const float* __restrict__ bias, const float* __restrict__ ln_w,
+                                              const float* __restrict__ ln_b, int T_in, int origin, int T_out, int C,
+                                              int K, float eps, bf16* __restrict__ y) {
     __shared__ float red[33];
     pdl_launch_dependents();
     pdl_wait();
@@ -59,8 +61,8 @@ dwconv_ln_kernel(const bf16* __restrict__ x, const float* __restrict__ w /*[C][K
         if (c < C) {
             float acc = bias[c];
             for (int j = 0; j < K; ++j) {
-                const int tt = t - (K - 1) + j;
-                if (tt >= 0) acc += w[c * K + j] * bf2f(x[(static_cast<size_t>(b) * T + tt) * C + c]);
+                const int tt = origin + t - (K - 1) + j;
+                if (tt >= 0) acc += w[c * K + j] * bf2f(x[(static_cast<size_t>(b) * T_in + tt) * C + c]);
             }
             v[e] = acc;
             s += acc;
@@ -78,7 +80,60 @@ dwconv_ln_kernel(const bf16* __restrict__ x, const float* __restrict__ w /*[C][K
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
         const int c = threadIdx.x + e * kDwThreads;
-        if (c < C) y[(static_cast<size_t>(b) * T + t) * C + c] = f2bf((v[e] - mean) * r * ln_w[c] + ln_b[c]);
+        if (c < C) y[(static_cast<size_t>(b) * T_out + t) * C + c] = f2bf((v[e] - mean) * r * ln_w[c] + ln_b[c]);
+    }
+}
+__global__ void __launch_bounds__(kDwThreads)
+dwconv_ln_kernel(const bf16* __restrict__ x, const float* __restrict__ w /*[C][K]*/, const float* __restrict__ bias,
+                 const float* __restrict__ ln_w, const float* __restrict__ ln_b, int T, int C, int K, float eps,
+                 bf16* __restrict__ y) {
+    dwconv_ln_row(x, w, bias, ln_w, ln_b, T, 0, T, C, K, eps, y);
+}
+// The same over a stream window (DecodeStreamPool): rows 0 .. origin-1 of each batch are the carried history and only
+// the T_out rows after them are computed.
+__global__ void __launch_bounds__(kDwThreads)
+dwconv_ln_window_kernel(const bf16* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
+                        const float* __restrict__ ln_w, const float* __restrict__ ln_b, int T_in, int origin, int T_out,
+                        int C, int K, float eps, bf16* __restrict__ y) {
+    dwconv_ln_row(x, w, bias, ln_w, ln_b, T_in, origin, T_out, C, K, eps, y);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Stream windows of DecodeStreamPool: window [nb][H + n][row] per layer input, rows 0 .. H-1 the carried history.
+// fill: history rows from state [slots][H][row] (row i's slot), rows H .. H + valid[i] - 1 from the producer's dense
+// output [nb][n][row]; roll: the last H valid rows back to the slot's state. Flat over 16-byte units.
+__global__ void window_fill_kernel(const uint4* __restrict__ state, const uint4* __restrict__ dense,
+                                   uint4* __restrict__ win, const int* __restrict__ slot, const int* __restrict__ valid,
+                                   int nb, int H, int n, int u16) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long total = static_cast<long long>(nb) * (H + n) * u16;
+    for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total;
+         e += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const int u = static_cast<int>(e % u16);
+        const long long r = e / u16;
+        const int i = static_cast<int>(r / (H + n)), w = static_cast<int>(r - static_cast<long long>(i) * (H + n));
+        const int s = slot[i];
+        if (s < 0) continue;
+        if (w < H) win[e] = state[(static_cast<size_t>(s) * H + w) * u16 + u];
+        else if (w - H < valid[i]) win[e] = dense[(static_cast<size_t>(i) * n + (w - H)) * u16 + u];
+    }
+}
+__global__ void window_roll_kernel(const uint4* __restrict__ win, uint4* __restrict__ state,
+                                   const int* __restrict__ slot, const int* __restrict__ valid, int nb, int H, int n,
+                                   int u16) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long total = static_cast<long long>(nb) * H * u16;
+    for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total;
+         e += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const int u = static_cast<int>(e % u16);
+        const long long r = e / u16;
+        const int i = static_cast<int>(r / H), h = static_cast<int>(r - static_cast<long long>(i) * H);
+        const int s = slot[i];
+        if (s < 0) continue;
+        state[(static_cast<size_t>(s) * H + h) * u16 + u] =
+            win[(static_cast<size_t>(i) * (H + n) + valid[i] + h) * u16 + u];
     }
 }
 
@@ -421,6 +476,42 @@ int fsb_dwconv_ln(const void* d_x, const float* d_w, const float* d_bias, const 
     return 0;
 }
 
+int fsb_dwconv_ln_window(const void* d_x, const float* d_w, const float* d_bias, const float* d_ln_w,
+                         const float* d_ln_b, int B, int T_in, int origin, int T_out, int C, int K, float eps, void* d_y,
+                         void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(C <= 8 * kDwThreads, "dwconv_ln: C=%d too large", C);
+    FSB_CHECK(origin >= 0 && origin + T_out <= T_in, "dwconv_ln_window: rows %d + %d outside %d", origin, T_out, T_in);
+    if (T_out <= 0 || B <= 0) return 0;
+    FSB_LAUNCH(dwconv_ln_window_kernel, dim3(T_out, B), dim3(kDwThreads), 0, st, reinterpret_cast<const bf16*>(d_x), d_w,
+               d_bias, d_ln_w, d_ln_b, T_in, origin, T_out, C, K, eps, reinterpret_cast<bf16*>(d_y));
+    return 0;
+}
+
+int fsb_window_fill(const void* d_state, const void* d_dense, void* d_win, const int32_t* d_slot,
+                    const int32_t* d_valid, int nb, int H, int n, int row_bytes, void* stream) {
+    FSB_CHECK(row_bytes > 0 && row_bytes % 16 == 0 && H >= 0 && n >= 0, "window_fill: row_bytes=%d H=%d n=%d", row_bytes,
+              H, n);
+    const long long total = static_cast<long long>(nb) * (H + n) * (row_bytes / 16);
+    if (total <= 0) return 0;
+    FSB_LAUNCH(window_fill_kernel, dim3(static_cast<unsigned>(std::min<long long>(cdivll(total, 256), 8192))), dim3(256),
+               0, reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const uint4*>(d_state),
+               reinterpret_cast<const uint4*>(d_dense), reinterpret_cast<uint4*>(d_win), d_slot, d_valid, nb, H, n,
+               row_bytes / 16);
+    return 0;
+}
+
+int fsb_window_roll(const void* d_win, void* d_state, const int32_t* d_slot, const int32_t* d_valid, int nb, int H,
+                    int n, int row_bytes, void* stream) {
+    FSB_CHECK(row_bytes > 0 && row_bytes % 16 == 0, "window_roll: row_bytes=%d", row_bytes);
+    const long long total = static_cast<long long>(nb) * H * (row_bytes / 16);
+    if (total <= 0) return 0;
+    FSB_LAUNCH(window_roll_kernel, dim3(static_cast<unsigned>(std::min<long long>(cdivll(total, 256), 8192))), dim3(256),
+               0, reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const uint4*>(d_win),
+               reinterpret_cast<uint4*>(d_state), d_slot, d_valid, nb, H, n, row_bytes / 16);
+    return 0;
+}
+
 int fsb_final_conv_tanh(const void* d_a, const float* d_w, float bias, int B, int T, int C, int K, float* d_wav,
                         void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -487,7 +578,14 @@ int fsb_resid_scale_norm(const float* d_y, int ld, const void* d_scale, const vo
 
 int fsb_qkv_rope(const float* d_qkv, int rows, int H, int Hkv, int Dh, const void* d_freqs, const int32_t* d_row_seq,
                  const int32_t* d_row_pos, void* d_q, void* d_k, void* d_v, int S, void* stream) {
+    return fsb_qkv_rope_ring(d_qkv, rows, H, Hkv, Dh, d_freqs, d_row_seq, d_row_pos, d_q, d_k, d_v, S, 0, stream);
+}
+
+int fsb_qkv_rope_ring(const float* d_qkv, int rows, int H, int Hkv, int Dh, const void* d_freqs,
+                      const int32_t* d_row_seq, const int32_t* d_row_pos, void* d_q, void* d_k, void* d_v, int S,
+                      int ring, void* stream) {
     QkvPrepArgs a{};
+    a.ring = ring != 0;
     a.y = d_qkv;
     a.ld = (H + 2 * Hkv) * Dh;
     a.freqs = reinterpret_cast<const bf16*>(d_freqs);
@@ -504,8 +602,15 @@ int fsb_qkv_rope(const float* d_qkv, int rows, int H, int Hkv, int Dh, const voi
 int fsb_window_attn(const void* d_q, const void* d_k, const void* d_v, const int32_t* d_row_seq,
                     const int32_t* d_row_pos, int rows, int H, int Hkv, int Dh, int S, int window, void* d_out,
                     void* stream) {
+    return fsb_window_attn_ring(d_q, d_k, d_v, d_row_seq, d_row_pos, rows, H, Hkv, Dh, S, window, 0, d_out, stream);
+}
+
+int fsb_window_attn_ring(const void* d_q, const void* d_k, const void* d_v, const int32_t* d_row_seq,
+                         const int32_t* d_row_pos, int rows, int H, int Hkv, int Dh, int S, int window, int ring,
+                         void* d_out, void* stream) {
     FSB_TRY(attn_init());
     AttnArgs a{};
+    a.ring = ring != 0;
     a.q = reinterpret_cast<const bf16*>(d_q);
     a.kcache = reinterpret_cast<const bf16*>(d_k);
     a.vcache = reinterpret_cast<const bf16*>(d_v);

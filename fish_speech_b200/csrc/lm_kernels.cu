@@ -277,7 +277,7 @@ __global__ void qkv_prep_kernel(QkvPrepArgs a) {
 // at head_dim 128), so the per-head norm is a warp reduction and a row costs one CTA of 8 warps instead of H + 2 Hkv
 // CTAs of Dh / 2 threads (393 216 one-warp CTAs per codec transformer layer at 32 x 256 frames).
 constexpr int kQkvRowThreads = 256;
-template <int DH>
+template <int DH, bool RING>
 __global__ void __launch_bounds__(kQkvRowThreads) qkv_prep_row_kernel(QkvPrepArgs a) {
     pdl_launch_dependents();
     pdl_wait();
@@ -331,6 +331,15 @@ __global__ void __launch_bounds__(kQkvRowThreads) qkv_prep_row_kernel(QkvPrepArg
             const uint32_t packed = pack_bf2(v0[u], v1[u]);
             if (kind == 0) {
                 reinterpret_cast<uint32_t*>(a.q + (static_cast<size_t>(row) * a.H + head) * DH)[t] = packed;
+            } else if (RING) {
+                if (pos >= 0) {
+                    const int g = kind == 1 ? head - a.H : head - a.H - a.Hkv;
+                    __nv_bfloat16* cache = kind == 1 ? a.kcache : a.vcache;
+                    const int r = pos % a.S;
+                    const long long base = kv_ring_row(b, g, a.Hkv, a.S);
+                    reinterpret_cast<uint32_t*>(cache + (base + r) * DH)[t] = packed;
+                    if (r < kKvPage) reinterpret_cast<uint32_t*>(cache + (base + a.S + r) * DH)[t] = packed;  // mirror
+                }
             } else if (pos >= 0 && pos < a.S) {
                 const int g = kind == 1 ? head - a.H : head - a.H - a.Hkv;
                 __nv_bfloat16* cache = kind == 1 ? a.kcache : a.vcache;
@@ -510,7 +519,9 @@ __device__ __forceinline__ void attend(const float* qs, float* sc, float* red, c
 }
 
 
-template <int DH, int G>
+// RING: the cache is a ring (kv_ring_row); the "pages" are then the runs of kKvPage positions from lo, each one run of
+// consecutive rows thanks to the mirror, so attend() walks the same positions in the same order as over a linear cache.
+template <int DH, int G, bool RING>
 __global__ void __launch_bounds__(kAttnThreads) attn_kernel(AttnArgs a, float scale, int lcap) {
     pdl_launch_dependents();
     pdl_wait();
@@ -520,7 +531,8 @@ __global__ void __launch_bounds__(kAttnThreads) attn_kernel(AttnArgs a, float sc
     float* red = sc + G * lcap;          // [kAttnWarps][G][DH]
     const int row = blockIdx.y, g = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int b = a.row_seq[row], pos = min(a.row_pos[row], a.S - 1);  // a position past the cache reads its last row
+    // a position past a linear cache reads its last row
+    const int b = a.row_seq[row], pos = RING ? a.row_pos[row] : min(a.row_pos[row], a.S - 1);
     if (pos < 0) {  // idle slot parked at position -1: nothing to attend to
         for (int e = threadIdx.x; e < G * DH; e += kAttnThreads)
             a.out[(static_cast<size_t>(row) * a.H + blockIdx.x * G) * DH + e] = f2bf(0.f);
@@ -531,12 +543,19 @@ __global__ void __launch_bounds__(kAttnThreads) attn_kernel(AttnArgs a, float sc
     int* pt = reinterpret_cast<int*>(red + kAttnWarps * G * DH);  // [pages of positions lo..pos]
     bool unmapped = false;
     for (int j = threadIdx.x; j <= (L - 1) / kKvPage; j += kAttnThreads) {
-        pt[j] = a.kv_page ? a.kv_page[static_cast<size_t>(b) * a.kv_page_ld + j] : j;
+        if (RING) pt[j] = (lo + j * kKvPage) % a.S;  // ring row of the run's first position
+        else pt[j] = a.kv_page ? a.kv_page[static_cast<size_t>(b) * a.kv_page_ld + j] : j;
         unmapped |= pt[j] < 0;
     }
-    const size_t cache_base = a.kv_page ? static_cast<size_t>(g) * kKvPage * DH
-                                        : ((static_cast<size_t>(b) * a.Hkv + g) * a.S + lo) * DH;
-    const size_t page_stride = static_cast<size_t>(a.kv_page ? a.Hkv : 1) * kKvPage * DH;
+    size_t cache_base, page_stride;
+    if (RING) {
+        cache_base = static_cast<size_t>(kv_ring_row(b, g, a.Hkv, a.S)) * DH;
+        page_stride = DH;
+    } else {
+        cache_base = a.kv_page ? static_cast<size_t>(g) * kKvPage * DH
+                               : ((static_cast<size_t>(b) * a.Hkv + g) * a.S + lo) * DH;
+        page_stride = static_cast<size_t>(a.kv_page ? a.Hkv : 1) * kKvPage * DH;
+    }
 
     for (int e = threadIdx.x; e < G * DH; e += kAttnThreads) {
         const int gg = e / DH, d = e - gg * DH;
@@ -1042,8 +1061,16 @@ int launch_qkv_prep(const QkvPrepArgs& a, cudaStream_t st) {
     if (a.rows <= 0) return 0;
     FSB_CHECK(a.Dh % 64 == 0 && a.Dh <= 256, "qkv_prep: head_dim %d unsupported", a.Dh);
     FSB_CHECK((a.ld & 1) == 0 && (reinterpret_cast<uintptr_t>(a.y) & 7) == 0, "qkv_prep: misaligned GEMM result");
-    if (a.Dh == 64) FSB_LAUNCH(qkv_prep_row_kernel<64>, dim3(a.rows), dim3(kQkvRowThreads), 0, st, a);
-    else if (a.Dh == 128) FSB_LAUNCH(qkv_prep_row_kernel<128>, dim3(a.rows), dim3(kQkvRowThreads), 0, st, a);
+    if (a.ring) {
+        FSB_CHECK(a.kv_page == nullptr && a.S > 0 && a.S % kKvPage == 0 && (a.Dh == 64 || a.Dh == 128),
+                  "qkv_prep: a ring cache needs S a multiple of %d (S=%d), head_dim 64 or 128 and no page table", kKvPage,
+                  a.S);
+        if (a.Dh == 64) FSB_LAUNCH((qkv_prep_row_kernel<64, true>), dim3(a.rows), dim3(kQkvRowThreads), 0, st, a);
+        else FSB_LAUNCH((qkv_prep_row_kernel<128, true>), dim3(a.rows), dim3(kQkvRowThreads), 0, st, a);
+        return 0;
+    }
+    if (a.Dh == 64) FSB_LAUNCH((qkv_prep_row_kernel<64, false>), dim3(a.rows), dim3(kQkvRowThreads), 0, st, a);
+    else if (a.Dh == 128) FSB_LAUNCH((qkv_prep_row_kernel<128, false>), dim3(a.rows), dim3(kQkvRowThreads), 0, st, a);
     else FSB_LAUNCH(qkv_prep_kernel, dim3(a.rows, a.H + 2 * a.Hkv), dim3(a.Dh / 2), 0, st, a);
     return 0;
 }
@@ -1077,7 +1104,8 @@ static int launch_attn_t(const AttnArgs& a, cudaStream_t st) {
     lcap = attn_score_chunk<DH, G>(lcap, pages);
     const size_t smem = attn_smem_bytes<DH, G>(lcap, pages);
     const float scale = 1.0f / sqrtf(static_cast<float>(DH));
-    FSB_LAUNCH((attn_kernel<DH, G>), dim3(a.Hkv, a.rows), dim3(kAttnThreads), smem, st, a, scale, lcap);
+    if (a.ring) FSB_LAUNCH((attn_kernel<DH, G, true>), dim3(a.Hkv, a.rows), dim3(kAttnThreads), smem, st, a, scale, lcap);
+    else FSB_LAUNCH((attn_kernel<DH, G, false>), dim3(a.Hkv, a.rows), dim3(kAttnThreads), smem, st, a, scale, lcap);
     return 0;
 }
 
@@ -1085,7 +1113,8 @@ int attn_init() {
     static bool done = false;
     if (done) return 0;
 #define FSB_ATTN_ATTR(DH_, G_) \
-    FSB_CUDA(cudaFuncSetAttribute(attn_kernel<DH_, G_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
+    FSB_CUDA(cudaFuncSetAttribute(attn_kernel<DH_, G_, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
+    FSB_CUDA(cudaFuncSetAttribute(attn_kernel<DH_, G_, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
     FSB_CUDA(cudaFuncSetAttribute(attn_decode_kernel<DH_, G_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     FSB_ATTN_ATTR(128, 1) FSB_ATTN_ATTR(128, 2) FSB_ATTN_ATTR(128, 4) FSB_ATTN_ATTR(128, 8)
     FSB_ATTN_ATTR(64, 1) FSB_ATTN_ATTR(64, 2) FSB_ATTN_ATTR(64, 4) FSB_ATTN_ATTR(64, 8)
@@ -1122,6 +1151,9 @@ int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st) {
 int launch_attn(const AttnArgs& a, cudaStream_t st) {
     if (a.rows <= 0) return 0;
     FSB_CHECK(a.kv_page == nullptr || a.window <= 0, "attention: a paged KV cache takes no window");
+    FSB_CHECK(!a.ring || (a.kv_page == nullptr && a.S > 0 && a.S % kKvPage == 0 && a.window > 0 && a.window < a.S),
+              "attention: a ring cache needs S a multiple of %d (S=%d) and 0 < window < S (window=%d)", kKvPage, a.S,
+              a.window);
     // one kernel whatever the number of rows: a sequence must get the same bits alone, in a batch or in pieces
     if (!g_attn_per_row && attn_tile_supported(a)) return launch_attn_tile(a, st);
     const int G = a.H / a.Hkv;

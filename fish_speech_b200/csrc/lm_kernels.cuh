@@ -72,6 +72,14 @@ __device__ __forceinline__ long long kv_offset(const int* kv_page, int kv_page_l
     const int pg = kv_page[static_cast<size_t>(b) * kv_page_ld + pos / kKvPage];
     return pg < 0 ? -1 : ((static_cast<long long>(pg) * Hkv + g) * kKvPage + pos % kKvPage) * Dh;
 }
+// A third layout, the ring (`ring` != 0 in the argument blocks below; codec streaming, DecodeStreamPool): a contiguous
+// block per sequence of S + kKvPage rows, [seqs][Hkv][S + kKvPage][Dh], S a multiple of kKvPage. Position p (any p >= 0)
+// lives in row p % S; rows [0, kKvPage) are mirrored in rows [S, S + kKvPage), so that any kKvPage consecutive positions
+// are consecutive rows from the row of the first. Only the latest S positions of a sequence are kept: a window
+// attention needs S >= window + (positions appended in one call) - 1.
+__device__ __forceinline__ long long kv_ring_row(int b, int g, int Hkv, int S) {
+    return (static_cast<long long>(b) * Hkv + g) * (S + kKvPage);
+}
 
 // q,k,v = rbf(y [+bias]); optional per-head nn.RMSNorm (single rounding); interleaved RoPE in
 // fp32 with bf16 tables; q -> qbuf[row][H][Dh]; k,v -> the cache at (row_seq, row_pos) (see kv_offset).
@@ -91,6 +99,7 @@ struct QkvPrepArgs {
     int kv_page_ld;
     int rows, H, Hkv, Dh, S;
     float eps;
+    int ring;  // 1: the cache is a ring of S positions (kv_ring_row); head_dim 64 or 128, no page table
 };
 int launch_qkv_prep(const QkvPrepArgs& a, cudaStream_t st);
 
@@ -111,6 +120,7 @@ struct AttnArgs {
     int window;  // <=0: unlimited
     int lcap;    // score-buffer length: an upper bound of (row_pos + 1); 0 = cache capacity S
     int bf16_math;
+    int ring;    // 1: the cache is a ring of S positions (kv_ring_row); needs 0 < window < S and no page table
 };
 int launch_attn(const AttnArgs& a, cudaStream_t st);
 // csrc/attn_tile.cu: 64 rows of one head per CTA, K/V tiles staged once, mma.sync tensor cores, online softmax; what

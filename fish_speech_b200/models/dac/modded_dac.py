@@ -116,6 +116,7 @@ class DAC:
         self._bufs: dict = {}
         self._graphs: dict = {}   # (B, S, T) -> (CUDAGraph, static index buffer, static waveform) of from_indices
         self._graph_seen: dict = {}
+        self._ws_gen = 0  # bumped whenever a workspace or the RoPE table is re-allocated (stream pools drop their graphs)
         # decoder ResidualUnits as one kernel each (csrc/codec_resunit.cu); False = two conv GEMM launches per unit
         self._fused_units = True
         self._lock = threading.RLock()
@@ -326,6 +327,7 @@ class DAC:
             if b is not None:
                 self._graphs.clear()  # captured graphs point into the buffer that is being replaced
                 self._graph_seen.clear()
+                self._ws_gen += 1
             b = torch.empty(max(numel, 1), dtype=dtype, device=self._device)
             self._bufs[name] = b
         return b
@@ -352,16 +354,20 @@ class DAC:
             if t is not None:
                 self._graphs.clear()  # captured graphs point into the table that is being replaced
                 self._graph_seen.clear()
+                self._ws_gen += 1
             t = new
             self._rope[key] = t
         return t
 
     def _transformer(self, tf: dict, x: torch.Tensor, B: int, T: int, tag: str, pos0: int = 0,
-                     kv_cache: Optional[list] = None, cache_len: int = 0) -> torch.Tensor:
+                     kv_cache: Optional[list] = None, cache_len: int = 0, rows_at: Optional[tuple] = None,
+                     ring: bool = False, rope_len: int = 0) -> torch.Tensor:
         """WindowLimitedTransformer.forward on x = flat [B*T, D] bf16 (updated in place as the residual
         stream); returns the final-normed tensor (a workspace view).
         Incremental use (DecodeStream): the T rows are positions pos0 .. pos0+T-1 of a longer sequence whose earlier
-        K/V live in `kv_cache` = per layer (K, V) buffers [B][H][cache_len][Dh]; the window attention reads them."""
+        K/V live in `kv_cache` = per layer (K, V) buffers [B][H][cache_len][Dh]; the window attention reads them.
+        DecodeStreamPool: `rows_at` = (sequence, position) int32 device tensors of the B*T rows, `kv_cache` per layer
+        ring buffers of `cache_len` positions (ring=True, see fsb_qkv_rope_ring), positions below `rope_len`."""
         t: TfmConfig = tf["cfg"]
         D, H, Dh, I = t.dim, t.n_head, t.head_dim, t.intermediate_size
         rows = B * T
@@ -375,16 +381,19 @@ class DAC:
         vc = self._buf("tf_v", rows * H * Dh)
         att = self._buf("tf_att", rows * H * Dh)
         hb = self._buf("tf_h", rows * I)
-        # (sequence, position) of every row: two persistent int32 buffers refilled per call (a per-(B, T) cache
-        # would grow without bound over a dataset-scale bulk encode, where almost every batch has a new shape)
-        seq = self._buf("tf_seq", rows, torch.int32)[:rows]
-        pos = self._buf("tf_pos", rows, torch.int32)[:rows]
-        ar = torch.arange(rows, dtype=torch.int32, device=self._device)
-        torch.div(ar, T, rounding_mode="floor", out=seq)
-        torch.remainder(ar, T, out=pos)
-        if pos0:
-            pos += pos0
-        freqs = self._rope_table(pos0 + T, Dh, t.rope_base)
+        if rows_at is not None:
+            seq, pos = rows_at
+        else:
+            # (sequence, position) of every row: two persistent int32 buffers refilled per call (a per-(B, T) cache
+            # would grow without bound over a dataset-scale bulk encode, where almost every batch has a new shape)
+            seq = self._buf("tf_seq", rows, torch.int32)[:rows]
+            pos = self._buf("tf_pos", rows, torch.int32)[:rows]
+            ar = torch.arange(rows, dtype=torch.int32, device=self._device)
+            torch.div(ar, T, rounding_mode="floor", out=seq)
+            torch.remainder(ar, T, out=pos)
+            if pos0:
+                pos += pos0
+        freqs = self._rope_table(max(pos0 + T, rope_len), Dh, t.rope_base)
         window = t.window_size if t.window_size is not None else 0
         layers = tf["layers"]
         chk = _lib.check
@@ -394,10 +403,16 @@ class DAC:
             if kv_cache is not None:
                 kc, vc = kv_cache[l]
             chk(L.fsb_linear_f32(n.data_ptr(), rows, D, lw["wqkv"].data_ptr(), 3 * H * Dh, ws.data_ptr(), st))
-            chk(L.fsb_qkv_rope(ws.data_ptr(), rows, H, H, Dh, freqs.data_ptr(), seq.data_ptr(), pos.data_ptr(),
-                               q.data_ptr(), kc.data_ptr(), vc.data_ptr(), S, st))
-            chk(L.fsb_window_attn(q.data_ptr(), kc.data_ptr(), vc.data_ptr(), seq.data_ptr(), pos.data_ptr(), rows,
-                                  H, H, Dh, S, window, att.data_ptr(), st))
+            if ring:
+                chk(L.fsb_qkv_rope_ring(ws.data_ptr(), rows, H, H, Dh, freqs.data_ptr(), seq.data_ptr(), pos.data_ptr(),
+                                        q.data_ptr(), kc.data_ptr(), vc.data_ptr(), S, 1, st))
+                chk(L.fsb_window_attn_ring(q.data_ptr(), kc.data_ptr(), vc.data_ptr(), seq.data_ptr(), pos.data_ptr(),
+                                           rows, H, H, Dh, S, window, 1, att.data_ptr(), st))
+            else:
+                chk(L.fsb_qkv_rope(ws.data_ptr(), rows, H, H, Dh, freqs.data_ptr(), seq.data_ptr(), pos.data_ptr(),
+                                   q.data_ptr(), kc.data_ptr(), vc.data_ptr(), S, st))
+                chk(L.fsb_window_attn(q.data_ptr(), kc.data_ptr(), vc.data_ptr(), seq.data_ptr(), pos.data_ptr(), rows,
+                                      H, H, Dh, S, window, att.data_ptr(), st))
             chk(L.fsb_linear_f32(att.data_ptr(), rows, H * Dh, lw["wo"].data_ptr(), D, ws.data_ptr(), st))
             chk(L.fsb_resid_scale_norm(ws.data_ptr(), D, lw["ls_attn"].data_ptr(), x.data_ptr(), x.data_ptr(),
                                        lw["ffn_norm"].data_ptr(), n.data_ptr(), rows, D, t.norm_eps, 0, st))
@@ -480,6 +495,12 @@ class DAC:
         """Incremental `from_indices` (SURVEY §8(f).3): push code frames as the LM emits them, get their samples back.
         The codec is causal (rvq.py:395-398 asserts it), so what a frame sounds like never depends on later frames."""
         return DecodeStream(self, batch, max_frames, conv_context)
+
+    def open_stream_pool(self, slots: int, k_max: int = 32, max_graphs: int = 8) -> "DecodeStreamPool":
+        """Streaming decode of up to `slots` independent streams at once: streams join and leave at any push, and one
+        push decodes the new frames of every stream that has some in one batched (graph-replayed) pass. Each stream's
+        audio is bit-identical to `from_indices` of its codes alone. See DecodeStreamPool."""
+        return DecodeStreamPool(self, slots, k_max, max_graphs)
 
     @torch.inference_mode()
     def decode(self, z: torch.Tensor) -> torch.Tensor:
@@ -688,6 +709,292 @@ class DecodeStream:
             self.pos += k
             dac._idx_keepalive = idx
             return wav[:, :, c * dac.frame_length:]
+
+
+def _pow2(n: int) -> int:
+    return 1 << max(0, int(n) - 1).bit_length()
+
+
+class DecodeStreamPool:
+    """Streaming `from_indices` of up to `slots` independent streams (one utterance each), decoded together; a push
+    computes only the new frames of the streams in it.
+
+    * post-transformer: per slot and layer a K/V ring of R = round_up(window + k_max + 63, 64) positions
+      (fsb_qkv_rope_ring / fsb_window_attn_ring): the attention walks the same absolute 64-position tiles as over a
+      linear cache, so the result is the same; memory is fixed per slot and a stream has no length cap.
+    * upsampler + decoder: every causal conv keeps its own left context per slot, the last (taps - 1) * dilation rows
+      of its input in the form the conv reads it (Snake-activated where the Snake is fused upstream): ConvTranspose 1
+      row, ConvNeXt depthwise 6, the dilated k7 convs 6 * d, the final conv K - 1. A layer's input is a window
+      [stream][H + new rows][C]: fsb_window_fill puts the slot's history in rows 0..H-1 and the producer's new rows after
+      it, the consumer computes only the new rows (conv GEMM taps shifted by H, fsb_dwconv_ln_window), and
+      fsb_window_roll keeps the last H valid rows as the slot's next history. At stream start the history is zeros, as
+      the zero fill at negative time of the one-shot decode. The decoder's ResidualUnits run as their two conv GEMMs
+      (bit-identical to the fused kernel); the final conv runs over the window and its history rows are dropped.
+    * ragged pushes: the streams are padded to the largest frame count; padding rows follow a stream's valid rows, so
+      a causal layer never carries them into a valid row, and the roll takes valid rows only. Padding rows of the
+      transformer attend in a scratch sequence of their own. Slots outside a push are not touched.
+    * each (stream bucket, frame bucket) shape, powers of two, is captured into a CUDA graph the second time it is seen
+      (at most `max_graphs`; others run eagerly), on the calling thread.
+    * a push that fails leaves the state of its slots undefined: they refuse further pushes until closed.
+    """
+
+    def __init__(self, dac: "DAC", slots: int, k_max: int, max_graphs: int):
+        t: TfmConfig = dac.post_tfm["cfg"]
+        if slots < 1 or k_max < 1:
+            raise ValueError(f"stream pool needs slots >= 1 and k_max >= 1 (got {slots}, {k_max})")
+        if not t.window_size or t.window_size <= 0:
+            raise ValueError("stream pool needs a window-limited post-transformer")
+        self.dac, self.slots, self.k_max, self.max_graphs = dac, int(slots), int(k_max), int(max_graphs)
+        self.ring = _pad64(t.window_size + self.k_max + 63)
+        dev = dac.device
+        # slot `slots` is the scratch sequence of padding rows
+        n = (self.slots + 1) * t.n_head * (self.ring + 64) * t.head_dim
+        self.kv = [(torch.zeros(n, dtype=torch.bfloat16, device=dev), torch.zeros(n, dtype=torch.bfloat16, device=dev))
+                   for _ in dac.post_tfm["layers"]]
+        # one (H rows, C channels, rows per frame) per conv input of the upsampler + decoder, in execution order
+        self.layers = self._layer_geometry()
+        self.hist = [torch.zeros(max(1, self.slots * H * Cc), dtype=torch.bfloat16, device=dev)
+                     for H, Cc, _ in self.layers]
+        self.rates = sorted({r for _, _, r in self.layers})
+        self.pos = [0] * self.slots
+        self.live = [False] * self.slots
+        self.broken = [False] * self.slots
+        self._graphs: dict = {}  # (nb, kb) -> (CUDAGraph, static waveform)
+        self._seen: dict = {}
+        self._gen = dac._ws_gen
+        self._static: dict = {}  # (nb, kb) -> (idx, meta) device buffers the pass reads
+        self._shifts: dict = {}
+
+    def _layer_geometry(self) -> list:
+        dac, D = self.dac, self.dac.cfg.latent_dim
+        out, r = [], 1
+        for u in dac.up:
+            out.append((-min(u["conv"].shifts), D, r))
+            r *= u["f"]
+            out.append((u["cnx"]["k"] - 1, D, r))
+        out.append((-min(dac.dec_in.shifts), D, r))
+        cin = dac.cfg.decoder_dim
+        for blk in dac.dec_blocks:
+            out.append((-min(blk["up"].shifts), cin, r))
+            r *= blk["stride"]
+            cin //= 2
+            for ru in blk["res"]:
+                assert ru["c1"].taps == 1
+                out.append((-min(ru["c7"].shifts), cin, r))
+        out.append((dac.dec_out_k - 1, cin, r))
+        return out
+
+    @property
+    def state_bytes(self) -> int:
+        """Device memory of the per-slot state (K/V rings and per-layer conv history)."""
+        return sum(t.numel() * t.element_size() for kv in self.kv for t in kv) + \
+            sum(h.numel() * h.element_size() for h in self.hist)
+
+    def open(self) -> int:
+        with self.dac._lock, torch.cuda.device(self.dac.device):
+            for s in range(self.slots):
+                if not self.live[s]:
+                    for (H, Cc, _), h in zip(self.layers, self.hist):
+                        if H:
+                            h[s * H * Cc: (s + 1) * H * Cc].zero_()  # zero history = the one-shot's zero fill
+                    self.live[s], self.broken[s], self.pos[s] = True, False, 0
+                    return s
+        raise ValueError(f"stream pool is full ({self.slots} slots)")
+
+    def close(self, slot: int) -> None:
+        with self.dac._lock:
+            self._check_slot(slot)
+            self.live[slot] = False
+
+    def n_open(self) -> int:
+        return sum(self.live)
+
+    def _check_slot(self, slot) -> None:
+        if not isinstance(slot, int) or not 0 <= slot < self.slots or not self.live[slot]:
+            raise ValueError(f"slot {slot!r} is not an open stream of this pool")
+
+    @torch.inference_mode()
+    def push(self, pieces: dict) -> dict:
+        """{slot: codes [1+n_codebooks, k]} (1 <= k <= k_max) of the next frames of each stream -> {slot: waveform fp32
+        [k * frame_length]}. The caller's tensors are not modified."""
+        dac, cfg = self.dac, self.dac.cfg
+        S_ = dac.n_stage
+        items = list(pieces.items())
+        for slot, codes in items:
+            self._check_slot(slot)
+            if self.broken[slot]:
+                raise ValueError(f"slot {slot}: an earlier push failed, its state is lost; close the slot")
+            if codes.ndim != 2 or codes.shape[0] != S_:
+                raise ValueError(f"slot {slot}: codes must be [{S_}, k], got {tuple(codes.shape)}")
+            if not 1 <= codes.shape[1] <= self.k_max:
+                raise ValueError(f"slot {slot}: {codes.shape[1]} frames, a push takes 1 .. {self.k_max}")
+        if not items:
+            return {}
+        n = len(items)
+        ks = [int(c.shape[1]) for _, c in items]
+        nb = min(_pow2(n), self.slots)
+        kb = min(_pow2(max(ks)), self.k_max)
+        FL = dac.frame_length
+        scratch = self.slots
+        with dac._lock, torch.cuda.device(dac.device):
+            # ---- host-side description of the push: rows, positions, slots and valid rows per rate ----
+            row_seq = [scratch] * (nb * kb)
+            row_pos = [j for _ in range(nb) for j in range(kb)]
+            slot_of = [-1] * nb
+            valid = {r: [0] * nb for r in self.rates}
+            for i, ((slot, _), k) in enumerate(zip(items, ks)):
+                p = self.pos[slot]
+                slot_of[i] = slot
+                for j in range(k):
+                    row_seq[i * kb + j], row_pos[i * kb + j] = slot, p + j
+                for r in self.rates:
+                    valid[r][i] = k * r
+            meta_h = torch.tensor(row_seq + row_pos + slot_of + [v for r in self.rates for v in valid[r]],
+                                  dtype=torch.int32)
+            idx_h = torch.zeros(nb, S_, kb, dtype=torch.int32)
+            for i, (_, codes) in enumerate(items):
+                idx_h[i, :, : ks[i]] = codes.to(device="cpu", dtype=torch.int32)
+            idx_h[:, 0].clamp_(min=0, max=cfg.semantic_codebook_size - 1)  # rvq.py:354-359 (on our copy)
+            idx_h[:, 1:].clamp_(min=0, max=cfg.codebook_size - 1)
+            # ---- the RoPE table must cover every position before a graph captures its address ----
+            t: TfmConfig = dac.post_tfm["cfg"]
+            top = max(self.pos[s] + k for (s, _), k in zip(items, ks))
+            rope_len = max(1024, _pow2(max(top, kb)))
+            dac._rope_table(rope_len, t.head_dim, t.rope_base)
+            if self._gen != dac._ws_gen:  # a workspace a graph points into was re-allocated
+                self._graphs.clear()
+                self._seen.clear()
+                self._gen = dac._ws_gen
+            key = (nb, kb)
+            st = self._static.get(key)
+            if st is None:
+                st = (torch.empty(nb * S_ * kb, dtype=torch.int32, device=dac.device),
+                      torch.empty(meta_h.numel(), dtype=torch.int32, device=dac.device))
+                self._static[key] = st
+            try:
+                st[0].copy_(idx_h.reshape(-1))
+                st[1].copy_(meta_h)
+                hit = self._graphs.get(key)
+                if hit is not None:
+                    hit[0].replay()
+                    wav = hit[1]
+                else:
+                    seen = self._seen.get(key, 0)
+                    self._seen[key] = seen + 1
+                    if seen == 0 or len(self._graphs) >= self.max_graphs:
+                        wav = self._body(nb, kb, st, rope_len)
+                    else:
+                        torch.cuda.current_stream().synchronize()
+                        graph = torch.cuda.CUDAGraph()
+                        with torch.cuda.graph(graph, capture_error_mode="thread_local"):  # other threads keep running
+                            wav = self._body(nb, kb, st, rope_len)
+                        if self._gen != dac._ws_gen:
+                            raise RuntimeError("stream pool: a workspace was re-allocated during graph capture")
+                        self._graphs[key] = (graph, wav)
+                        graph.replay()
+                out = {slot: wav[i, : k * FL].clone() for i, ((slot, _), k) in enumerate(zip(items, ks))}
+            except BaseException:
+                for slot, _ in items:  # the device work may have advanced part of their state
+                    self.broken[slot] = True
+                raise
+            for slot, k in zip(pieces, ks):
+                self.pos[slot] += k
+            return out
+
+    def _gemm_win(self, cv: _Conv, win: torch.Tensor, nb: int, H: int, n: int, c_in: int, out0=None, out1=None,
+                  snake: Optional[_Snake] = None, resid=None):
+        """Conv GEMM over a window [nb][H + n][c_in]: only the n new rows, taps shifted by the H history rows."""
+        sh = self._shifts.get((id(cv), H))
+        if sh is None:
+            sh = (C.c_int * cv.taps)(*[v + H for v in cv.shifts])
+            self._shifts[(id(cv), H)] = sh
+        vp = lambda t: None if t is None else t.data_ptr()
+        _lib.check(self.dac.lib.fsb_conv_gemm(
+            win.data_ptr(), nb, H + n, c_in, c_in, (H + n) * c_in, cv.w.data_ptr(), cv.c_out, cv.taps, cv.kpad, sh, n,
+            vp(cv.bias), None, vp(resid), 0, vp(out0), vp(out1),
+            snake.alpha.data_ptr() if snake is not None else None,
+            snake.inv.data_ptr() if snake is not None else None, 0, _stream()))
+
+    def _body(self, nb: int, kb: int, st: tuple, rope_len: int) -> torch.Tensor:
+        """The device work of one push (eager or under capture): codes -> transformer (ring K/V) -> upsampler + decoder,
+        each conv on a window of its slot's history + the new rows -> waveform [nb, kb * frame_length]."""
+        dac, cfg = self.dac, self.dac.cfg
+        L, chk = dac.lib, _lib.check
+        S_, D = dac.n_stage, cfg.latent_dim
+        idx, meta = st
+        rows = nb * kb
+        row_seq, row_pos, slot_t = meta[:rows], meta[rows: 2 * rows], meta[2 * rows: 2 * rows + nb]
+        valid = {r: meta[2 * rows + nb * (1 + j): 2 * rows + nb * (2 + j)] for j, r in enumerate(self.rates)}
+        z = dac._buf("pl_z", rows * D)
+        chk(L.fsb_codebook_sum(idx.data_ptr(), dac.vq_tab_ptrs.data_ptr(), dac.vq_sizes.data_ptr(), S_, nb, kb, D,
+                               z.data_ptr(), _stream()))
+        x = dac._transformer(dac.post_tfm, z, nb, kb, "post", kv_cache=self.kv, cache_len=self.ring,
+                             rows_at=(row_seq, row_pos), ring=True, rope_len=rope_len)
+        layer = iter(range(len(self.layers)))
+
+        def window(dense: torch.Tensor, n: int):
+            """The next layer's input window from its new rows `dense` [nb][n][C]; rolls the slot's history."""
+            li = next(layer)
+            H, Cc, r = self.layers[li]
+            win = dac._buf("pl_win", nb * (H + n) * Cc)
+            chk(L.fsb_window_fill(self.hist[li].data_ptr(), dense.data_ptr(), win.data_ptr(), slot_t.data_ptr(),
+                                  valid[r].data_ptr(), nb, H, n, Cc * 2, _stream()))
+            chk(L.fsb_window_roll(win.data_ptr(), self.hist[li].data_ptr(), slot_t.data_ptr(), valid[r].data_ptr(),
+                                  nb, H, n, Cc * 2, _stream()))
+            return win, H
+
+        n = kb
+        for i, u in enumerate(dac.up):
+            win, H = window(x, n)
+            out = dac._buf(f"pl_up_{i}", nb * n * u["f"] * D)
+            self._gemm_win(u["conv"], win, nb, H, n, D, out0=out)
+            n *= u["f"]
+            cn = u["cnx"]
+            win, H = window(out, n)
+            y = dac._buf("pl_cnx_y", nb * n * D)
+            h = dac._buf("pl_cnx_h", nb * n * 4 * D)
+            chk(L.fsb_dwconv_ln_window(win.data_ptr(), cn["dw"].data_ptr(), cn["dw_b"].data_ptr(), cn["ln_w"].data_ptr(),
+                                       cn["ln_b"].data_ptr(), nb, H + n, H, n, D, cn["k"], 1e-6, y.data_ptr(),
+                                       _stream()))
+            dac._gemm(cn["pw1"], y, nb, n, D, n, out0=h, act=1)
+            dac._gemm(cn["pw2"], h, nb, n, 4 * D, n, out0=out, gamma=cn["gamma"], resid=out)
+            x = out
+        c = cfg.decoder_dim
+        numel = nb * n * c
+        for s_ in cfg.decoder_rates:
+            numel = max(numel, nb * n * s_ * c // 2)
+            n, c = n * s_, c // 2
+        n = kb * int(math.prod(cfg.downsample_factor))
+        bufs = {k: dac._buf(f"pl_dec_{k}", numel) for k in ("a0", "a1", "x", "m")}
+        win, H = window(x, n)
+        first = dac.dec_blocks[0]
+        self._gemm_win(dac.dec_in, win, nb, H, n, cfg.latent_dim, out1=bufs["a0"], snake=first["s_in"])
+        a, spare = "a0", "a1"
+        cin = cfg.decoder_dim
+        for bi, blk in enumerate(dac.dec_blocks):
+            cout = cin // 2
+            win, H = window(bufs[a], n)
+            self._gemm_win(blk["up"], win, nb, H, n, cin, out0=bufs["x"], out1=bufs[spare], snake=blk["up_snake"])
+            a, spare = spare, a
+            n *= blk["stride"]
+            for j, ru in enumerate(blk["res"]):
+                if j < 2:
+                    nxt = blk["res"][j + 1]["s0"]
+                elif bi + 1 < len(dac.dec_blocks):
+                    nxt = dac.dec_blocks[bi + 1]["s_in"]
+                else:
+                    nxt = dac.dec_out_snake
+                win, H = window(bufs[a], n)
+                self._gemm_win(ru["c7"], win, nb, H, n, cout, out1=bufs["m"], snake=ru["s1"])
+                dac._gemm(ru["c1"], bufs["m"], nb, n, cout, n, out0=bufs["x"] if j < 2 else None, out1=bufs[spare],
+                          snake=nxt, resid=bufs["x"])
+                a, spare = spare, a
+            cin = cout
+        win, H = window(bufs[a], n)
+        wav = torch.empty(nb, H + n, dtype=torch.float32, device=dac.device)
+        chk(L.fsb_final_conv_tanh(win.data_ptr(), dac.dec_out_w.data_ptr(), dac.dec_out_b, nb, H + n, cin,
+                                  dac.dec_out_k, wav.data_ptr(), _stream()))
+        return wav[:, H:]
 
 
 class _SnakeView:

@@ -259,6 +259,32 @@ int fsb_window_attn(const void* d_q, const void* d_k, const void* d_v, const int
                     const int32_t* d_row_pos, int rows, int H, int Hkv, int Dh, int S, int window, void* d_out,
                     void* stream);
 int fsb_swiglu_f32(const float* d_y, int rows, int I, void* d_h, void* stream);
+/* The same K/V append and window attention over a RING cache when ring != 0 (streaming decode of unbounded length):
+ * per (sequence, KV head) S + 64 rows, S a multiple of 64; position p (any p >= 0) is row p % S and rows [0, 64) are
+ * mirrored in rows [S, S + 64). Only the latest S positions are kept, so the attention needs 0 < window < S and
+ * S >= window + (positions appended per sequence in one call) - 1. Same terms in the same order as over a linear cache:
+ * the results are bit-identical to fsb_qkv_rope / fsb_window_attn with a cache long enough to hold every position.
+ * head_dim 64 or 128. ring == 0: exactly fsb_qkv_rope / fsb_window_attn. */
+int fsb_qkv_rope_ring(const float* d_qkv, int rows, int H, int Hkv, int Dh, const void* d_freqs,
+                      const int32_t* d_row_seq, const int32_t* d_row_pos, void* d_q, void* d_k, void* d_v, int S,
+                      int ring, void* stream);
+int fsb_window_attn_ring(const void* d_q, const void* d_k, const void* d_v, const int32_t* d_row_seq,
+                         const int32_t* d_row_pos, int rows, int H, int Hkv, int Dh, int S, int window, int ring,
+                         void* d_out, void* stream);
+/* Per-layer stream windows (DecodeStreamPool): a layer's input is viewed per stream as [H + n][row] with rows 0..H-1
+ * its carried causal history. fsb_window_fill writes win [nb][H + n][row]: rows 0..H-1 from state [slots][H][row] at
+ * d_slot[i], rows H..H+d_valid[i]-1 from the producer's dense output [nb][n][row]; other rows are left as they are
+ * (padding after the valid rows). fsb_window_roll writes the last H valid rows (window rows d_valid[i] ..
+ * d_valid[i]+H-1) back to the slot's state. A negative slot skips the stream. row_bytes a multiple of 16. */
+int fsb_window_fill(const void* d_state, const void* d_dense, void* d_win, const int32_t* d_slot,
+                    const int32_t* d_valid, int nb, int H, int n, int row_bytes, void* stream);
+int fsb_window_roll(const void* d_win, void* d_state, const int32_t* d_slot, const int32_t* d_valid, int nb, int H,
+                    int n, int row_bytes, void* stream);
+/* fsb_dwconv_ln over such a window: output row t = input row origin + t of x [B][T_in][C] (its history = the rows
+ * before it); y [B][T_out][C]. origin + T_out <= T_in. */
+int fsb_dwconv_ln_window(const void* d_x, const float* d_w, const float* d_bias, const float* d_ln_w,
+                         const float* d_ln_b, int B, int T_in, int origin, int T_out, int C, int K, float eps, void* d_y,
+                         void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Unit-test hooks (used by tests/ only)

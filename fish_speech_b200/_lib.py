@@ -78,6 +78,10 @@ def lib() -> C.CDLL:
     L.fsb_lm_reset.argtypes = [vp, vp]
     L.fsb_lm_set_context_bound.argtypes = [vp, i32]
     L.fsb_lm_set_slot_control.argtypes = [vp, i32]
+    L.fsb_lm_slot_blob_bytes.argtypes = [vp]
+    L.fsb_lm_slot_blob_bytes.restype = C.c_size_t
+    L.fsb_lm_slot_save.argtypes = [vp, i32, vp, vp]
+    L.fsb_lm_slot_restore.argtypes = [vp, i32, vp, vp]
     L.fsb_lm_buffer.argtypes = [vp, C.c_char_p, C.POINTER(vp), C.POINTER(C.c_size_t)]
     L.fsb_lm_set_sampler_noise.argtypes = [vp, vp, i32, i32]
     L.fsb_lm_copy_kv.argtypes = [vp, i32, i32, i32, vp]

@@ -700,6 +700,37 @@ int fsb_lm_set_slot_control(fsb_lm* h, int enable) {
     return 0;
 }
 
+size_t fsb_lm_slot_blob_bytes(fsb_lm* h) {
+    if (h == nullptr) return 0;
+    return slot_blob_ints(h->cfg.num_codebooks + 1, h->cfg.max_frames) * sizeof(int);
+}
+
+// Neither call is part of the decode graph: the graph reads the per-slot arrays at run time, so it stays valid.
+static int slot_state_args(fsb_lm* h, int slot, const void* d_blob, const char* what, SlotStateArgs* a) {
+    FSB_CHECK(h != nullptr, "%s: null handle", what);
+    FSB_CHECK(h->slot_control, "%s: slot control is not enabled (fsb_lm_set_slot_control)", what);
+    FSB_CHECK(slot >= 0 && slot < h->cfg.max_batch, "%s: slot=%d outside [0, %d)", what, slot, h->cfg.max_batch);
+    FSB_CHECK(d_blob != nullptr, "%s: null blob", what);
+    FSB_CHECK((reinterpret_cast<uintptr_t>(d_blob) & 15) == 0, "%s: the blob must be 16-byte aligned", what);
+    *a = SlotStateArgs{h->slot_state, h->slot_limit, h->slot_temperature, h->slot_top_p, h->slot_top_k, h->slot_seed,
+                       h->n_out, h->pos, h->finished, h->ras_window, h->cur_tok, h->out_tokens,
+                       static_cast<int*>(const_cast<void*>(d_blob)), slot, h->cfg.num_codebooks + 1,
+                       h->cfg.max_frames};
+    return 0;
+}
+
+int fsb_lm_slot_save(fsb_lm* h, int slot, void* d_blob, void* stream) {
+    SlotStateArgs a{};
+    FSB_TRY(slot_state_args(h, slot, d_blob, "slot_save", &a));
+    return launch_slot_save(a, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int fsb_lm_slot_restore(fsb_lm* h, int slot, const void* d_blob, void* stream) {
+    SlotStateArgs a{};
+    FSB_TRY(slot_state_args(h, slot, d_blob, "slot_restore", &a));
+    return launch_slot_restore(a, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int fsb_lm_set_sampler_noise(fsb_lm* h, const float* d_u, int draws_per_frame, int ld) {
     FSB_CHECK(h != nullptr, "set_sampler_noise: null handle");
     FSB_CHECK(d_u == nullptr || (draws_per_frame >= 2 * h->cfg.num_codebooks && ld >= h->head_rows && ld >= h->cfg.codebook_size),

@@ -1025,6 +1025,57 @@ __global__ void kv_copy_kernel(uint4* cache, size_t layer16, size_t page16, size
     }
 }
 
+// Blob of one slot's request state (SlotStateArgs): kBlobScalars scalars, the RAS window, cur_tok[ncols], then the
+// out_tokens rows [ncols][T_cap] from a 16-byte boundary.
+constexpr int kBlobScalars = 10, kBlobRas = 10;
+__host__ __device__ inline int blob_head_ints(int ncols) { return (kBlobScalars + kBlobRas + ncols + 3) & ~3; }
+
+// CTA c moves row c of out_tokens (the n_out frames produced so far); CTA 0 also moves the scalars. SAVE: slot ->
+// blob, then the slot is parked; otherwise blob -> slot.
+template <bool SAVE>
+__global__ void slot_state_kernel(SlotStateArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int s = a.slot;
+    int* sc = a.blob;
+    int* ras = a.blob + kBlobScalars;
+    int* ct = ras + kBlobRas;
+    const int n = SAVE ? a.n_out[s] : sc[3];
+    const size_t row = static_cast<size_t>(blockIdx.x) * a.T_cap;
+    int* dev = a.out_tokens + static_cast<size_t>(s) * a.ncols * a.T_cap + row;
+    int* sav = a.blob + blob_head_ints(a.ncols) + row;
+    for (int f = threadIdx.x; f < n && f < a.T_cap; f += blockDim.x) {
+        if (SAVE) sav[f] = dev[f];
+        else dev[f] = sav[f];
+    }
+    if (blockIdx.x != 0) return;
+    const int t = threadIdx.x;
+    if (t < kBlobRas) {
+        if (SAVE) ras[t] = a.ras_window[s * kBlobRas + t];
+        else a.ras_window[s * kBlobRas + t] = ras[t];
+    }
+    if (t >= 32 && t - 32 < a.ncols) {
+        if (SAVE) ct[t - 32] = a.cur_tok[s * a.ncols + t - 32];
+        else a.cur_tok[s * a.ncols + t - 32] = ct[t - 32];
+    }
+    if (t != 0) return;
+    if (SAVE) {
+        const unsigned long long seed = a.seed[s];
+        sc[0] = a.state[s]; sc[1] = a.limit[s]; sc[2] = a.top_k[s]; sc[3] = a.n_out[s]; sc[4] = a.pos[s];
+        sc[5] = a.finished[s];
+        sc[6] = __float_as_int(a.temperature[s]); sc[7] = __float_as_int(a.top_p[s]);
+        sc[8] = static_cast<int>(seed & 0xffffffffull); sc[9] = static_cast<int>(seed >> 32);
+        a.state[s] = 0;
+        a.pos[s] = -1;
+    } else {
+        a.state[s] = sc[0]; a.limit[s] = sc[1]; a.top_k[s] = sc[2]; a.n_out[s] = sc[3]; a.pos[s] = sc[4];
+        a.finished[s] = sc[5];
+        a.temperature[s] = __int_as_float(sc[6]); a.top_p[s] = __int_as_float(sc[7]);
+        a.seed[s] = static_cast<unsigned long long>(static_cast<unsigned int>(sc[8])) |
+                    (static_cast<unsigned long long>(static_cast<unsigned int>(sc[9])) << 32);
+    }
+}
+
 __global__ void step_inc_kernel(unsigned long long* step) {
     pdl_launch_dependents();
     pdl_wait();
@@ -1193,6 +1244,22 @@ int launch_kv_copy(__nv_bfloat16* cache, int layers, int n_pages, int Hkv, int D
     const int n16 = n_pos * (Dh / 8);
     FSB_LAUNCH(kv_copy_kernel, dim3(cdiv(n16, 256 * 4), Hkv, layers), dim3(256), 0, st,
                reinterpret_cast<uint4*>(cache), layer16, page16, head16, src_tab, src0, dst_tab, dst0, n16);
+    return 0;
+}
+
+size_t slot_blob_ints(int ncols, int T_cap) {
+    return static_cast<size_t>(blob_head_ints(ncols)) + static_cast<size_t>(ncols) * T_cap;
+}
+
+int launch_slot_save(const SlotStateArgs& a, cudaStream_t st) {
+    FSB_CHECK(a.ncols >= 1 && a.ncols <= 224, "slot_save: %d token rows unsupported", a.ncols);
+    FSB_LAUNCH(slot_state_kernel<true>, dim3(a.ncols), dim3(256), 0, st, a);
+    return 0;
+}
+
+int launch_slot_restore(const SlotStateArgs& a, cudaStream_t st) {
+    FSB_CHECK(a.ncols >= 1 && a.ncols <= 224, "slot_restore: %d token rows unsupported", a.ncols);
+    FSB_LAUNCH(slot_state_kernel<false>, dim3(a.ncols), dim3(256), 0, st, a);
     return 0;
 }
 

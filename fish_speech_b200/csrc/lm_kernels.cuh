@@ -244,4 +244,22 @@ int launch_frame_end(const FrameEndArgs& a, cudaStream_t st);
 int launch_kv_copy(__nv_bfloat16* cache, int layers, int n_pages, int Hkv, int Dh, const int* src_tab, int src0,
                    const int* dst_tab, int dst0, int n_pos, cudaStream_t st);
 
+// Everything a decode frame reads back from the previous one for one slot, gathered into / scattered from one blob of
+// slot_blob_ints(ncols, T_cap) int32: the slot-control scalars, the frame counter, position, finished flag, RAS window,
+// the frame's tokens and the frames produced so far (out_tokens[slot][:, :n_out]). Saving also parks the slot
+// (state 0, pos -1: the following frames neither attend for the row nor write its K/V). The slow K/V stays where it
+// is, in the pages the slot maps; the fast K/V is rebuilt every frame.
+struct SlotStateArgs {
+    int *state, *limit;
+    float *temperature, *top_p;
+    int* top_k;
+    unsigned long long* seed;
+    int *n_out, *pos, *finished, *ras_window, *cur_tok, *out_tokens;
+    int* blob;
+    int slot, ncols, T_cap;
+};
+size_t slot_blob_ints(int ncols, int T_cap);
+int launch_slot_save(const SlotStateArgs& a, cudaStream_t st);
+int launch_slot_restore(const SlotStateArgs& a, cudaStream_t st);
+
 }  // namespace fsb

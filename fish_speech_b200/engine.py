@@ -4,6 +4,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+from dataclasses import dataclass
 from typing import Optional, Sequence
 
 import numpy as np
@@ -76,7 +77,9 @@ class KvPagePool:
     mapped by several slots (a shared prompt prefix); `ref[page]` counts them and a page returns to the free list when
     the count drops to 0. A slot is live (reserved for a request that may still write) or retired: a retired slot keeps
     its pages mapped, as a prefix later requests may reuse, until an allocation needs them; retired slots are then
-    released least recently retired first, and `on_reclaim(slot)` lets the owner forget what the slot held.
+    released least recently retired first, and `on_reclaim(slot)` lets the owner forget what the slot held. A row can
+    also be detached: taken out of the table with its page references, for a request that is parked between two frames
+    and continues later in whichever slot is idle then.
 
     Device effects are callbacks, so that the rules can run without a GPU: `copy_page(src, dst, n)` copies positions
     [0, n) of a page, stream-ordered before the writes that follow."""
@@ -89,6 +92,7 @@ class KvPagePool:
         self.ref = np.zeros(n_pages, dtype=np.int32)
         self.free = list(range(n_pages - 1, -1, -1))  # popped from the end: page 0 first
         self.retired: dict[int, None] = {s: None for s in range(slots)}  # insertion order = retirement order
+        self.detached: list[np.ndarray] = []  # rows of parked requests: they keep their page references, in no slot
         self.copy_page = copy_page or (lambda src, dst, n: None)
         self.on_reclaim = on_reclaim or (lambda slot: None)
         self.dirty = True
@@ -101,7 +105,7 @@ class KvPagePool:
     def available(self) -> int:
         """Pages a reservation can get: free ones plus those that only retired slots map."""
         live = [s for s in range(self.slots) if s not in self.retired]
-        pages = self.table[live]
+        pages = np.concatenate([self.table[live].ravel(), *self.detached])
         return self.n_pages - len(np.unique(pages[pages >= 0]))
 
     # ---- mapping ------------------------------------------------------------------------------------------------
@@ -122,6 +126,43 @@ class KvPagePool:
     def retire(self, slot: int):
         """`slot` will not write again until its next reservation; its pages stay mapped until needed."""
         self.retired.setdefault(slot, None)
+
+    # ---- parked requests: a page-table row outside every slot -------------------------------------------------------
+    def detach(self, slot: int) -> np.ndarray:
+        """Take the live `slot`'s row out of the table, with its page references: the pages count as live in
+        `available()` and no reservation reclaims them (only rows of retired slots are released), while the slot, now
+        mapping nothing, is free for another request. Pages other slots map too stay shared. No K/V moves."""
+        if slot in self.retired:
+            raise ValueError(f"slot {slot} is retired: only a live slot's pages can be detached")
+        row = self.table[slot].copy()
+        self.table[slot] = -1
+        self.detached.append(row)
+        self.retired[slot] = None
+        self.dirty = True
+        return row
+
+    def _undetach(self, row: np.ndarray):
+        k = next((i for i, r in enumerate(self.detached) if r is row), None)
+        if k is None:
+            raise ValueError("not a detached row of this pool (or already attached / dropped)")
+        del self.detached[k]
+
+    def attach(self, slot: int, row: np.ndarray):
+        """Map a detached row into `slot`, which runs no request: the pages it still maps (a retired prefix) are
+        released first, and the slot becomes live."""
+        self._undetach(row)
+        self.retired.pop(slot, None)
+        self.release(slot)
+        self.on_reclaim(slot)
+        self.table[slot] = row
+        self.dirty = True
+
+    def drop(self, row: np.ndarray):
+        """Give up a detached row: its references are released, pages nobody else maps return to the free list."""
+        self._undetach(row)
+        pages = row[row >= 0]
+        self.ref[pages] -= 1
+        self.free.extend(pages[self.ref[pages] == 0].tolist())
 
     def hold(self, slot: int, end: int, start: int = 0):
         """Make `slot` live without mapping anything yet, and release its pages past position `end` as well as the
@@ -195,6 +236,18 @@ class KvPagePool:
         for j in missing:
             row[j] = self._take()
         self.peak = max(self.peak, self.in_use())
+
+
+@dataclass(eq=False)
+class ParkedSlot:
+    """A request taken out of its slot between two frames (LmEngine.park_slot): everything it needs to continue in
+    any slot of the same engine. Its K/V stays in the pool pages `row` references; nothing was copied."""
+
+    blob: torch.Tensor  # device bytes written by fsb_lm_slot_save
+    row: np.ndarray  # its detached page-table row (KvPagePool.detach)
+    tokens: Optional[torch.Tensor]  # prompt rows whose K/V the pages hold, for prefix reuse once it has a slot again
+    covered: Optional[int]  # pages its reservation mapped
+    ctx_len: int  # upper bound of its context length, kept for the scheduler
 
 
 class LmEngine:
@@ -431,6 +484,35 @@ class LmEngine:
     def retire_slot(self, slot: int):
         """The slot's request is done: its pages stay mapped as a reusable prefix until the pool needs them."""
         self.kv_pool.retire(int(slot))
+
+    def park_slot(self, slot: int, ctx_len: int = 0) -> ParkedSlot:
+        """Take the request running in `slot` out of it, between two frames: its per-slot decode state goes into a
+        device blob (one small kernel, which also idles the row), its page-table row is detached with its pages, and
+        the slot is free for another request. `resume_slot` continues it in any slot with the same bits."""
+        slot = int(slot)
+        with torch.cuda.device(self.device):
+            blob = torch.empty(int(self.lib.fsb_lm_slot_blob_bytes(self.h)), dtype=torch.uint8, device=self.device)
+            _lib.check(self.lib.fsb_lm_slot_save(self.h, slot, blob.data_ptr(), _stream()))
+        parked = ParkedSlot(blob, self.kv_pool.detach(slot), self._slot_tokens.pop(slot, None),
+                            self._covered.pop(slot, None), int(ctx_len))
+        self._reserve([])  # the emptied row reaches the device before the slot's next request
+        return parked
+
+    def resume_slot(self, slot: int, parked: ParkedSlot):
+        """Continue a parked request in `slot` (idle; what it still maps as a retired prefix is released)."""
+        slot = int(slot)
+        self.kv_pool.attach(slot, parked.row)
+        if parked.tokens is not None:
+            self._slot_tokens[slot] = parked.tokens
+        if parked.covered is not None:
+            self._covered[slot] = parked.covered
+        self._reserve([])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.fsb_lm_slot_restore(self.h, slot, parked.blob.data_ptr(), _stream()))
+
+    def drop_parked(self, parked: ParkedSlot):
+        """A parked request will not continue: its pages go back to the pool."""
+        self.kv_pool.drop(parked.row)
 
     def release_kv(self):
         """Forget every slot's K/V: all pages return to the pool."""

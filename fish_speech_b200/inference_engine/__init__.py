@@ -265,6 +265,9 @@ class TTSInferenceEngine(ReferenceLoader, VQManager):
                     yield hand_out(wav)
         finally:
             chunk.close()  # a request that ends inside a chunk (error, abandoned generator) gives its pool slot back
+            cancel = getattr(responses, "cancel", None)
+            if cancel is not None:
+                cancel.set()  # ... and its LM slot: the slot scheduler takes a request still in flight out
         if not finished:
             yield InferenceResult(code="error", audio=None,
                                   error=RuntimeError("No audio generated, please check the input text."))
@@ -283,6 +286,7 @@ class TTSInferenceEngine(ReferenceLoader, VQManager):
         if req.streaming and self.stream_frames > 0:
             request["stream_frames"] = self.stream_frames
         response_queue: queue.Queue = queue.Queue()
+        response_queue.cancel = request["cancel"] = threading.Event()  # set when the caller stops listening
         self.llama_queue.put(GenerateRequest(request=request, response_queue=response_queue))
         return response_queue
 

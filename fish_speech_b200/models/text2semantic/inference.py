@@ -494,20 +494,51 @@ class GenerateRequest:
     response_queue: queue.Queue
 
 
+# Frames per second a listener plays: the codec's sample_rate / frame_length (models/dac/modded_dac.py).
+PLAYBACK_FRAMES_PER_S = 44100 / 2048
+
+
 def serve_requests(model, input_queue: "queue.Queue", max_slots: int, frames_per_poll: int = 8,
                    batcher=None) -> None:
     """Worker loop of the slot scheduler: every queued request's `generate_long` plan advances concurrently,
     their `generate` calls share the decode frames (fish_speech_b200/scheduler.py). Responses of one request
     arrive in the reference's order on its own response queue; `None` shuts the loop down once the running
-    requests are finished."""
-    from ...scheduler import ContinuousBatcher, SlotRequest
+    requests are finished.
+
+    FSB_SERVE_LIVE=n (n > max_slots) lets up to n requests be live at a time: streaming requests
+    (`stream_frames`) are then paced at playback speed, one playback clock per request across its chunks, so
+    that the scheduler parks the ones far ahead of their listener and gives their slots to the ones about to run
+    dry. A request dict may carry `cancel` (a threading.Event): once it is set the request in flight is taken out
+    of the scheduler, the plan ends and nothing more is put on its response queue."""
+    from ...scheduler import Cancelled, ContinuousBatcher, SlotRequest, StreamClock
 
     if batcher is None:
-        batcher = ContinuousBatcher(model, max_slots=max_slots, frames_per_poll=frames_per_poll)
+        max_live = max(max_slots, int(os.environ.get("FSB_SERVE_LIVE", "0") or 0))
+        batcher = ContinuousBatcher(model, max_slots=max_slots, frames_per_poll=frames_per_poll, max_live=max_live)
+    paced = getattr(batcher, "max_live", 0) > getattr(batcher, "max_slots", 0)
     live = 0  # plans not yet exhausted
     waiting_queues: dict = {}  # id(plan) -> response queue of every plan that has a generate call in flight
-    streaming: set = set()  # id(plan) of requests that asked for partial codes (`stream_frames`)
+    streaming: dict = {}  # id(plan) -> playback clock of requests that asked for partial codes (`stream_frames`)
+    cancels: dict = {}  # id(plan) -> (cancel event, plan) of requests that carry one
+    inflight: dict = {}  # id(plan) -> the SlotRequest of its generate call in flight
     closing = False
+
+    def end(plan):
+        nonlocal live
+        live -= 1
+        streaming.pop(id(plan), None)
+        cancels.pop(id(plan), None)
+        inflight.pop(id(plan), None)
+
+    def finished(r, plan, response_queue):
+        inflight.pop(id(plan), None)
+        if r.error is None:
+            return advance(plan, response_queue, r.result)
+        waiting_queues.pop(id(plan), None)
+        plan.close()
+        if not isinstance(r.error, Cancelled):
+            response_queue.put(WrappedGenerateResponse(status="error", response=r.error))
+        end(plan)
 
     def advance(plan, response_queue, reply):
         """Run a plan until it asks for the next `generate` (submitted to the batcher) or ends."""
@@ -527,21 +558,21 @@ def serve_requests(model, input_queue: "queue.Queue", max_slots: int, frames_per
                     def on_frames(r, codes, q=response_queue):
                         q.put(WrappedGenerateResponse(status="success",
                                                       response=GenerateResponse(action="partial", codes=codes)))
-                batcher.submit(SlotRequest(
+                pace = dict(pace=PLAYBACK_FRAMES_PER_S, stream=streaming[id(plan)]) if paced and on_frames else {}
+                inflight[id(plan)] = req = SlotRequest(
                     prompt=payload["prompt"], max_new_tokens=payload["max_new_tokens"],
                     temperature=payload["temperature"], top_p=payload["top_p"], top_k=payload["top_k"],
                     seed=_next_seed(model), reuse_prefix=bool(payload.get("reuse_prefix", False)), on_frames=on_frames,
-                    on_done=lambda r, plan=plan, q=response_queue: advance(plan, q, r.result)))
+                    on_done=lambda r, plan=plan, q=response_queue: finished(r, plan, q), **pace)
+                batcher.submit(req)
                 waiting_queues[id(plan)] = response_queue
                 return
         except StopIteration:
-            live -= 1
-            streaming.discard(id(plan))
+            end(plan)
         except Exception as e:
             logger.error(traceback.format_exc())
             response_queue.put(WrappedGenerateResponse(status="error", response=e))
-            live -= 1
-            streaming.discard(id(plan))
+            end(plan)
 
     try:
         while True:
@@ -557,14 +588,19 @@ def serve_requests(model, input_queue: "queue.Queue", max_slots: int, frames_per
                 live += 1
                 try:
                     plan = _generate_long_plan(model=model, **{k: v for k, v in item.request.items()
-                                                               if k not in ("decode_one_token", "stream_frames")})
+                                                               if k not in ("decode_one_token", "stream_frames", "cancel")})
                 except Exception as e:  # pragma: no cover - argument errors surface on first send
                     item.response_queue.put(WrappedGenerateResponse(status="error", response=e))
                     live -= 1
                     continue
                 if item.request.get("stream_frames", 0):
-                    streaming.add(id(plan))
+                    streaming[id(plan)] = StreamClock()
+                if item.request.get("cancel") is not None:
+                    cancels[id(plan)] = (item.request["cancel"], plan)
                 advance(plan, item.response_queue, None)
+            for event, plan in list(cancels.values()):
+                if event.is_set() and id(plan) in inflight:
+                    batcher.cancel(inflight[id(plan)])  # -> finished(): the plan ends without another response
             if live == 0 and closing:
                 return
             try:
@@ -673,6 +709,7 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
             kwargs = dict(item.request)
             response_queue = item.response_queue
             on_partial = None
+            kwargs.pop("cancel", None)  # requests are served one at a time here: nothing to give back early
             if kwargs.pop("stream_frames", 0):
                 # streaming request (TTSInferenceEngine with req.streaming): codes leave the worker as frames finish
                 def on_partial(codes, q=response_queue):

@@ -7,16 +7,35 @@ share every decode frame: a request is prefilled into a free slot while the othe
 its stop rule runs on the device, and its slot is handed to the next waiting request as soon as it
 finishes. The kernels are batch-invariant and a request's random stream depends on its own seed and
 frame index only, so every request returns exactly the tokens `generate` would return for it alone.
+
+Paced requests (`SlotRequest.pace`, frames per second the consumer plays) let an engine serve more live streams
+than it has slots: a slot produces frames several times faster than they are heard, so a stream that is far
+enough ahead of its playback is parked between two polls (its K/V stays in its pool pages, nothing is copied) and
+its slot serves a stream that is about to run dry; `schedule_live` is the whole policy.
 """
 from __future__ import annotations
 
 import threading
+import time
 from dataclasses import dataclass, field
-from typing import Callable, Optional
+from typing import Callable, NamedTuple, Optional, Sequence
 
 import torch
 
 from .engine import MAX_DECODE_BATCH, bf16_round, kv_pages_for
+
+
+class Cancelled(Exception):
+    """`SlotRequest.error` of a request taken out by `ContinuousBatcher.cancel`."""
+
+
+@dataclass
+class StreamClock:
+    """Playback clock of one utterance, shared by the requests (chunks) that make it up: a later chunk continues the
+    clock of the frames already handed out instead of starting as a new arrival."""
+
+    t_first: Optional[float] = None  # when the first frames were handed out
+    frames: int = 0  # frames handed out so far
 
 
 @dataclass(eq=False)  # identity semantics: requests hold tensors
@@ -35,6 +54,9 @@ class SlotRequest:
     # whole request exactly result[1:, T:-1] (what generate_long keeps, inference.py:708), before on_done
     on_frames: Optional[Callable[["SlotRequest", torch.Tensor], None]] = None
     tag: object = None
+    # frames per second the consumer plays; None: FIFO admission, never parked
+    pace: Optional[float] = None
+    stream: Optional[StreamClock] = None  # one per utterance (made at submit when a paced request has none)
     # filled by the batcher
     result: Optional[torch.Tensor] = None  # [C+1, T+n] like generate()
     error: Optional[BaseException] = None
@@ -43,14 +65,81 @@ class SlotRequest:
     _limit: int = 0
     _emitted: int = 0
     _host_prompt: Optional[torch.Tensor] = None  # the prompt on the host, for page-limited admission with reuse
+    _t_submit: float = 0.0
+    _parked: object = None  # engine.ParkedSlot while the request is live without a slot
+    parks: int = 0
+    resumes: int = 0
+
+    def lead(self, now: float) -> float:
+        """Frames the consumer holds beyond what it has played at `now` (negative: it is waiting for frames). An
+        unpaced request has no playback clock: it is always due."""
+        if self.pace is None:
+            return float("-inf")
+        st = self.stream
+        if st is None or st.t_first is None:
+            return -self.pace * (now - self._t_submit)
+        return st.frames - self.pace * (now - st.t_first)
+
+
+# Policy thresholds, in polls (multiples of `frames_per_poll` frames of lead). They are choices, not measurements.
+# A parked request gets a slot back once less than RESUME_POLLS polls of audio are left with its consumer: after the
+# resume its next frames are final one poll later, and a poll of frames takes several times longer to play than to
+# make, so one poll of lead is enough not to run dry. A running request may be parked once it is PARK_POLLS polls
+# ahead: low enough that a request reaches it well before an utterance of a few seconds ends, or nothing is ever
+# parked. The gap of three polls is what keeps requests from flapping: a resumed request gains less than one poll of
+# lead per poll (the consumer plays meanwhile), so it runs at least three polls before it can be parked again, and a
+# parked one plays three polls' worth of audio before it needs a slot.
+RESUME_POLLS = 1
+PARK_POLLS = 4
+
+
+class LivePlan(NamedTuple):
+    park: list  # running requests that give up their slot now
+    resume: list  # parked requests that get a slot, in this order, before any admission
+    admit: list  # waiting requests in admission order (as many as may be admitted)
+    fill: list  # parked requests for slots that are still free after the admissions
+
+
+def schedule_live(running: Sequence[SlotRequest], parked: Sequence[SlotRequest], waiting: Sequence[SlotRequest],
+                  now: float, slots: int, max_live: int, frames_per_poll: int) -> LivePlan:
+    """Who runs for the next poll: a pure function of the requests and the clock.
+
+    1. Only when no slot is free and a paced request below the resume threshold is parked or waiting: the running
+       paced requests at or above the park threshold give up their slots, largest lead first, at most one per such
+       candidate. An unpaced request is never parked.
+    2. Parked requests below the resume threshold get slots, smallest lead first.
+    3. Waiting requests are admitted while slots and `max_live` (running + parked) allow: overdue paced ones
+       (negative lead) first, smallest lead first, then everything else in order of arrival.
+    Slots still free after that go to parked requests, smallest lead first: a slot never idles while work exists."""
+    resume_at, park_at = RESUME_POLLS * frames_per_poll, PARK_POLLS * frames_per_poll
+    by_lead = lambda rs: sorted(rs, key=lambda r: r.lead(now))  # stable: ties keep their order
+    due = by_lead(r for r in parked if r.lead(now) < resume_at)
+    room = max_live - len(running) - len(parked)
+    starting = [r for r in waiting if r.pace is not None and r.lead(now) < resume_at][:max(room, 0)]
+    free = slots - len(running)
+    park = []
+    if free <= 0 and (due or starting):
+        ahead = by_lead(r for r in running if r.pace is not None and r.lead(now) >= park_at)[::-1]
+        park = ahead[:len(due) + len(starting)]
+        free += len(park)
+    resume = due[:max(free, 0)]
+    free -= len(resume)
+    overdue = by_lead(r for r in waiting if r.pace is not None and r.lead(now) < 0)
+    order = overdue + [r for r in waiting if not (r.pace is not None and r.lead(now) < 0)]
+    admit = order[:max(min(free, room), 0)]
+    rest = [r for r in by_lead(parked) if not any(r is x for x in resume)]
+    return LivePlan(park, resume, admit, rest)
 
 
 class ContinuousBatcher:
-    def __init__(self, model, max_slots: int = 32, frames_per_poll: int = 8, min_free_to_admit: int = 1):
+    def __init__(self, model, max_slots: int = 32, frames_per_poll: int = 8, min_free_to_admit: int = 1,
+                 max_live: Optional[int] = None, clock: Callable[[], float] = time.monotonic):
         """`frames_per_poll`: decode frames between two looks at the device-side slot states (a finished slot
         idles for at most that many frames). `min_free_to_admit`: admissions wait until that many slots are
         free (or nothing is running) — every admission is one extra prefill pass + first frame that streams
-        all weights for the new rows only, so grouping them trades admission latency for throughput."""
+        all weights for the new rows only, so grouping them trades admission latency for throughput.
+        `max_live`: the most requests admitted at a time, running plus parked; the default, `max_slots`, means
+        nothing is ever parked. `clock`: the time source of the pacing policy (seconds)."""
         from .models.text2semantic.inference import _ensure_engine
 
         if not 1 <= max_slots <= MAX_DECODE_BATCH:
@@ -59,6 +148,11 @@ class ContinuousBatcher:
         self.cfg = model.config
         self.eng = _ensure_engine(model, max_slots)
         self.max_slots = max_slots
+        self.max_live = max_slots if max_live is None else int(max_live)
+        if self.max_live < max_slots:
+            raise ValueError(f"max_live must be >= max_slots ({max_slots}), got {max_live}")
+        self.clock = clock
+        self.parked: list[SlotRequest] = []  # admitted, between two polls without a slot (SlotRequest._parked)
         self.frames_per_poll = int(frames_per_poll)
         self.min_free_to_admit = max(1, int(min_free_to_admit))
         self.waiting: list[SlotRequest] = []
@@ -118,27 +212,106 @@ class ContinuousBatcher:
         if pool is not None and kv_pages_for(T + n) > pool.n_pages:
             raise ValueError(f"{T} prompt rows + {n} frames need {kv_pages_for(T + n)} KV pages, more than the "
                              f"engine's whole pool of {pool.n_pages} (kv_pages)")
+        if req.pace is not None:
+            if not float(req.pace) > 0.0:
+                raise ValueError(f"pace must be > 0 frames per second, got {req.pace}")
+            if req.stream is None:
+                req.stream = StreamClock()
         req._limit = n
+        req._t_submit = self.clock()
         self.waiting.append(req)
         return req
 
     def idle(self) -> bool:
-        return not self.waiting and not self.active
+        return not self.waiting and not self.active and not self.parked
 
-    def _admit(self):
-        free = [s for s in range(self.max_slots) if s not in self.active]
-        if not free or not self.waiting:
+    def _free_slots(self) -> list[int]:
+        return [s for s in range(self.max_slots) if s not in self.active]
+
+    def _park(self, req: SlotRequest):
+        s = req.slot
+        req._parked = self.eng.park_slot(s, self._len.pop(s))
+        del self.active[s]
+        req.slot = -1
+        req.parks += 1
+        self.parked.append(req)
+
+    def _resume(self, req: SlotRequest, s: int):
+        self.parked.remove(req)
+        parked, req._parked = req._parked, None
+        self.eng.resume_slot(s, parked)
+        req.slot = s
+        req.resumes += 1
+        self.active[s] = req
+        self._len[s] = parked.ctx_len
+
+    def _schedule(self):
+        """One scheduling decision (schedule_live) carried out: park, resume, admit, fill."""
+        plan = schedule_live(list(self.active.values()), self.parked, self.waiting, self.clock(), self.max_slots,
+                             self.max_live, self.frames_per_poll)
+        for req in plan.park:
+            self._park(req)
+        free = self._free_slots()
+        for req in plan.resume:
+            self._resume(req, free.pop(0))
+        self._admit(plan.admit)
+        free = self._free_slots()
+        for req in plan.fill[:len(free)]:
+            self._resume(req, free.pop(0))
+
+    def cancel(self, req: SlotRequest) -> bool:
+        """Take `req` out wherever it is: waiting, running or parked. A running request's slot idles from the next
+        frame on and its pages stay a reusable prefix, as after a normal end; a parked one's pages go back to the
+        pool. `req.error` becomes a `Cancelled`, `done` / `on_done` fire; the other requests are unaffected.
+        False when the request is already done (or was never submitted here)."""
+        if req.done.is_set():
+            return False
+        if any(r is req for r in self.waiting):
+            self.waiting.remove(req)
+        elif self.active.get(req.slot) is req:
+            self._vacate([req])
+        elif req._parked is not None and any(r is req for r in self.parked):
+            self.parked.remove(req)
+            parked, req._parked = req._parked, None
+            self.eng.drop_parked(parked)
+        else:
+            return False
+        req.error = Cancelled("the request was cancelled")
+        req.done.set()
+        if req.on_done is not None:
+            req.on_done(req)
+        return True
+
+    def _vacate(self, reqs: list):
+        """The slots of `reqs` idle from the next frame on; their pages stay mapped as a reusable prefix."""
+        idx = torch.tensor([r.slot for r in reqs], dtype=torch.long, device=self._state.device)
+        self._state[idx] = 0
+        self._pos[idx] = -1  # parked: the decode frames neither attend for this row nor touch its K/V (which a
+        #                      later request with the same prompt prefix may reuse)
+        for r in reqs:
+            del self.active[r.slot]
+            del self._len[r.slot]
+            if hasattr(self.eng, "retire_slot"):
+                self.eng.retire_slot(r.slot)  # its pages stay a reusable prefix until the pool needs them
+
+    def _admit(self, order: Optional[list] = None):
+        """Admit the requests of `order` (from `waiting`; default: as they arrived), in that order, into free slots."""
+        order = list(self.waiting) if order is None else order
+        free = self._free_slots()
+        if not free or not order:
             return
         if self.active and len(free) < min(self.min_free_to_admit, len(self.waiting)):
             return
         batch, slots = [], []
         budget = self.eng.max_rows  # one prefill pass worth of rows per step keeps decode latency bounded
         pool = getattr(self.eng, "kv_pool", None)
-        # a pool with room for every slot at full capacity never runs out: no page accounting needed
-        paged = pool is not None and pool.n_pages < pool.slots * pool.pages_per_slot
+        # a pool with room for every slot at full capacity never runs out, unless parked requests hold pages beside
+        # the slots' own: otherwise no page accounting is needed
+        paged = pool is not None and (pool.n_pages < pool.slots * pool.pages_per_slot or self.max_live > self.max_slots)
         pages = self.eng.kv_pages_available() if paged else 0
-        while free and self.waiting:
-            head = self.waiting[0]
+        for head in order:
+            if not free:
+                break
             T = int(head.prompt.size(1))
             if batch and T > budget:
                 break
@@ -151,7 +324,8 @@ class ContinuousBatcher:
                 if need > pages:
                     break
                 pages -= need
-            req = self.waiting.pop(0)
+            req = head
+            self.waiting.remove(req)
             s = free.pop(0)
             req.slot = s
             batch.append(req)
@@ -188,11 +362,16 @@ class ContinuousBatcher:
         for s, req in self.active.items():
             # frames of a streaming request leave as soon as they are final: all but the newest one (the last frame of
             # a request -- <|im_end|> or the one at the budget -- is never part of what generate_long keeps)
-            if req.on_frames is None:
+            if req.on_frames is None and req.stream is None:
                 continue
             n = int(st[1, s])
             if n - 1 > req._emitted:
-                req.on_frames(req, self._out[s, 1:, req._emitted: n - 1].cpu())
+                if req.on_frames is not None:
+                    req.on_frames(req, self._out[s, 1:, req._emitted: n - 1].cpu())
+                if req.stream is not None:  # the playback clock starts with the first frames handed out
+                    if req.stream.t_first is None:
+                        req.stream.t_first = self.clock()
+                    req.stream.frames += n - 1 - req._emitted
                 req._emitted = n - 1
         finished = []
         for s, req in list(self.active.items()):
@@ -202,16 +381,8 @@ class ContinuousBatcher:
             gen = self._out[s, :, :n].to(req.prompt.dtype)
             req.result = torch.cat([req.prompt.to(gen.device), gen], dim=1)
             finished.append(req)
-            del self.active[s]
-            del self._len[s]
         if finished:
-            idx = torch.tensor([r.slot for r in finished], dtype=torch.long, device=self._state.device)
-            self._state[idx] = 0
-            self._pos[idx] = -1  # parked: the decode frames neither attend for this row nor touch its K/V (which a
-            #                      later request with the same prompt prefix may reuse)
-            for r in finished:
-                if hasattr(self.eng, "retire_slot"):
-                    self.eng.retire_slot(r.slot)  # its pages stay a reusable prefix until the pool needs them
+            self._vacate(finished)
         for req in finished:
             req.done.set()
             if req.on_done is not None:
@@ -219,8 +390,9 @@ class ContinuousBatcher:
         return finished
 
     def step(self) -> list[SlotRequest]:
-        """Admit waiting requests into free slots, run `frames_per_poll` frames, retire what finished."""
-        self._admit()
+        """Park / resume paced requests and admit waiting ones into free slots (schedule_live), run
+        `frames_per_poll` frames, retire what finished."""
+        self._schedule()
         if not self.active:
             return []
         k = self.frames_per_poll

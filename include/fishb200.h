@@ -163,6 +163,18 @@ int fsb_lm_set_context_bound(fsb_lm* h, int max_positions);
  * the same tokens alone or with any neighbours, in any slot. */
 int fsb_lm_set_slot_control(fsb_lm* h, int enable);
 
+/* Take a running request out of its slot between two decode frames and put it back later, into any slot, with the
+ * same bits (slot control must be enabled). fsb_lm_slot_save gathers what the frames keep per slot between frames
+ * (the slot-control arrays, frame counter, position, finished flag, RAS window, the last frame's tokens and
+ * "out_tokens"[slot][:, :n_out]) into a device blob of fsb_lm_slot_blob_bytes bytes (16-byte aligned), and parks the
+ * slot: state 0, position -1, so the frames that follow neither attend for the row nor write its K/V.
+ * fsb_lm_slot_restore scatters a blob into `slot`. Each is one small kernel on `stream`; the decode graph stays valid.
+ * The slow K/V is not part of the blob: it stays in the pages the slot mapped ("kv_page"), and the caller maps those
+ * pages into the slot it restores to. A blob is valid for the handle that wrote it. */
+size_t fsb_lm_slot_blob_bytes(fsb_lm* h);
+int fsb_lm_slot_save(fsb_lm* h, int slot, void* d_blob, void* stream);
+int fsb_lm_slot_restore(fsb_lm* h, int slot, const void* d_blob, void* stream);
+
 /* Reset per-slot generation state (frame counters, RAS window, finished flags, slot states). */
 int fsb_lm_reset(fsb_lm* h, void* stream);
 

@@ -20,7 +20,7 @@ class LmConfig(C.Structure):
         "semantic_begin_id", "semantic_end_id", "im_end_id")] + [("norm_eps", C.c_float)] + [
         (n, C.c_int) for n in (
             "qk_norm", "fast_qk_norm", "scale_codebook_embeddings", "norm_fastlayer_input",
-            "max_batch", "kv_len", "max_rows", "max_frames", "debug", "kv_pages")]
+            "max_batch", "kv_len", "max_rows", "max_frames", "debug", "kv_pages", "attn_split")]
 
 
 class LmLayer(C.Structure):

@@ -94,6 +94,7 @@ struct fsb_lm {
     bf16 *q_d = nullptr, *attn_d = nullptr, *h_d = nullptr, *hid_d = nullptr;
     float* step_ws = nullptr;
     size_t step_ws_floats = 0;
+    float* span_ws = nullptr;  // span records of the split attention (cfg.attn_split > 0), see AttnSplit
     // prefill workspaces
     bf16 *xres_p = nullptr, *xn_p = nullptr, *q_p = nullptr, *attn_p = nullptr, *h_p = nullptr;
     float* ws = nullptr;
@@ -232,6 +233,19 @@ AttnDecodeArgs decode_attn_args(const fsb_lm* h, const Stack& s, int l, const St
     return aa;
 }
 
+// Layer l's decode attention, the consumer of the qkv GEMM `qkv` ran. With cfg.attn_split set, a slow-stack launch
+// whose context bound exceeds it runs as the three kernels of launch_attn_decode_split; the base kernel's score
+// buffer then only has to hold the rows that are not split. Every other launch is the single attn_decode_kernel.
+int launch_decode_attn(const fsb_lm* h, const Stack& s, int l, const StepGemmPlan& qkv, int rows, const int* row_seq,
+                       const int* row_pos, bool kv_only, cudaStream_t st) {
+    AttnDecodeArgs aa = decode_attn_args(h, s, l, qkv, rows, row_seq, row_pos, kv_only);
+    const int span = h->cfg.attn_split;
+    const int bound = h->ctx_lcap > 0 ? h->ctx_lcap : s.S;
+    if (span <= 0 || s.bf16_math != 0 || bound <= span) return launch_attn_decode(aa, st);
+    aa.lcap = span;
+    return launch_attn_decode_split(aa, AttnSplit{h->q_d, h->span_ws, span, bound}, st);
+}
+
 // The first `upto` (GEMM, finalize) pairs of a layer after its attention: wo + residual add, w1|w3 + SwiGLU,
 // w2 + residual add.
 int run_layer_gemms(const StepLayer& P, int rows, int upto, cudaStream_t st) {
@@ -252,7 +266,7 @@ int run_stack_decode(fsb_lm* h, Stack& s, int rows, const int* row_seq, const in
         StepLayer& P = s.dec[l];
         FSB_TRY(step_gemm_launch(P.qkv, rows, st));
         const bool kv_only = stop_after_kv && l == s.nl - 1;  // fast pass 0 only fills the KV cache (inference.py:147)
-        FSB_TRY(launch_attn_decode(decode_attn_args(h, s, l, P.qkv, rows, row_seq, row_pos, kv_only), st));
+        FSB_TRY(launch_decode_attn(h, s, l, P.qkv, rows, row_seq, row_pos, kv_only, st));
         if (kv_only) return 0;
         FSB_TRY(run_layer_gemms(P, rows, 3, st));
     }
@@ -461,6 +475,14 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
               "head_dim must be 64 or 128");
     FSB_CHECK(w->head_rows == cfg->semantic_end_id - cfg->semantic_begin_id + 2, "head_rows mismatch");
     FSB_CHECK(cfg->kv_len >= 1 && cfg->kv_pages >= 0, "kv_len must be >= 1 and kv_pages >= 0");
+    if (cfg->attn_split != 0) {
+        const int most = attn_split_max_span(cfg->n_head, cfg->n_kv_head, cfg->head_dim);
+        FSB_CHECK(cfg->attn_split > 0 && cfg->attn_split % kKvPage == 0 && cfg->attn_split <= most,
+                  "attn_split=%d must be 0 (off) or a multiple of %d in [%d, %d] (what one span's scores fit in shared "
+                  "memory at head_dim %d, %d query heads per KV head)",
+                  cfg->attn_split, kKvPage, kKvPage, most, cfg->head_dim,
+                  cfg->n_kv_head > 0 ? cfg->n_head / cfg->n_kv_head : 0);
+    }
     fsb_lm* h = new fsb_lm();
     h->cfg = *cfg;
     int dev = 0;
@@ -542,7 +564,12 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &f.xres, static_cast<size_t>(RT) * f.D, "x_fast"));
     TRYC(dalloc(h, &f.ssq, static_cast<size_t>(RT) * kSsqStride, "ssq_fast"));
     TRYC(dalloc(h, &h->hid_d, static_cast<size_t>(RT) * Dm));
-    TRYC(dalloc(h, &h->q_d, static_cast<size_t>(RT) * Qm));
+    TRYC(dalloc(h, &h->q_d, static_cast<size_t>(RT) * Qm, "q"));
+    if (cfg->attn_split > 0)
+        TRYC(dalloc(h, &h->span_ws,
+                    static_cast<size_t>(cfg->max_batch) * s.Hkv * cdiv(cfg->kv_len, cfg->attn_split) *
+                        attn_span_floats(s.H / s.Hkv, s.Dh),
+                    "attn_span_ws"));
     TRYC(dalloc(h, &h->attn_d, static_cast<size_t>(RT) * Qm, "attn"));
     TRYC(dalloc(h, &h->h_d, static_cast<size_t>(RT) * Im, "ffn_h"));
     TRYC(dalloc(h, &h->xres_p, static_cast<size_t>(R) * s.D));
@@ -887,7 +914,7 @@ int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only
     // its operand is the residual stream as the caller left it, normalised on load
     const StepGemmPlan& qkv = s.dec[layer].qkv;
     FSB_TRY(step_gemm_launch(qkv, rows, st));
-    return launch_attn_decode(decode_attn_args(h, s, layer, qkv, rows, h->iota, h->pos, kv_only != 0), st);
+    return launch_decode_attn(h, s, layer, qkv, rows, h->iota, h->pos, kv_only != 0, st);
 }
 
 int fsb_lm_copy_kv(fsb_lm* h, int src_slot, int dst_slot, int n_pos, void* stream) {

@@ -574,8 +574,10 @@ __global__ void __launch_bounds__(kAttnThreads) attn_kernel(AttnArgs a, float sc
 // ------------------------------------------------------------------------------------------------
 // decode-step attention with the qkv GEMM's fix-up in front (see lm_kernels.cuh)
 // ------------------------------------------------------------------------------------------------
-template <int DH, int G>
-__global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArgs a, float scale, int lcap) {
+// SPLIT (attn_decode_split_kernel): a row of more than sp.span positions stops after the front end, its finished q heads
+// stored to sp.q for attn_span_kernel; every other row runs the code of SPLIT = false.
+template <int DH, int G, bool SPLIT>
+__device__ __forceinline__ void attn_decode_body(const AttnDecodeArgs a, const float scale, const int lcap, const AttnSplit sp) {
     pdl_launch_dependents();
     const int row = blockIdx.y, g = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -654,6 +656,7 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
         unmapped |= pt[j] < 0;
     }
     if (__syncthreads_or(unmapped)) return;  // unmapped history: nothing is written, nothing attended
+    const bool split_row = SPLIT && wpos + 1 > sp.span;
     // (cos, sin) of this lane's rotary pair at the row's position: the same for q and k
     const uint32_t cs = *reinterpret_cast<const uint32_t*>(a.freqs + (static_cast<size_t>(wpos) * (DH / 2) + (d >> 1)) * 2);
     // bias, the GEMM output's bf16 rounding, and per-head nn.RMSNorm (fp32 math, weight multiply included, ONE
@@ -699,18 +702,216 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArg
         if (live) {
             if (kind == 0) {
                 qs[hh * DH + d] = x;
+                if (split_row) sp.q[(static_cast<size_t>(row) * a.H + g * G + hh) * DH + d] = f2bf(x);  // x is a bf16 value
             } else if (rpos < a.S) {
                 __nv_bfloat16* cache = kind == 1 ? a.kcache : a.vcache;
                 cache[cache_base + pt[rpos / kKvPage] * page_stride + (rpos % kKvPage) * DH + d] = f2bf(x);
             }
         }
     }
-    if (a.kv_only) return;
+    if (a.kv_only || split_row) return;
     __syncthreads();  // q in shared memory, this row's new K/V visible to the whole CTA
 
     const int L = wpos + 1;
     attend<DH, G>(qs, sc, red, a.kcache + cache_base, a.vcache + cache_base, pt, page_stride, L, lcap, scale,
                   a.bf16_math, a.out + (static_cast<size_t>(row) * a.H + g * G) * DH);
+}
+
+template <int DH, int G>
+__global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArgs a, float scale, int lcap) {
+    attn_decode_body<DH, G, false>(a, scale, lcap, AttnSplit{});
+}
+
+template <int DH, int G>
+__global__ void __launch_bounds__(kAttnThreads) attn_decode_split_kernel(AttnDecodeArgs a, AttnSplit sp, float scale,
+                                                                         int lcap) {
+    attn_decode_body<DH, G, true>(a, scale, lcap, sp);
+}
+
+// A long row's page-table walk, shared by attn_span_kernel and attn_combine_kernel so that both take the same
+// decision: false when any page of positions [0, L) is not mapped (the row then attends to nothing, as in
+// attn_decode_kernel). Entries of pages [page0, page0 + npt) go to pt (the identity when the cache is contiguous).
+__device__ __forceinline__ bool split_row_pages(const AttnDecodeArgs& a, int row, int L, int page0, int npt, int* pt) {
+    const int* ptab = a.kv_page ? a.kv_page + static_cast<size_t>(a.row_seq[row]) * a.kv_page_ld : nullptr;
+    bool unmapped = false;
+    for (int j = threadIdx.x; j <= (L - 1) / kKvPage; j += kAttnThreads) {
+        const int pg = ptab ? ptab[j] : j;
+        unmapped |= pg < 0;
+        if (j >= page0 && j < page0 + npt) pt[j - page0] = pg;
+    }
+    return !__syncthreads_or(unmapped);
+}
+
+// One span of one long row (see AttnSplit): positions [p0, p0 + n) of KV group g against the row's G query heads. K is
+// read once: the span's scores stay in shared memory. Stores acc[G][DH] = sum_p exp(s_p - m) v_p, m = max_p s_p and
+// z = sum_p exp(s_p - m) per head. The loops are attend()'s one-pass ones over the span, so every lane and warp sums
+// a fixed sequence of terms that depends on the span's positions only.
+template <int DH, int G>
+__global__ void __launch_bounds__(kAttnThreads) attn_span_kernel(AttnDecodeArgs a, AttnSplit sp, float scale) {
+    static_assert(G <= kAttnWarps, "one warp per query head in the softmax");
+    pdl_launch_dependents();
+    pdl_wait();  // every CTA, the idle ones too: the kernels behind this one count on the whole chain of waits
+    const int g = blockIdx.x, row = blockIdx.y, p0 = blockIdx.z * sp.span;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int rpos = a.row_pos[row];
+    if (rpos < 0) return;  // parked
+    const int L = min(rpos, a.S - 1) + 1;
+    if (L <= sp.span || p0 >= L) return;  // a short row (attended by the front end), or a span past the row's end
+    const int n = min(sp.span, L - p0);
+    extern __shared__ float sm[];
+    float* qs = sm;                      // [G][DH]
+    float* sc = qs + G * DH;             // [G][span]
+    float* red = sc + G * sp.span;       // [kAttnWarps][G][DH]
+    int* pt = reinterpret_cast<int*>(red + kAttnWarps * G * DH);  // pages of the span
+    for (int e = threadIdx.x; e < G * DH; e += kAttnThreads)
+        qs[e] = bf2f(sp.q[(static_cast<size_t>(row) * a.H + g * G) * DH + e]);
+    if (!split_row_pages(a, row, L, p0 / kKvPage, sp.span / kKvPage, pt)) return;
+    const size_t cache_base = a.kv_page ? static_cast<size_t>(g) * kKvPage * DH
+                                        : (static_cast<size_t>(a.row_seq[row]) * a.Hkv + g) * a.S * DH;
+    const size_t page_stride = static_cast<size_t>(a.kv_page ? a.Hkv : 1) * kKvPage * DH;
+    const __nv_bfloat16* kc = a.kcache + cache_base;
+    const __nv_bfloat16* vc = a.vcache + cache_base;
+    const int lcap = sp.span;
+
+    constexpr int LPR = DH / 8;    // lanes per cache row (16-byte loads)
+    constexpr int RPW = 32 / LPR;  // rows per warp iteration
+    constexpr int UNR = 4;         // independent 16-byte loads in flight per lane
+    constexpr int DPL = DH / 32;   // value dims per lane
+    const int sub = lane / LPR, li = lane % LPR;
+    auto at = [&](const __nv_bfloat16* base, int p) {  // p relative to the span's first position, a page edge
+        return base + static_cast<size_t>(pt[p / kKvPage]) * page_stride + (p % kKvPage) * DH;
+    };
+    {
+        float qr[G][8];
+#pragma unroll
+        for (int gg = 0; gg < G; ++gg)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) qr[gg][e] = qs[gg * DH + li * 8 + e];
+        for (int pb = warp * RPW * UNR; pb < n; pb += kAttnWarps * RPW * UNR) {
+            uint4 u[UNR];
+            const __nv_bfloat16* kp = at(kc, pb);  // RPW * UNR positions from a multiple of 8: one page
+#pragma unroll
+            for (int j = 0; j < UNR; ++j) {
+                const int p = pb + j * RPW + sub;
+                u[j] = make_uint4(0, 0, 0, 0);
+                if (p < n) u[j] = *reinterpret_cast<const uint4*>(kp + (j * RPW + sub) * DH + li * 8);
+            }
+#pragma unroll
+            for (int j = 0; j < UNR; ++j) {
+                const int p = pb + j * RPW + sub;
+                const bool ok = p < n;
+                const float kf[8] = {bf_lo(u[j].x), bf_hi(u[j].x), bf_lo(u[j].y), bf_hi(u[j].y),
+                                     bf_lo(u[j].z), bf_hi(u[j].z), bf_lo(u[j].w), bf_hi(u[j].w)};
+#pragma unroll
+                for (int gg = 0; gg < G; ++gg) {
+                    float d = 0.f;
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) d += qr[gg][e] * kf[e];
+#pragma unroll
+                    for (int o = LPR / 2; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+                    if (ok && li == 0) sc[gg * lcap + p] = d * scale;
+                }
+            }
+        }
+    }
+    __syncthreads();
+    float* rec = sp.ws + ((static_cast<size_t>(row) * a.Hkv + g) * gridDim.z + blockIdx.z) * attn_span_floats(G, DH);
+    if (warp < G) {
+        float* s = sc + warp * lcap;
+        float m = -INFINITY, z = 0.f;
+        for (int p = lane; p < n; p += 32) m = fmaxf(m, s[p]);
+        m = warp_max(m);
+        for (int p = lane; p < n; p += 32) {
+            const float e = expf(s[p] - m);
+            s[p] = e;
+            z += e;
+        }
+        z = warp_sum(z);
+        if (lane == 0) {
+            rec[G * DH + warp] = m;
+            rec[G * DH + G + warp] = z;
+        }
+    }
+    __syncthreads();
+    float acc[G][DPL];
+#pragma unroll
+    for (int gg = 0; gg < G; ++gg)
+#pragma unroll
+        for (int e = 0; e < DPL; ++e) acc[gg][e] = 0.f;
+    for (int pb = warp; pb < n; pb += kAttnWarps * UNR) {
+        const __nv_bfloat16* vp = at(vc, pb);  // positions pb + 8 j, inside a run of 32 from a multiple of 32: one page
+        float vf[UNR][DPL];
+#pragma unroll
+        for (int j = 0; j < UNR; ++j) {
+            const int p = pb + j * kAttnWarps;
+#pragma unroll
+            for (int e = 0; e < DPL; ++e) vf[j][e] = 0.f;
+            if (p < n) {
+                if (DPL == 4) {
+                    const uint2 u2 = *reinterpret_cast<const uint2*>(vp + (j * kAttnWarps) * DH + lane * 4);
+                    vf[j][0] = bf_lo(u2.x); vf[j][1] = bf_hi(u2.x); vf[j][2 % DPL] = bf_lo(u2.y); vf[j][3 % DPL] = bf_hi(u2.y);
+                } else {
+                    const uint32_t u1 = *reinterpret_cast<const uint32_t*>(vp + (j * kAttnWarps) * DH + lane * 2);
+                    vf[j][0] = bf_lo(u1); vf[j][1] = bf_hi(u1);
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < UNR; ++j) {
+            const int p = pb + j * kAttnWarps;
+            if (p < n) {
+#pragma unroll
+                for (int gg = 0; gg < G; ++gg) {
+                    const float w = sc[gg * lcap + p];
+#pragma unroll
+                    for (int e = 0; e < DPL; ++e) acc[gg][e] += w * vf[j][e];
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int gg = 0; gg < G; ++gg)
+#pragma unroll
+        for (int e = 0; e < DPL; ++e) red[(warp * G + gg) * DH + lane * DPL + e] = acc[gg][e];
+    __syncthreads();
+    for (int e = threadIdx.x; e < G * DH; e += kAttnThreads) {
+        float s = 0.f;
+#pragma unroll
+        for (int w = 0; w < kAttnWarps; ++w) s += red[w * G * DH + e];
+        rec[e] = s;
+    }
+}
+
+// Merge of a long row's spans: with M = max_s m_s, out = (sum_s acc_s exp(m_s - M)) / (sum_s z_s exp(m_s - M)), both
+// sums in ascending span order, rounded to bf16 once. A kernel of its own rather than the last span CTA to arrive:
+// the order of the sum must not depend on which CTA finishes first.
+template <int DH, int G>
+__global__ void __launch_bounds__(kAttnThreads) attn_combine_kernel(AttnDecodeArgs a, AttnSplit sp) {
+    pdl_launch_dependents();
+    pdl_wait();  // every CTA: the wo GEMM behind this kernel waits on it for the rows of all three attention kernels
+    const int g = blockIdx.x, row = blockIdx.y;
+    const int rpos = a.row_pos[row];
+    if (rpos < 0) return;
+    const int L = min(rpos, a.S - 1) + 1;
+    if (L <= sp.span) return;
+    if (!split_row_pages(a, row, L, 0, 0, nullptr)) return;
+    constexpr int R = attn_span_floats(G, DH);
+    const int ns = (L + sp.span - 1) / sp.span, nspans = (sp.bound + sp.span - 1) / sp.span;
+    const float* rec = sp.ws + (static_cast<size_t>(row) * a.Hkv + g) * nspans * R;
+    __nv_bfloat16* out = a.out + (static_cast<size_t>(row) * a.H + g * G) * DH;
+    for (int e = threadIdx.x; e < G * DH; e += kAttnThreads) {
+        const int gg = e / DH;
+        float M = -INFINITY;
+        for (int s = 0; s < ns; ++s) M = fmaxf(M, rec[static_cast<size_t>(s) * R + G * DH + gg]);
+        float Z = 0.f, o = 0.f;
+        for (int s = 0; s < ns; ++s) {
+            const float* r = rec + static_cast<size_t>(s) * R;
+            const float w = expf(r[G * DH + gg] - M);
+            Z += r[G * DH + G + gg] * w;
+            o += r[e] * w;
+        }
+        out[e] = f2bf(o / Z);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1166,7 +1367,9 @@ int attn_init() {
 #define FSB_ATTN_ATTR(DH_, G_) \
     FSB_CUDA(cudaFuncSetAttribute(attn_kernel<DH_, G_, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
     FSB_CUDA(cudaFuncSetAttribute(attn_kernel<DH_, G_, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
-    FSB_CUDA(cudaFuncSetAttribute(attn_decode_kernel<DH_, G_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    FSB_CUDA(cudaFuncSetAttribute(attn_decode_kernel<DH_, G_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
+    FSB_CUDA(cudaFuncSetAttribute(attn_decode_split_kernel<DH_, G_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
+    FSB_CUDA(cudaFuncSetAttribute(attn_span_kernel<DH_, G_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     FSB_ATTN_ATTR(128, 1) FSB_ATTN_ATTR(128, 2) FSB_ATTN_ATTR(128, 4) FSB_ATTN_ATTR(128, 8)
     FSB_ATTN_ATTR(64, 1) FSB_ATTN_ATTR(64, 2) FSB_ATTN_ATTR(64, 4) FSB_ATTN_ATTR(64, 8)
 #undef FSB_ATTN_ATTR
@@ -1192,6 +1395,59 @@ int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st) {
     FSB_CHECK(a.H % a.Hkv == 0, "attention: H %% Hkv != 0");
 #define FSB_ATTN_CASE(DH_, G_) \
     if (a.Dh == DH_ && G == G_) return launch_attn_decode_t<DH_, G_>(a, st);
+    FSB_ATTN_CASE(128, 1) FSB_ATTN_CASE(128, 2) FSB_ATTN_CASE(128, 4) FSB_ATTN_CASE(128, 8)
+    FSB_ATTN_CASE(64, 1) FSB_ATTN_CASE(64, 2) FSB_ATTN_CASE(64, 4) FSB_ATTN_CASE(64, 8)
+#undef FSB_ATTN_CASE
+    set_error("attention: unsupported head_dim=%d group=%d", a.Dh, G);
+    return 1;
+}
+
+// shared memory of attn_span_kernel for a span of `span` positions
+template <int DH, int G>
+static size_t attn_span_smem_bytes(int span) {
+    return attn_smem_bytes<DH, G>(span, span / kKvPage);
+}
+
+template <int DH, int G>
+static int launch_attn_decode_split_t(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st) {
+    int lcap = a.S;
+    if (a.lcap > 0 && a.lcap < lcap) lcap = a.lcap;
+    const int pages = cdiv(a.S, kKvPage);
+    lcap = attn_score_chunk<DH, G>(lcap, pages);
+    const float scale = 1.0f / sqrtf(static_cast<float>(DH));
+    FSB_LAUNCH((attn_decode_split_kernel<DH, G>), dim3(a.Hkv, a.rows), dim3(kAttnThreads),
+               (attn_smem_bytes<DH, G>(lcap, pages)), st, a, sp, scale, lcap);
+    if (a.kv_only) return 0;
+    FSB_LAUNCH((attn_span_kernel<DH, G>), dim3(a.Hkv, a.rows, cdiv(sp.bound, sp.span)), dim3(kAttnThreads),
+               (attn_span_smem_bytes<DH, G>(sp.span)), st, a, sp, scale);
+    FSB_LAUNCH((attn_combine_kernel<DH, G>), dim3(a.Hkv, a.rows), dim3(kAttnThreads), 0, st, a, sp);
+    return 0;
+}
+
+int attn_split_max_span(int H, int Hkv, int Dh) {
+    if (Hkv <= 0 || H % Hkv != 0) return 0;
+    const int G = H / Hkv;
+#define FSB_ATTN_CASE(DH_, G_)                                                                                \
+    if (Dh == DH_ && G == G_)                                                                                 \
+        return static_cast<int>((200 * 1024 - attn_span_smem_bytes<DH_, G_>(0)) / (sizeof(float) * G_ + 1)) / \
+               kKvPage * kKvPage;
+    FSB_ATTN_CASE(128, 1) FSB_ATTN_CASE(128, 2) FSB_ATTN_CASE(128, 4) FSB_ATTN_CASE(128, 8)
+    FSB_ATTN_CASE(64, 1) FSB_ATTN_CASE(64, 2) FSB_ATTN_CASE(64, 4) FSB_ATTN_CASE(64, 8)
+#undef FSB_ATTN_CASE
+    return 0;
+}
+
+int launch_attn_decode_split(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st) {
+    if (a.rows <= 0) return 0;
+    const int G = a.H / a.Hkv;
+    FSB_CHECK(a.H % a.Hkv == 0, "attention: H %% Hkv != 0");
+    FSB_CHECK(a.bf16_math == 0, "attention: the split runs the fp32 attention only");
+    FSB_CHECK(sp.span > 0 && sp.span % kKvPage == 0 && sp.span <= attn_split_max_span(a.H, a.Hkv, a.Dh),
+              "attention: a span of %d positions is not a multiple of %d in [%d, %d]", sp.span, kKvPage, kKvPage,
+              attn_split_max_span(a.H, a.Hkv, a.Dh));
+    FSB_CHECK(sp.bound > 0 && cdiv(sp.bound, sp.span) <= 65535, "attention: %d spans", cdiv(sp.bound, sp.span));
+#define FSB_ATTN_CASE(DH_, G_) \
+    if (a.Dh == DH_ && G == G_) return launch_attn_decode_split_t<DH_, G_>(a, sp, st);
     FSB_ATTN_CASE(128, 1) FSB_ATTN_CASE(128, 2) FSB_ATTN_CASE(128, 4) FSB_ATTN_CASE(128, 8)
     FSB_ATTN_CASE(64, 1) FSB_ATTN_CASE(64, 2) FSB_ATTN_CASE(64, 4) FSB_ATTN_CASE(64, 8)
 #undef FSB_ATTN_CASE

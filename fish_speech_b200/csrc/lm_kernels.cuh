@@ -157,6 +157,30 @@ struct AttnDecodeArgs {
 };
 int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st);
 
+// The same attention with the history of a LONG row -- more than `span` positions -- split over several CTAs, so that
+// one long context does not set the time of the whole launch. Three kernels instead of one:
+//   1. attn_decode_split_kernel: attn_decode_kernel's front end and, for rows of at most `span` positions, its
+//      attention (the same code, the same bits); for a long row it stores the finished q heads to `q` and stops.
+//   2. attn_span_kernel, grid (Hkv, rows, spans): CTA (g, row, s) scores positions [s * span, min(L, (s + 1) * span))
+//      of a long row once and stores the span's own maximum, sum of exponentials and unnormalised weighted values
+//      (fp32) to `ws`.
+//   3. attn_combine_kernel, grid (Hkv, rows): merges a long row's spans in ascending order and rounds to bf16 once.
+// Span edges are absolute positions and the merge order is fixed: a long row's bits depend on its own history only,
+// not on the slot, the neighbours, `bound` or the number of SMs. They are not the bits of attn_decode_kernel for that
+// row (a different summation order), which is why the caller opts in. fp32 attention only (bf16_math == 0).
+struct AttnSplit {
+    __nv_bfloat16* q;  // [rows, H, Dh] finished q heads of the long rows
+    float* ws;         // [rows][Hkv][spans] records of attn_span_floats(G, Dh)
+    int span;          // positions per span, a multiple of kKvPage; rows longer than this are split
+    int bound;         // upper bound of (row_pos + 1) over the rows: spans = ceil(bound / span) are launched
+};
+// floats of one span record: acc[G][Dh], then max[G], then sum[G]
+constexpr int attn_span_floats(int G, int Dh) { return G * (Dh + 2); }
+// the longest span attn_span_kernel can hold in shared memory for this geometry (0: unsupported geometry)
+int attn_split_max_span(int H, int Hkv, int Dh);
+// a.lcap is the base kernel's score bound as for launch_attn_decode; the caller caps it at sp.span
+int launch_attn_decode_split(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st);
+
 // h = rbf( rbf(silu(rbf(a))) * rbf(c) ): a = w1 feature i, c = w3 feature i of the fused GEMM result.
 // interleaved = 0: a = y[i], c = y[I + i];  1: the step-GEMM row order (w13_gate_row in lm_gemm.cuh)
 struct SwigluArgs {

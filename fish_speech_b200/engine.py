@@ -255,9 +255,11 @@ class LmEngine:
 
     def __init__(self, config, state_dict: dict, device, im_end_id: int, max_batch: int = 1,
                  kv_len: Optional[int] = None, max_rows: int = 2048, max_frames: Optional[int] = None,
-                 debug: bool = False, kv_pages: Optional[int] = None):
+                 debug: bool = False, kv_pages: Optional[int] = None, attn_split: int = 0):
         """`kv_len`: KV positions one sequence can hold. `kv_pages`: size of the slow KV cache's page pool (pages of
-        64 positions); None = room for every slot at full capacity, so that no reservation can fail."""
+        64 positions); None = room for every slot at full capacity, so that no reservation can fail. `attn_split`:
+        0 = off; else a multiple of 64: a decode row with a longer context has its attention split into spans of that
+        many positions over several CTAs (include/fishb200.h fsb_lm_config.attn_split)."""
         if not torch.cuda.is_available():
             raise _lib.FsbError("fish_speech_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.lib = _lib.lib()
@@ -335,6 +337,7 @@ class LmEngine:
         K.max_batch, K.kv_len, K.max_rows, K.max_frames, K.debug = max_batch, kv_len, max_rows, max_frames, int(debug)
         pages_per_slot = kv_pages_for(kv_len)
         K.kv_pages = int(kv_pages) if kv_pages else max_batch * pages_per_slot
+        K.attn_split = self.attn_split = int(attn_split or 0)
         self._K, self._W = K, W
         h = C.c_void_p()
         with torch.cuda.device(self.device):
@@ -396,6 +399,9 @@ class LmEngine:
             "ssq_slow": ((rt, 32), "<f4"),
             "ssq_fast": ((rt, 32), "<f4"),
             "attn": ((rt * max(c.n_head * c.head_dim, c.fast_n_head * c.fast_head_dim),), "<u2"),
+            "q": ((rt * max(c.n_head * c.head_dim, c.fast_n_head * c.fast_head_dim),), "<u2"),
+            # split attention: one record per (slot, KV head, span of the launch); the span count follows the bound
+            "attn_span_ws": ((nbytes.value // 4,), "<f4"),
             "ffn_h": ((rt * max(c.intermediate_size, c.fast_intermediate_size),), "<u2"),
             # KV caches (include/fishb200.h fsb_lm_test_layer_attn): the slow page pool, the fast stack per slot
             "k_slow": ((c.n_layer, self._K.kv_pages, c.n_local_heads, KV_PAGE, c.head_dim), "<u2"),

@@ -661,6 +661,20 @@ def serve_kv_pool_pages(gb: float, config, free_bytes: int) -> int:
     return pages
 
 
+def serve_attn_split(value: Optional[str]) -> int:
+    """FSB_ATTN_SPLIT: positions per span of the split decode attention (setup_caches(attn_split=)); unset, empty or
+    0 = off. A ValueError naming FSB_ATTN_SPLIT for anything that is not a non-negative multiple of 64."""
+    if value is None or value.strip() == "":
+        return 0
+    try:
+        n = int(value)
+    except ValueError:
+        n = -1
+    if n < 0 or n % KV_PAGE != 0:
+        raise ValueError(f"FSB_ATTN_SPLIT={value!r} must be 0 (off) or a multiple of {KV_PAGE} positions")
+    return n
+
+
 def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool = False):
     """inference.py:736-799: the model lives in ONE daemon worker thread fed by a queue; `None` shuts
     it down; errors are returned as WrappedGenerateResponse(status="error", response=exc).
@@ -671,7 +685,10 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
     KV caches do not fit in free device memory, this raises a ValueError naming FSB_SERVE_KV_LEN.
     FSB_SERVE_KV_GB=g (with FSB_SERVE_SLOTS > 1) instead gives the slots one shared pool of g GB of KV pages, each
     slot a capacity of FSB_SERVE_KV_LEN (default: the model's max_seq_len) positions, and a request is admitted when
-    its pages fit; a pool that does not fit in free device memory raises a ValueError naming FSB_SERVE_KV_GB."""
+    its pages fit; a pool that does not fit in free device memory raises a ValueError naming FSB_SERVE_KV_GB.
+    FSB_ATTN_SPLIT=p (a multiple of 64; 0 or unset = off) makes a decode row whose context is longer than p positions
+    split its attention into spans of p positions over several CTAs, so that one long conversation does not slow the
+    frames of every slot; requests that stay at or below p keep their bits, longer ones change in the last places."""
     input_queue = queue.Queue()
     init_event = threading.Event()
     init_error: list = []
@@ -685,14 +702,16 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
             kv = min(int(os.environ.get("FSB_SERVE_KV_LEN", default_kv)), model.config.max_seq_len)
             try:
                 cuda = torch.device(device).type == "cuda"
+                split = serve_attn_split(os.environ.get("FSB_ATTN_SPLIT"))
                 if gb:
                     free = torch.cuda.mem_get_info(torch.device(device))[0] if cuda else float("inf")
                     pages = serve_kv_pool_pages(float(gb), model.config, free)
-                    model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype, kv_pages=pages)
+                    model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype, kv_pages=pages,
+                                       attn_split=split)
                 else:
                     if cuda:
                         check_serve_kv_fits(slots, kv, model.config, torch.cuda.mem_get_info(torch.device(device))[0])
-                    model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype)
+                    model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype, attn_split=split)
             except Exception as e:
                 init_error.append(e)
                 init_event.set()

@@ -63,6 +63,16 @@ typedef struct {
                                             ceil(kv_len / 64), room for every slot at full capacity. Sequences map
                                             pages through the "kv_page" table (fsb_lm_buffer), which the caller
                                             fills: a position whose page is not mapped is neither written nor read */
+    int attn_split;                      /* 0 = off. Otherwise positions per span of the decode attention, a multiple
+                                            of 64: a slow-stack row whose context is longer than this has its history
+                                            split into spans of this many positions (edges at absolute positions), one
+                                            CTA each, merged in ascending order by a kernel of its own, so that one
+                                            long request does not set the frame time of every slot. Such a row's bits
+                                            depend on its own history only (not on slot, neighbours or context bound)
+                                            but differ in the last places from the unsplit kernel's; rows up to this
+                                            length, and every frame whose context bound is at most this, keep today's
+                                            kernel and bits. At most what one span's scores fit in shared memory
+                                            (10 944 at head_dim 128 with 4 query heads per KV head) */
 } fsb_lm_config;
 
 /* One TransformerBlock (llama.py:831-987). bf16, row-major [out_features, in_features]. */
@@ -146,7 +156,8 @@ int fsb_lm_copy_kv(fsb_lm* h, int src_slot, int dst_slot, int n_pos, void* strea
 int fsb_lm_copy_kv_page(fsb_lm* h, int src_page, int dst_page, int n_pos, void* stream);
 
 /* Upper bound of (position + 1) over all slots for the calls that follow (prompt length + frames decoded so
- * far). Sizes the attention score buffer; must be set before prefill / decode whenever it grows. */
+ * far). Sizes the attention score buffer and, with attn_split, the number of spans launched (a row longer than the
+ * bound would lose its last spans); must be set before prefill / decode whenever it grows. */
 int fsb_lm_set_context_bound(fsb_lm* h, int max_positions);
 
 /* Per-slot request control — continuous batching over the KV slots, i.e. the batched form of the loop
@@ -187,7 +198,9 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
  *   debug only: "slow_logits" f32 [max_batch][head_rows], "fast_logits" f32 [C][max_batch][codebook_size];
  *   the decode state (for fsb_lm_test_layer_gemms), RT = the decode row tile (32 for max_batch <= 32, else 64):
  *   "x_slow" / "x_fast" bf16 [RT][dim] / [RT][fast_dim] residual streams, "ssq_slow" / "ssq_fast" f32 [RT][32] their
- *   per-128-feature sums of squares, "attn" bf16 [RT * max H*Dh] (the wo operand: rows of the stack being run at
+ *   per-128-feature sums of squares, "q" bf16 [RT * max H*Dh] (attn_split only: the finished q heads of the rows
+ *   that are split, rows at stride H*Dh) and "attn_span_ws" f32 [max_batch][n_kv_head][spans of the launch]
+ *   [G*(head_dim+2)] (attn_split only: per span acc[G][head_dim], max[G], sum[G]; G = n_head / n_kv_head), "attn" bf16 [RT * max H*Dh] (the wo operand: rows of the stack being run at
  *   stride H*Dh), "ffn_h" bf16 [RT * max I] (the w2 operand: rows at stride I of the stack being run);
  *   the KV caches (for fsb_lm_test_layer_attn and the copy tests): "k_slow" / "v_slow" bf16
  *   [n_layer][kv_pages][n_kv_head][64][head_dim] (the page pool), "k_fast" / "v_fast" bf16
@@ -336,7 +349,8 @@ int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, 
 /* Runs the qkv step GEMM of decode layer `layer` and the decode attention after it (csrc/lm_kernels.cu
  * attn_decode_kernel: the GEMM's fix-up -- bias, qk-norm, RoPE --, the K/V append and the attention) for `rows` batch
  * rows, with the arguments fsb_lm_decode gives them: the handle's own plan and partial workspace, the "kv_page" table,
- * the context bound (fsb_lm_set_context_bound) and the score chunk (fsb_op_attn_score_chunk). The GEMM's operand is
+ * the context bound (fsb_lm_set_context_bound) and the score chunk (fsb_op_attn_score_chunk); with attn_split set and
+ * a bound above it, the slow stack's launch is the split sequence (front end, spans, combine). The GEMM's operand is
  * "x_slow" / "x_fast" exactly as the caller wrote them, normalised on load with "ssq_slow" / "ssq_fast". Row i is
  * slot i at position "pos"[i] in both stacks (decode gives the fast stack its codebook positions instead); -1 parks a
  * row. kv_only != 0 stops after the append, as the fast stack's pass 0 does. Outputs: "attn" (rows at stride H*Dh)

@@ -339,6 +339,50 @@ int run_stack_prefill(fsb_lm* h, Stack& s, int rows, const int* row_seq, const i
     return 0;
 }
 
+// Arguments of the sampler behind the slow head (p = 0) or behind fast pass p's head (codebook p, p >= 1) over `rows`
+// batch rows whose logits are `parts`: one place for run_frame_tail and fsb_lm_test_sample, so that the test hook
+// launches exactly what a frame launches.
+SampleArgs frame_sample_args(const fsb_lm* h, int p, const StepPartials& parts, int rows, const int* row_slot,
+                             bool use_ras, const fsb_sampling& sp) {
+    const fsb_lm_config& c = h->cfg;
+    SampleArgs a{};
+    a.ctl = slot_ctl(h);
+    a.parts = parts;
+    a.rows = rows;
+    a.temperature = sp.temperature; a.top_p = sp.top_p; a.top_k = sp.top_k;
+    a.seed = sp.seed;
+    a.rng_offset = h->step;
+    a.cur_tok = h->cur_tok;
+    a.num_cb = c.num_codebooks;
+    a.row_slot = row_slot;
+    a.noise_u = h->noise_u;
+    a.noise_draws = h->noise_draws;
+    a.noise_ld = h->noise_ld;
+    if (p == 0) {
+        a.n = h->head_rows;
+        a.slow = 1;
+        a.n_sem = h->head_rows - 1;
+        a.sem_begin = c.semantic_begin_id;
+        a.im_end_id = c.im_end_id;
+        a.codebook_size = c.codebook_size;
+        a.use_ras = use_ras ? 1 : 0;
+        a.ras_window = h->ras_window;
+        a.ras_update = use_ras ? 1 : 0;
+        a.draw_id = 0;
+        a.cb_index = 0;
+        a.logits_out = h->slow_logits;
+        a.finished = h->finished;
+    } else {
+        a.n = c.codebook_size;
+        a.slow = 0;
+        a.draw_id = p;
+        a.cb_index = p;
+        a.logits_out = h->fast_logits ? h->fast_logits + static_cast<size_t>(p - 1) * c.max_batch * c.codebook_size
+                                      : nullptr;
+    }
+    return a;
+}
+
 // Head + sampling + fast passes + bookkeeping for `rows` sequences whose last residual-stream rows (un-normed)
 // are in slow.xres[0..rows) with their sums of squares in slow.ssq. inference.py:114-181.
 int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const int* set_pos_rows,
@@ -348,39 +392,9 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
     const int* slots = row_slot ? row_slot : h->iota;
     Stack& s = h->slow;
     Stack& f = h->fast;
-    auto sample_args = [&](int n, const StepGemmPlan& head) {
-        SampleArgs a{};
-        a.ctl = slot_ctl(h);
-        a.parts = step_plan_partials(head);
-        a.n = n;
-        a.rows = rows;
-        a.temperature = sp.temperature; a.top_p = sp.top_p; a.top_k = sp.top_k;
-        a.seed = sp.seed;
-        a.rng_offset = h->step;
-        a.cur_tok = h->cur_tok;
-        a.num_cb = C;
-        a.row_slot = row_slot;
-        a.noise_u = h->noise_u;
-        a.noise_draws = h->noise_draws;
-        a.noise_ld = h->noise_ld;
-        return a;
-    };
     // ---- slow head over the selectable rows (the final norm is applied on load) ----
     FSB_TRY(step_gemm_launch(h->head_plan, rows, st));
-    SampleArgs sa = sample_args(h->head_rows, h->head_plan);
-    sa.slow = 1;
-    sa.n_sem = h->head_rows - 1;
-    sa.sem_begin = c.semantic_begin_id;
-    sa.im_end_id = c.im_end_id;
-    sa.codebook_size = c.codebook_size;
-    sa.use_ras = use_ras ? 1 : 0;
-    sa.ras_window = h->ras_window;
-    sa.ras_update = use_ras ? 1 : 0;
-    sa.draw_id = 0;
-    sa.cb_index = 0;
-    sa.logits_out = h->slow_logits;
-    sa.finished = h->finished;
-    FSB_TRY(launch_sample(sa, st));
+    FSB_TRY(launch_sample(frame_sample_args(h, 0, step_plan_partials(h->head_plan), rows, row_slot, use_ras, sp), st));
 
     // ---- fast pass 0 input: hidden = norm(x) (norm_fastlayer_input) [-> fast_project_in]  (llama.py:459-461, 819-828)
     RowsArgs hr{};
@@ -414,13 +428,8 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
         FSB_TRY(run_stack_decode(h, f, rows, slots, h->fpos + p * h->rt, p == 0, st));
         if (p == 0) continue;
         FSB_TRY(step_gemm_launch(h->fast_out_plan, rows, st));
-        SampleArgs fa = sample_args(c.codebook_size, h->fast_out_plan);
-        fa.slow = 0;
-        fa.draw_id = p;
-        fa.cb_index = p;
-        fa.logits_out = h->fast_logits ? h->fast_logits + static_cast<size_t>(p - 1) * c.max_batch * c.codebook_size
-                                       : nullptr;
-        FSB_TRY(launch_sample(fa, st));
+        FSB_TRY(launch_sample(frame_sample_args(h, p, step_plan_partials(h->fast_out_plan), rows, row_slot, false, sp),
+                              st));
     }
     FrameEndArgs fe{};
     fe.ctl = slot_ctl(h);
@@ -474,6 +483,11 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     FSB_CHECK((cfg->head_dim == 64 || cfg->head_dim == 128) && (cfg->fast_head_dim == 64 || cfg->fast_head_dim == 128),
               "head_dim must be 64 or 128");
     FSB_CHECK(w->head_rows == cfg->semantic_end_id - cfg->semantic_begin_id + 2, "head_rows mismatch");
+    // the sampler holds one row's candidates in shared memory: refuse here, not in the middle of the first frame
+    FSB_CHECK(w->head_rows >= 1 && w->head_rows <= kSampleMaxN && cfg->codebook_size >= 1 &&
+                  cfg->codebook_size <= kSampleMaxN,
+              "head_rows=%d and codebook_size=%d must be in [1, %d] (candidates the sampler holds)", w->head_rows,
+              cfg->codebook_size, kSampleMaxN);
     FSB_CHECK(cfg->kv_len >= 1 && cfg->kv_pages >= 0, "kv_len must be >= 1 and kv_pages >= 0");
     if (cfg->attn_split != 0) {
         const int most = attn_split_max_span(cfg->n_head, cfg->n_kv_head, cfg->head_dim);
@@ -605,7 +619,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &h->slot_seed, cfg->max_batch, "slot_seed"));
     TRYC(dalloc(h, &h->iota, RT));
     TRYC(dalloc(h, &h->fpos, static_cast<size_t>(C) * RT));
-    TRYC(dalloc(h, &h->step, 1));
+    TRYC(dalloc(h, &h->step, 1, "step"));
     if (cfg->debug) {
         TRYC(dalloc(h, &h->slow_logits, static_cast<size_t>(cfg->max_batch) * h->head_rows, "slow_logits"));
         TRYC(dalloc(h, &h->fast_logits, static_cast<size_t>(C) * cfg->max_batch * cfg->codebook_size, "fast_logits"));
@@ -915,6 +929,55 @@ int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only
     const StepGemmPlan& qkv = s.dec[layer].qkv;
     FSB_TRY(step_gemm_launch(qkv, rows, st));
     return launch_decode_attn(h, s, layer, qkv, rows, h->iota, h->pos, kv_only != 0, st);
+}
+
+int fsb_lm_test_sample(fsb_lm* h, int fast, int cb_index, int rows, const int32_t* d_row_slot, const float* d_logits,
+                       int use_ras, const fsb_sampling* sp, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(h != nullptr, "test_sample: null handle");
+    const fsb_lm_config& c = h->cfg;
+    FSB_CHECK(rows >= 1 && rows <= c.max_batch, "test_sample: rows=%d outside [1, %d]", rows, c.max_batch);
+    FSB_CHECK(fast ? (cb_index >= 1 && cb_index < c.num_codebooks) : cb_index == 0,
+              "test_sample: cb_index=%d must be %s", cb_index, fast ? "a sampled codebook in [1, num_codebooks)" : "0");
+    FSB_CHECK(!fast || !use_ras, "test_sample: the fast head has no RAS draw");
+    FSB_CHECK(d_logits != nullptr, "test_sample: null logits");
+    FSB_CHECK(sp != nullptr || h->slot_control, "test_sample: sampling parameters required");
+    const fsb_sampling sp_none{1.f, 1.f, 1, 0};
+    const int n = fast ? c.codebook_size : h->head_rows;
+    // the logits as the single partial of a step GEMM with a row tile of `rows`: ws[tile][row][128]
+    const int tiles = cdiv(n, 128);
+    const size_t ws_bytes = static_cast<size_t>(tiles) * rows * 128 * sizeof(float);
+    float* ws = nullptr;
+    int* nparts = nullptr;
+    FSB_CUDA(cudaMalloc(&ws, ws_bytes));
+    int rc = 1;
+    if (cudaMalloc(&nparts, tiles * sizeof(int)) != cudaSuccess) {
+        set_error("test_sample: out of device memory");
+    } else {
+        const std::vector<int> ones(tiles, 1);
+        bool ok = cudaMemsetAsync(ws, 0, ws_bytes, st) == cudaSuccess &&
+                  cudaMemcpyAsync(nparts, ones.data(), tiles * sizeof(int), cudaMemcpyHostToDevice, st) == cudaSuccess;
+        for (int t = 0; ok && t < tiles; ++t)
+            ok = cudaMemcpy2DAsync(ws + static_cast<size_t>(t) * rows * 128, 128 * sizeof(float), d_logits + t * 128,
+                                   static_cast<size_t>(n) * sizeof(float), std::min(128, n - t * 128) * sizeof(float),
+                                   rows, cudaMemcpyDeviceToDevice, st) == cudaSuccess;
+        if (!ok) {
+            set_error("test_sample: staging the logits failed: %s", cudaGetErrorString(cudaGetLastError()));
+        } else {
+            const StepPartials P{ws, nparts, tiles, n, 1, rows};
+            rc = launch_sample(frame_sample_args(h, fast ? cb_index : 0, P, rows, d_row_slot, use_ras != 0,
+                                                 sp ? *sp : sp_none),
+                               st);
+            const cudaError_t e = cudaStreamSynchronize(st);
+            if (rc == 0 && e != cudaSuccess) {
+                set_error("test_sample: %s", cudaGetErrorString(e));
+                rc = 1;
+            }
+        }
+    }
+    cudaFree(nparts);
+    cudaFree(ws);
+    return rc;
 }
 
 int fsb_lm_copy_kv(fsb_lm* h, int src_slot, int dst_slot, int n_pos, void* stream) {

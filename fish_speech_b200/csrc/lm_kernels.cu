@@ -962,7 +962,6 @@ __global__ void swiglu4_kernel(SwigluArgs a) {
 // slow-token RAS rule inference.py:114-144.
 // ------------------------------------------------------------------------------------------------
 constexpr int kSampleThreads = 1024;
-constexpr int kSampleMaxN = 8192;
 constexpr int kSelCap = 256;  // ranks materialised for top-k / top-p
 
 __device__ __forceinline__ void philox4x32(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1,
@@ -1056,8 +1055,10 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     }
     __syncthreads();
 
-    const bool two = a.slow && a.use_ras && top_k != 1;
-    if (top_k == 1) {
+    // top_k <= 1 keeps rank 0 only, as the reference's mask does (ranks >= top_k removed, then rank 0 restored): the
+    // greedy argmax, and no RAS re-draw, whose top-k cut is the same
+    const bool two = a.slow && a.use_ras && top_k > 1;
+    if (top_k <= 1) {
         ArgMax x{-INFINITY, 0x7fffffff};
         for (int e = threadIdx.x; e < n; e += kSampleThreads) x = better(x, ArgMax{lg[e], e});
         x = block_argmax(x, red);
@@ -1485,7 +1486,6 @@ int launch_swiglu(const SwigluArgs& a, cudaStream_t st) {
 int launch_sample(const SampleArgs& a, cudaStream_t st) {
     if (a.rows <= 0) return 0;
     FSB_CHECK(a.n > 0 && a.n <= kSampleMaxN, "sample: n=%d out of range", a.n);
-    FSB_CHECK(a.ctl.state != nullptr || a.top_k >= 1, "sample: top_k must be >= 1");
     FSB_LAUNCH(sample_kernel, dim3(a.rows), dim3(kSampleThreads), 0, st, a);
     return 0;
 }

@@ -212,13 +212,15 @@ __device__ __forceinline__ bool slot_live(const SlotCtl& c, int slot) {
     return s == 1 || s == 3;
 }
 
+constexpr int kSampleMaxN = 8192;  // most candidates the sampler holds (one fp32 logit each in shared memory)
+
 struct SampleArgs {
     StepPartials parts;  // stream-K partials of the (restricted) head GEMM: logit = rbf(slot-ordered sum)
-    int n;           // number of candidate entries (<= 8192)
+    int n;           // number of candidate entries (<= kSampleMaxN)
     int rows;
     // sampling parameters
     float temperature, top_p;
-    int top_k;
+    int top_k;  // <= 1: rank 0 only (greedy argmax, no RAS re-draw); above 256 the same as 256
     // token mapping for the slow head: entry e -> token id (e < n_sem ? sem_begin + e : im_end_id)
     int slow;  // 1: slow head (RAS + token mapping), 0: fast head (codes)
     int n_sem, sem_begin, im_end_id, codebook_size;

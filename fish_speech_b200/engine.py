@@ -380,6 +380,7 @@ class LmEngine:
             "out_tokens": ((self.max_batch, C1, self.max_frames), "<i4"),
             "n_out": ((self.max_batch,), "<i4"),
             "pos": ((self.row_tile,), "<i4"),
+            "step": ((1,), "<i8"),
             "finished": ((self.max_batch,), "<i4"),
             "cur_tok": ((self.max_batch, C1), "<i4"),
             "ras_window": ((self.max_batch, 10), "<i4"),
@@ -454,6 +455,16 @@ class LmEngine:
         u = u.to(device=self.device, dtype=torch.float32).contiguous()
         self._noise = u
         _lib.check(self.lib.fsb_lm_set_sampler_noise(self.h, u.data_ptr(), u.shape[1], u.shape[2]))
+
+    def test_sample(self, logits: torch.Tensor, sp: Optional[_lib.Sampling], codebook: int = 0,
+                    row_slot: Optional[torch.Tensor] = None, use_ras: bool = False):
+        """Test hook (include/fishb200.h fsb_lm_test_sample): the sampler alone on fp32 logits [rows][n], behind the
+        slow head (codebook 0) or fast codebook `codebook`; row_slot int32 [rows] on the device or None."""
+        logits = logits.to(device=self.device, dtype=torch.float32).contiguous()
+        rs = None if row_slot is None else row_slot.to(device=self.device, dtype=torch.int32).contiguous()
+        _lib.check(self.lib.fsb_lm_test_sample(self.h, int(codebook > 0), int(codebook), logits.shape[0],
+                                               None if rs is None else rs.data_ptr(), logits.data_ptr(),
+                                               int(bool(use_ras)), None if sp is None else C.byref(sp), _stream()))
 
     # ---- paged slow KV cache (KvPagePool) --------------------------------------------------------------------------
     def _forget_slot(self, slot: int):

@@ -112,7 +112,9 @@ typedef struct {
 } fsb_lm_weights;
 
 /* sample() parameters (inference.py:54-93).  temperature / top_p must already be rounded to the
- * model dtype the way the reference builds them (torch.tensor(v, dtype=bf16), inference.py:303-304). */
+ * model dtype the way the reference builds them (torch.tensor(v, dtype=bf16), inference.py:303-304).
+ * top_k <= 1 keeps the most likely candidate only (greedy, no RAS re-draw), as the reference's mask does for any
+ * top_k <= 1; a top_k above 256 samples exactly as 256 (see INTEGRATION.md). */
 typedef struct {
     float temperature;
     float top_p;
@@ -166,7 +168,8 @@ int fsb_lm_set_context_bound(fsb_lm* h, int max_positions);
  * `s` (may be NULL) and read, per slot, the device arrays
  *   "slot_state" int32 (0 idle, 1 active, 2 finished, 3 finishing), "slot_limit" int32 (frames allowed,
  *   the prefill's frame included), "slot_temperature" f32, "slot_top_p" f32 (both already rounded to
- *   bf16 by the host, as the reference's tensors are), "slot_top_k" int32, "slot_seed" uint64.
+ *   bf16 by the host, as the reference's tensors are), "slot_top_k" int32 (any value: <= 1 is greedy, as in
+ *   fsb_sampling), "slot_seed" uint64.
  * The host writes them (fsb_lm_buffer) before prefilling a request into a slot; the frame kernels stop
  * a slot on <|im_end|> (from its second frame on) or at its limit, freeze its position and counters,
  * and set state = 2; the host collects "out_tokens"[slot][:, :n_out[slot]] and sets the state to 0.
@@ -191,6 +194,7 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
 
 /* Named device buffers of the handle, for reading results and for tests:
  *   "out_tokens" int32 [max_batch][C+1][max_frames], "n_out" int32 [max_batch], "pos" int32 [RT],
+ *   "step" uint64 [1] (frames decoded since fsb_lm_reset: the Philox counter of the per-call sampling parameters),
  *   "finished" int32 [max_batch], "cur_tok" int32 [max_batch][C+1], "ras_window" int32 [max_batch][10],
  *   the slot-control arrays listed at fsb_lm_set_slot_control, "kv_page" int32 [max_batch][ceil(kv_len / 64)]
  *   (page of each 64-position block of each slot, -1 = not mapped; read by the kernels at run time, so a captured
@@ -356,6 +360,18 @@ int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, 
  * row. kv_only != 0 stops after the append, as the fast stack's pass 0 does. Outputs: "attn" (rows at stride H*Dh)
  * and the caches "k_*" / "v_*". rows in [1, max_batch]. */
 int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only, void* stream);
+
+/* Runs the sampler (csrc/lm_kernels.cu sample_kernel) on its own for `rows` batch rows, with the arguments a decode
+ * frame gives it: the slow head's (fast = 0, cb_index = 0; use_ras != 0 as in a decode frame, 0 as in the prefill's) or
+ * fast codebook cb_index's (fast = 1, cb_index in [1, num_codebooks), use_ras = 0). d_logits is fp32 [rows][n], n =
+ * head_rows (slow) or codebook_size (fast), staged as the single partial of a step GEMM so that the sampler's logit
+ * is exactly rbf(d_logits). Row i is slot d_row_slot[i] (NULL: slot i); the slots must lie in [0, max_batch) and be
+ * distinct, as in a frame (they are not checked: a slot outside writes outside the state arrays). Everything else is the handle's own state,
+ * read and written as a frame does: slot control, "cur_tok", "ras_window", "finished", "slow_logits" / "fast_logits",
+ * the noise of fsb_lm_set_sampler_noise and the frame counter "step" (frame counters are not advanced). `s` is
+ * ignored with slot control (may be NULL then). rows in [1, max_batch]. Synchronises `stream`. */
+int fsb_lm_test_sample(fsb_lm* h, int fast, int cb_index, int rows, const int32_t* d_row_slot, const float* d_logits,
+                       int use_ras, const fsb_sampling* s, void* stream);
 
 /* Attention keeps one fp32 score per position and head in shared memory; contexts longer than the buffer are walked
  * in chunks, bit-identically (csrc/lm_kernels.cu attend()).  positions > 0 forces a smaller chunk; 0 = automatic. */

@@ -96,8 +96,10 @@ def lib() -> C.CDLL:
     L.fsb_dwconv_ln.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, C.c_float, vp, vp]
     L.fsb_final_conv_tanh.argtypes = [vp, vp, C.c_float, i32, i32, i32, i32, vp, vp]
     L.fsb_first_conv.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp]
+    L.fsb_first_conv_window.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]
     L.fsb_snake.argtypes = [vp, vp, vp, ll, i32, vp, vp]
     L.fsb_vq_encode.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp]
+    L.fsb_vq_encode_valid.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
     L.fsb_resid_scale_norm.argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, i32, C.c_float, i32, vp]
     L.fsb_qkv_rope.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp]
     L.fsb_res_unit_supported.argtypes = [i32]
@@ -109,6 +111,7 @@ def lib() -> C.CDLL:
     L.fsb_qkv_rope_ring.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]
     L.fsb_window_attn_ring.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp]
     L.fsb_window_fill.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    L.fsb_window_fill_zero.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     L.fsb_window_roll.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, vp]
     L.fsb_dwconv_ln_window.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, C.c_float, vp, vp]
     L.fsb_op_gemm.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]

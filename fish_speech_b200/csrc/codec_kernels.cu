@@ -6,7 +6,7 @@
 //   codebook_sum   rvq.py:361-363 + dac/nn/quantize.py from_codes (tables = out_proj(codebook), folded at load)
 //   dwconv_ln      rvq.py:176-179 (ConvNeXt: causal depthwise conv k=7, LayerNorm eps 1e-6)
 //   final_conv     modded_dac.py:793-797 (Snake'd input -> conv7 C->1 -> tanh)
-//   first_conv     modded_dac.py:683 (conv7 1->C on the raw waveform)
+//   first_conv     modded_dac.py:683 (conv7 1->C on the raw waveform; a stream-window variant for EncodeStreamPool)
 //   vq_encode      rvq.py:304-317 + dac/nn/quantize.py VectorQuantize.forward (10 residual VQ stages)
 #include <algorithm>
 #include <map>
@@ -102,6 +102,9 @@ dwconv_ln_window_kernel(const bf16* __restrict__ x, const float* __restrict__ w,
 // Stream windows of DecodeStreamPool: window [nb][H + n][row] per layer input, rows 0 .. H-1 the carried history.
 // fill: history rows from state [slots][H][row] (row i's slot), rows H .. H + valid[i] - 1 from the producer's dense
 // output [nb][n][row]; roll: the last H valid rows back to the slot's state. Flat over 16-byte units.
+// ZERO (EncodeStreamPool): rows past a stream's valid rows, and every row of a stream with a negative slot, are zeroed,
+// so that padding rows stay finite whatever the buffer held before (see fsb_window_fill_zero).
+template <bool ZERO>
 __global__ void window_fill_kernel(const uint4* __restrict__ state, const uint4* __restrict__ dense,
                                    uint4* __restrict__ win, const int* __restrict__ slot, const int* __restrict__ valid,
                                    int nb, int H, int n, int u16) {
@@ -114,9 +117,13 @@ __global__ void window_fill_kernel(const uint4* __restrict__ state, const uint4*
         const long long r = e / u16;
         const int i = static_cast<int>(r / (H + n)), w = static_cast<int>(r - static_cast<long long>(i) * (H + n));
         const int s = slot[i];
-        if (s < 0) continue;
+        if (s < 0) {
+            if (ZERO) win[e] = make_uint4(0, 0, 0, 0);
+            continue;
+        }
         if (w < H) win[e] = state[(static_cast<size_t>(s) * H + w) * u16 + u];
         else if (w - H < valid[i]) win[e] = dense[(static_cast<size_t>(i) * n + (w - H)) * u16 + u];
+        else if (ZERO) win[e] = make_uint4(0, 0, 0, 0);
     }
 }
 __global__ void window_roll_kernel(const uint4* __restrict__ win, uint4* __restrict__ state,
@@ -200,28 +207,43 @@ final_conv_tanh_kernel(const bf16* __restrict__ a, const float* __restrict__ w /
 }
 
 // ------------------------------------------------------------------------------------------------
-// y[b][t][co] = bias[co] + sum_j w[co][j] * wav[b][t-(K-1)+j]   (+ optional Snake for the consumer)
-__global__ void first_conv_kernel(const float* __restrict__ wav, const float* __restrict__ w /*[C][K]*/,
-                                  const float* __restrict__ bias, const float* __restrict__ alpha,
-                                  const float* __restrict__ inv_alpha, int T, int C, int K, bf16* __restrict__ raw,
-                                  bf16* __restrict__ act) {
+// y[b][t][co] = bias[co] + sum_j w[co][j] * wav[b][origin + t-(K-1)+j]   (+ optional Snake for the consumer)
+// wav [B][T_in] fp32, y [B][T_out][C]; samples before index 0 are the causal zero pad.
+__device__ __forceinline__ void first_conv_elem(const float* __restrict__ wav, const float* __restrict__ w,
+                                                const float* __restrict__ bias, const float* __restrict__ alpha,
+                                                const float* __restrict__ inv_alpha, int T_in, int origin, int T_out,
+                                                int C, int K, bf16* __restrict__ raw, bf16* __restrict__ act) {
     pdl_launch_dependents();
     pdl_wait();
     const int b = blockIdx.y;
     const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (e >= static_cast<long long>(T) * C) return;
+    if (e >= static_cast<long long>(T_out) * C) return;
     const int t = static_cast<int>(e / C), c = static_cast<int>(e - static_cast<long long>(t) * C);
     float acc = bias[c];
     for (int j = 0; j < K; ++j) {
-        const int tt = t - (K - 1) + j;
-        if (tt >= 0) acc += w[c * K + j] * wav[static_cast<size_t>(b) * T + tt];
+        const int tt = origin + t - (K - 1) + j;
+        if (tt >= 0) acc += w[c * K + j] * wav[static_cast<size_t>(b) * T_in + tt];
     }
-    const size_t o = (static_cast<size_t>(b) * T + t) * C + c;
+    const size_t o = (static_cast<size_t>(b) * T_out + t) * C + c;
     if (raw) raw[o] = f2bf(acc);
     if (act) {
         const float s = sinf(alpha[c] * acc);
         act[o] = f2bf(acc + inv_alpha[c] * s * s);
     }
+}
+__global__ void first_conv_kernel(const float* __restrict__ wav, const float* __restrict__ w /*[C][K]*/,
+                                  const float* __restrict__ bias, const float* __restrict__ alpha,
+                                  const float* __restrict__ inv_alpha, int T, int C, int K, bf16* __restrict__ raw,
+                                  bf16* __restrict__ act) {
+    first_conv_elem(wav, w, bias, alpha, inv_alpha, T, 0, T, C, K, raw, act);
+}
+// The same over a stream window (EncodeStreamPool): samples 0 .. origin-1 of each batch item are the carried history
+// and only the T_out samples after them are computed.
+__global__ void first_conv_window_kernel(const float* __restrict__ wav, const float* __restrict__ w,
+                                         const float* __restrict__ bias, const float* __restrict__ alpha,
+                                         const float* __restrict__ inv_alpha, int T_in, int origin, int T_out, int C,
+                                         int K, bf16* __restrict__ raw, bf16* __restrict__ act) {
+    first_conv_elem(wav, w, bias, alpha, inv_alpha, T_in, origin, T_out, C, K, raw, act);
 }
 
 // elementwise Snake (used where no producing GEMM exists to fuse it into)
@@ -241,12 +263,16 @@ __global__ void snake_kernel(const bf16* __restrict__ x, const float* __restrict
 // Residual vector quantisation of one latent frame per CTA (10 stages in sequence):
 //   e = in_proj_s(res) (8 dims); code = argmax_k cos(e, codebook_s[k]); res -= out_proj_s(codebook_s[code])
 // in_w [S][cd][D], in_b [S][cd], cbn [sum sizes][cd] (L2-normalised codebooks), tabs[s] = out_proj(codebook) [size][D]
+// VALID (EncodeStreamPool): only frames t < valid[b] of each batch item are quantised, the codes of the others are not
+// written (its padding frames hold whatever the window buffers held, possibly not finite).
 constexpr int kVqThreads = 256;
 constexpr int kVqMaxCd = 16;
+template <bool VALID>
 __global__ void __launch_bounds__(kVqThreads)
 vq_encode_kernel(const bf16* __restrict__ z, const float* __restrict__ in_w, const float* __restrict__ in_b,
                  const float* __restrict__ cbn, const int* __restrict__ cb_off, const int* __restrict__ sizes,
-                 const float* const* __restrict__ tabs, int S, int cd, int T, int D, int* __restrict__ codes) {
+                 const float* const* __restrict__ tabs, int S, int cd, int T, int D, int* __restrict__ codes,
+                 const int* __restrict__ valid) {
     extern __shared__ float vsm[];
     float* res = vsm;  // [D]
     __shared__ float e_s[kVqMaxCd];
@@ -256,6 +282,7 @@ vq_encode_kernel(const bf16* __restrict__ z, const float* __restrict__ in_w, con
     pdl_launch_dependents();
     pdl_wait();
     const int t = blockIdx.x, b = blockIdx.y;
+    if (VALID && t >= valid[b]) return;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int d = threadIdx.x; d < D; d += kVqThreads) res[d] = bf2f(z[(static_cast<size_t>(b) * T + t) * D + d]);
     __syncthreads();
@@ -335,6 +362,20 @@ std::map<ConvKey, GemmPlan> g_conv_plans;
 // workspaces are re-allocated) would otherwise grow this map without bound. Tiled plans own no device memory.
 constexpr size_t kMaxConvPlans = 8192;
 std::mutex g_conv_mutex;
+
+template <bool ZERO>
+int window_fill(const void* d_state, const void* d_dense, void* d_win, const int32_t* d_slot,
+                       const int32_t* d_valid, int nb, int H, int n, int row_bytes, void* stream) {
+    FSB_CHECK(row_bytes > 0 && row_bytes % 16 == 0 && H >= 0 && n >= 0, "window_fill: row_bytes=%d H=%d n=%d", row_bytes,
+              H, n);
+    const long long total = static_cast<long long>(nb) * (H + n) * (row_bytes / 16);
+    if (total <= 0) return 0;
+    FSB_LAUNCH(window_fill_kernel<ZERO>, dim3(static_cast<unsigned>(std::min<long long>(cdivll(total, 256), 8192))), dim3(256),
+               0, reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const uint4*>(d_state),
+               reinterpret_cast<const uint4*>(d_dense), reinterpret_cast<uint4*>(d_win), d_slot, d_valid, nb, H, n,
+               row_bytes / 16);
+    return 0;
+}
 
 }  // namespace
 
@@ -490,15 +531,12 @@ int fsb_dwconv_ln_window(const void* d_x, const float* d_w, const float* d_bias,
 
 int fsb_window_fill(const void* d_state, const void* d_dense, void* d_win, const int32_t* d_slot,
                     const int32_t* d_valid, int nb, int H, int n, int row_bytes, void* stream) {
-    FSB_CHECK(row_bytes > 0 && row_bytes % 16 == 0 && H >= 0 && n >= 0, "window_fill: row_bytes=%d H=%d n=%d", row_bytes,
-              H, n);
-    const long long total = static_cast<long long>(nb) * (H + n) * (row_bytes / 16);
-    if (total <= 0) return 0;
-    FSB_LAUNCH(window_fill_kernel, dim3(static_cast<unsigned>(std::min<long long>(cdivll(total, 256), 8192))), dim3(256),
-               0, reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const uint4*>(d_state),
-               reinterpret_cast<const uint4*>(d_dense), reinterpret_cast<uint4*>(d_win), d_slot, d_valid, nb, H, n,
-               row_bytes / 16);
-    return 0;
+    return window_fill<false>(d_state, d_dense, d_win, d_slot, d_valid, nb, H, n, row_bytes, stream);
+}
+
+int fsb_window_fill_zero(const void* d_state, const void* d_dense, void* d_win, const int32_t* d_slot,
+                         const int32_t* d_valid, int nb, int H, int n, int row_bytes, void* stream) {
+    return window_fill<true>(d_state, d_dense, d_win, d_slot, d_valid, nb, H, n, row_bytes, stream);
 }
 
 int fsb_window_roll(const void* d_win, void* d_state, const int32_t* d_slot, const int32_t* d_valid, int nb, int H,
@@ -536,6 +574,21 @@ int fsb_first_conv(const float* d_wav, const float* d_w, const float* d_bias, co
     return 0;
 }
 
+int fsb_first_conv_window(const float* d_wav, const float* d_w, const float* d_bias, const float* d_alpha,
+                          const float* d_inv_alpha, int B, int T_in, int origin, int T_out, int C, int K, void* d_raw,
+                          void* d_act, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(origin >= 0 && origin + T_out <= T_in, "first_conv_window: samples %d + %d outside %d", origin, T_out,
+              T_in);
+    FSB_CHECK(d_raw || d_act, "first_conv_window: no output");
+    const long long n = static_cast<long long>(T_out) * C;
+    if (n <= 0 || B <= 0) return 0;
+    FSB_LAUNCH(first_conv_window_kernel, dim3(static_cast<unsigned>(cdivll(n, 256)), B), dim3(256), 0, st, d_wav, d_w,
+               d_bias, d_alpha, d_inv_alpha, T_in, origin, T_out, C, K, reinterpret_cast<bf16*>(d_raw),
+               reinterpret_cast<bf16*>(d_act));
+    return 0;
+}
+
 int fsb_snake(const void* d_x, const float* d_alpha, const float* d_inv_alpha, long long n, int C, void* d_y,
               void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -549,9 +602,22 @@ int fsb_vq_encode(const void* d_z, const float* d_in_w, const float* d_in_b, con
                   int T, int D, int32_t* d_codes, void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     FSB_CHECK(cd <= kVqMaxCd, "vq_encode: codebook_dim %d too large", cd);
-    FSB_LAUNCH(vq_encode_kernel, dim3(T, B), dim3(kVqThreads), static_cast<size_t>(D) * sizeof(float), st,
+    FSB_LAUNCH(vq_encode_kernel<false>, dim3(T, B), dim3(kVqThreads), static_cast<size_t>(D) * sizeof(float), st,
                reinterpret_cast<const bf16*>(d_z), d_in_w, d_in_b, d_cbn, d_cb_off, d_sizes, d_tabs, S, cd, T, D,
-               d_codes);
+               d_codes, nullptr);
+    return 0;
+}
+
+int fsb_vq_encode_valid(const void* d_z, const float* d_in_w, const float* d_in_b, const float* d_cbn,
+                        const int32_t* d_cb_off, const int32_t* d_sizes, const float* const* d_tabs, int S, int cd,
+                        int B, int T, int D, const int32_t* d_valid, int32_t* d_codes, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(cd <= kVqMaxCd, "vq_encode: codebook_dim %d too large", cd);
+    FSB_CHECK(d_valid != nullptr, "vq_encode_valid: no valid frame counts");
+    if (T <= 0 || B <= 0) return 0;
+    FSB_LAUNCH(vq_encode_kernel<true>, dim3(T, B), dim3(kVqThreads), static_cast<size_t>(D) * sizeof(float), st,
+               reinterpret_cast<const bf16*>(d_z), d_in_w, d_in_b, d_cbn, d_cb_off, d_sizes, d_tabs, S, cd, T, D,
+               d_codes, d_valid);
     return 0;
 }
 

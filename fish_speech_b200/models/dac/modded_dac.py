@@ -580,73 +580,175 @@ class DAC:
     # -------------------------------------------------------------------------------------------
     # encode
     # -------------------------------------------------------------------------------------------
+    # encode routes to the streamed path when its one-shot workspaces would not fit in free device memory with a margin
+    # of this plus 5 % of the estimate left over (the caching allocator's rounding, the small buffers the estimate omits)
+    ENCODE_MARGIN_BYTES = 512 << 20
+    # the transformers' row-wise glue kernels launch one CTA row per token row (grid.y), so one pass takes at most this
+    # many rows per transformer: for the S2-Pro encoder transformer (4 rows per frame) about 12.7 minutes of audio
+    ONE_SHOT_MAX_ROWS = 65535
+    ENCODE_STREAM_FRAMES = 128  # frames per push of the streamed path (about 6 s at 44.1 kHz)
+    ENCODE_STREAM_SLOTS = 4  # batch rows encoded side by side by the streamed path
+
     @torch.inference_mode()
     def encode(self, audio_data: torch.Tensor, audio_lengths: Optional[torch.Tensor] = None,
                n_quantizers: Optional[int] = None, **kwargs):
-        """modded_dac.py:874-923: audio [B,1,N] or [B,N] -> (codes int64 [B, 1+n_codebooks, T], lens [B])."""
-        cfg = self.cfg
+        """modded_dac.py:874-923: audio [B,1,N] or [B,N] -> (codes int64 [B, 1+n_codebooks, T], lens [B]).
+        When the one-shot pass's workspaces fit in free device memory and its transformer rows fit its launches
+        (ONE_SHOT_MAX_ROWS), it runs as it always has; otherwise the batch is encoded through an EncodeStreamPool in
+        pieces of ENCODE_STREAM_FRAMES frames, in bounded memory and with the same codes and lengths."""
         with self._lock, torch.cuda.device(self._device):
-            if audio_data.ndim == 2:
-                audio_data = audio_data.unsqueeze(1)
-            length = audio_data.shape[-1]
-            right_pad = math.ceil(length / self.frame_length) * self.frame_length - length
-            wav = torch.nn.functional.pad(audio_data.to(device=self._device, dtype=torch.float32), (0, right_pad))
-            if audio_lengths is None:
-                audio_lengths = torch.LongTensor([length + right_pad]).to(self._device)
-            B, _, N = wav.shape
-            wav = wav.reshape(B, N).contiguous()
-            d0 = cfg.encoder_dim
-            numel = B * N * d0
-            bufs = [self._buf(f"enc_{k}", numel) for k in range(3)]
-            x, a, m = 0, 1, 2
-            r0 = self.enc_blocks[0]["res"][0]
-            _lib.check(self.lib.fsb_first_conv(wav.data_ptr(), self.enc_in_w.data_ptr(), self.enc_in_b.data_ptr(),
-                                               r0["s0"].alpha.data_ptr(), r0["s0"].inv.data_ptr(), B, N, d0,
-                                               self.enc_in_w.shape[1], bufs[x].data_ptr(), bufs[a].data_ptr(), _stream()))
-            Tc, c = N, d0
-            for bi, blk in enumerate(self.enc_blocks):
-                for j, ru in enumerate(blk["res"]):
-                    self._gemm(ru["c7"], bufs[a], B, Tc, c, Tc, out1=bufs[m], snake=ru["s1"])
-                    nxt = blk["res"][j + 1]["s0"] if j < 2 else blk["s_out"]
-                    self._gemm(ru["c1"], bufs[m], B, Tc, c, Tc, out0=bufs[x] if j < 2 else None, out1=bufs[a],
-                               snake=nxt, resid=bufs[x])
-                s, cout = blk["stride"], blk["dim"]
-                Tn = Tc // s
-                # strided conv reads the activation as [Tc/s][s*c] rows
-                last = bi + 1 == len(self.enc_blocks)
-                if blk["tfm"] is not None:
-                    self._gemm(blk["down"], bufs[a], B, Tn, s * c, Tn, out0=bufs[x])
-                    n_out = self._transformer(blk["tfm"], bufs[x], B, Tn, f"enc{bi}")
-                    sn = self.enc_out_snake if last else self.enc_blocks[bi + 1]["res"][0]["s0"]
-                    _lib.check(self.lib.fsb_snake(n_out.data_ptr(), sn.alpha.data_ptr(), sn.inv.data_ptr(),
-                                                  B * Tn * cout, cout, bufs[a].data_ptr(), _stream()))
-                    bufs[x][: B * Tn * cout].copy_(n_out[: B * Tn * cout])
-                else:
-                    sn = self.enc_out_snake if last else self.enc_blocks[bi + 1]["res"][0]["s0"]
-                    self._gemm(blk["down"], bufs[a], B, Tn, s * c, Tn, out0=bufs[x], out1=bufs[m], snake=sn)
-                    a, m = m, a
-                Tc, c = Tn, cout
-            z = self._buf("enc_z", B * Tc * cfg.latent_dim)
-            self._gemm(self.enc_out, bufs[a], B, Tc, c, Tc, out0=z)
-            # ---- quantizer.forward up to the codes (rvq.py:293-317) ----
-            D = cfg.latent_dim
-            cur = z
-            for i, dn in enumerate(self.down):
-                f = dn["f"]
-                Tn = Tc // f
-                out = self._buf(f"down_{i}", B * Tn * D)
-                self._gemm(dn["conv"], cur, B, Tn, f * D, Tn, out0=out)
-                self._convnext_block(dn["cnx"], out, B, Tn, D, f"down{i}")
-                cur, Tc = out, Tn
-            zq = self._transformer(self.pre_tfm, cur, B, Tc, "pre")
-            S = self.n_stage if n_quantizers is None else min(self.n_stage, 1 + int(n_quantizers))
-            codes = torch.empty(B, S, Tc, dtype=torch.int32, device=self._device)
-            _lib.check(self.lib.fsb_vq_encode(zq.data_ptr(), self.vq_in_w.data_ptr(), self.vq_in_b.data_ptr(),
-                                              self.vq_cbn.data_ptr(), self.vq_cb_off.data_ptr(), self.vq_sizes.data_ptr(),
-                                              self.vq_tab_ptrs.data_ptr(), S, cfg.codebook_dim, B, Tc, D,
-                                              codes.data_ptr(), _stream()))
-            indices_lens = torch.ceil(audio_lengths.to(self._device) / self.frame_length).long()
-            return codes.long(), indices_lens
+            B, length = audio_data.shape[0], audio_data.shape[-1]
+            N = math.ceil(length / self.frame_length) * self.frame_length
+            need = self._encode_one_shot_bytes(B, N)
+            rows = max(r for _, r in self._encode_one_shot_tfm_rows(B, N))
+            fits = need + need // 20 + self.ENCODE_MARGIN_BYTES <= self._free_device_bytes()
+            if fits and rows <= self.ONE_SHOT_MAX_ROWS:
+                return self._encode_one_shot(audio_data, audio_lengths, n_quantizers)
+            return self._encode_streamed(audio_data, audio_lengths, n_quantizers)
+
+    def _free_device_bytes(self) -> int:
+        """Device memory a new allocation can use: free on the device plus what the caching allocator holds unused."""
+        free, _ = torch.cuda.mem_get_info(self._device)
+        return free + torch.cuda.memory_reserved(self._device) - torch.cuda.memory_allocated(self._device)
+
+    def _encode_one_shot_bytes(self, B: int, N: int) -> int:
+        """Bytes the one-shot encode of B x N padded samples would allocate: its fp32 waveform copy and codes, plus every
+        named workspace that is not already large enough (a workspace that grows is allocated before the old one is
+        released). The bf16 encoder activations (3 x B x N x encoder_dim) dominate."""
+        cfg = self.cfg
+
+        def grow(name: str, numel: int, elt: int = 2, dtype=torch.bfloat16) -> int:
+            b = self._bufs.get(name)
+            return 0 if b is not None and b.numel() >= numel and b.dtype == dtype else max(numel, 1) * elt
+
+        need = 2 * B * N * 4  # the padded fp32 waveform (and the input's conversion to it)
+        need += sum(grow(f"enc_{k}", B * N * cfg.encoder_dim) for k in range(3))
+        T = N // self.hop_length
+        D = cfg.latent_dim
+        need += grow("enc_z", B * T * D)
+        for i, f in enumerate(cfg.downsample_factor):
+            T //= f
+            need += grow(f"down_{i}", B * T * D) + grow("cnx_y", B * T * D) + grow("cnx_h", B * T * 4 * D)
+        for tf, rows in self._encode_one_shot_tfm_rows(B, N):
+            t: TfmConfig = tf["cfg"]
+            HD = t.n_head * t.head_dim
+            need += grow("tf_ws", rows * max(3 * HD, 2 * t.intermediate_size, t.dim), 4, torch.float32)
+            need += grow("tf_n", rows * t.dim) + sum(grow(f"tf_{k}", rows * HD) for k in ("q", "k", "v", "att"))
+            need += grow("tf_h", rows * t.intermediate_size) + 3 * rows * 4  # + row (sequence, position), arange
+        need += B * self.n_stage * T * (4 + 8)  # int32 codes and their int64 copy
+        return need
+
+    def _encode_one_shot_tfm_rows(self, B: int, N: int) -> list:
+        """(transformer, rows) of every transformer the one-shot encode of B x N padded samples runs."""
+        out = [(blk["tfm"], B * N // math.prod(self.encoder_rates[: i + 1]))
+               for i, blk in enumerate(self.enc_blocks) if blk["tfm"] is not None]
+        return out + [(self.pre_tfm, B * N // self.hop_length // math.prod(self.cfg.downsample_factor))]
+
+    def _encode_streamed(self, audio_data: torch.Tensor, audio_lengths: Optional[torch.Tensor],
+                         n_quantizers: Optional[int]):
+        """encode through an EncodeStreamPool: ENCODE_STREAM_SLOTS batch rows at a time, each pushed as whole frames of
+        its waveform zero-padded to the batch's padded length, as the one-shot pass sees it."""
+        FL = self.frame_length
+        B, length = audio_data.shape[0], audio_data.shape[-1]
+        wav = audio_data.reshape(B, length)
+        T = math.ceil(length / FL)
+        k = self.ENCODE_STREAM_FRAMES
+        pool = self.open_encode_pool(min(B, self.ENCODE_STREAM_SLOTS), k_max=k, n_quantizers=n_quantizers)
+        codes = torch.empty(B, pool.n_stage, T, dtype=torch.int64, device=self._device)
+        for b0 in range(0, B, pool.slots):
+            rows = range(b0, min(B, b0 + pool.slots))
+            slot = {b: pool.open() for b in rows}
+            for f0 in range(0, T, k):
+                f1 = min(T, f0 + k)
+                pieces = {}
+                for b in rows:
+                    piece = wav[b, f0 * FL: f1 * FL].to(torch.float32)
+                    if piece.numel() < (f1 - f0) * FL:  # encode's right pad
+                        piece = torch.nn.functional.pad(piece, (0, (f1 - f0) * FL - piece.numel()))
+                    pieces[slot[b]] = piece
+                out = pool.push(pieces)
+                for b in rows:
+                    codes[b, :, f0:f1] = out[slot[b]]
+            for b in rows:
+                pool.close(slot[b])
+        if audio_lengths is None:
+            audio_lengths = torch.LongTensor([T * FL])
+        indices_lens = torch.ceil(audio_lengths.to(self._device) / FL).long()
+        return codes, indices_lens
+
+    def open_encode_pool(self, slots: int, k_max: int = 32, n_quantizers: Optional[int] = None,
+                         max_graphs: int = 8) -> "EncodeStreamPool":
+        """Streaming `encode` of up to `slots` independent streams at once: streams join and leave at any push, and one
+        push encodes the new frames of every stream that has some in one batched (graph-replayed) pass, in memory that
+        does not grow with a stream's length. Each stream's codes are bit-identical to `encode` of its waveform alone.
+        See EncodeStreamPool."""
+        return EncodeStreamPool(self, slots, k_max, n_quantizers, max_graphs)
+
+    def _encode_one_shot(self, audio_data: torch.Tensor, audio_lengths: Optional[torch.Tensor],
+                         n_quantizers: Optional[int]):
+        """Every layer over the whole (padded) batch at once."""
+        cfg = self.cfg
+        if audio_data.ndim == 2:
+            audio_data = audio_data.unsqueeze(1)
+        length = audio_data.shape[-1]
+        right_pad = math.ceil(length / self.frame_length) * self.frame_length - length
+        wav = torch.nn.functional.pad(audio_data.to(device=self._device, dtype=torch.float32), (0, right_pad))
+        if audio_lengths is None:
+            audio_lengths = torch.LongTensor([length + right_pad]).to(self._device)
+        B, _, N = wav.shape
+        wav = wav.reshape(B, N).contiguous()
+        d0 = cfg.encoder_dim
+        numel = B * N * d0
+        bufs = [self._buf(f"enc_{k}", numel) for k in range(3)]
+        x, a, m = 0, 1, 2
+        r0 = self.enc_blocks[0]["res"][0]
+        _lib.check(self.lib.fsb_first_conv(wav.data_ptr(), self.enc_in_w.data_ptr(), self.enc_in_b.data_ptr(),
+                                           r0["s0"].alpha.data_ptr(), r0["s0"].inv.data_ptr(), B, N, d0,
+                                           self.enc_in_w.shape[1], bufs[x].data_ptr(), bufs[a].data_ptr(), _stream()))
+        Tc, c = N, d0
+        for bi, blk in enumerate(self.enc_blocks):
+            for j, ru in enumerate(blk["res"]):
+                self._gemm(ru["c7"], bufs[a], B, Tc, c, Tc, out1=bufs[m], snake=ru["s1"])
+                nxt = blk["res"][j + 1]["s0"] if j < 2 else blk["s_out"]
+                self._gemm(ru["c1"], bufs[m], B, Tc, c, Tc, out0=bufs[x] if j < 2 else None, out1=bufs[a],
+                           snake=nxt, resid=bufs[x])
+            s, cout = blk["stride"], blk["dim"]
+            Tn = Tc // s
+            # strided conv reads the activation as [Tc/s][s*c] rows
+            last = bi + 1 == len(self.enc_blocks)
+            if blk["tfm"] is not None:
+                self._gemm(blk["down"], bufs[a], B, Tn, s * c, Tn, out0=bufs[x])
+                n_out = self._transformer(blk["tfm"], bufs[x], B, Tn, f"enc{bi}")
+                sn = self.enc_out_snake if last else self.enc_blocks[bi + 1]["res"][0]["s0"]
+                _lib.check(self.lib.fsb_snake(n_out.data_ptr(), sn.alpha.data_ptr(), sn.inv.data_ptr(),
+                                              B * Tn * cout, cout, bufs[a].data_ptr(), _stream()))
+                bufs[x][: B * Tn * cout].copy_(n_out[: B * Tn * cout])
+            else:
+                sn = self.enc_out_snake if last else self.enc_blocks[bi + 1]["res"][0]["s0"]
+                self._gemm(blk["down"], bufs[a], B, Tn, s * c, Tn, out0=bufs[x], out1=bufs[m], snake=sn)
+                a, m = m, a
+            Tc, c = Tn, cout
+        z = self._buf("enc_z", B * Tc * cfg.latent_dim)
+        self._gemm(self.enc_out, bufs[a], B, Tc, c, Tc, out0=z)
+        # ---- quantizer.forward up to the codes (rvq.py:293-317) ----
+        D = cfg.latent_dim
+        cur = z
+        for i, dn in enumerate(self.down):
+            f = dn["f"]
+            Tn = Tc // f
+            out = self._buf(f"down_{i}", B * Tn * D)
+            self._gemm(dn["conv"], cur, B, Tn, f * D, Tn, out0=out)
+            self._convnext_block(dn["cnx"], out, B, Tn, D, f"down{i}")
+            cur, Tc = out, Tn
+        zq = self._transformer(self.pre_tfm, cur, B, Tc, "pre")
+        S = self.n_stage if n_quantizers is None else min(self.n_stage, 1 + int(n_quantizers))
+        codes = torch.empty(B, S, Tc, dtype=torch.int32, device=self._device)
+        _lib.check(self.lib.fsb_vq_encode(zq.data_ptr(), self.vq_in_w.data_ptr(), self.vq_in_b.data_ptr(),
+                                          self.vq_cbn.data_ptr(), self.vq_cb_off.data_ptr(), self.vq_sizes.data_ptr(),
+                                          self.vq_tab_ptrs.data_ptr(), S, cfg.codebook_dim, B, Tc, D,
+                                          codes.data_ptr(), _stream()))
+        indices_lens = torch.ceil(audio_lengths.to(self._device) / self.frame_length).long()
+        return codes.long(), indices_lens
 
 
 class DecodeStream:
@@ -715,74 +817,29 @@ def _pow2(n: int) -> int:
     return 1 << max(0, int(n) - 1).bit_length()
 
 
-class DecodeStreamPool:
-    """Streaming `from_indices` of up to `slots` independent streams (one utterance each), decoded together; a push
-    computes only the new frames of the streams in it.
+class _StreamPool:
+    """Slot, bucket and CUDA-graph bookkeeping shared by DecodeStreamPool and EncodeStreamPool.
 
-    * post-transformer: per slot and layer a K/V ring of R = round_up(window + k_max + 63, 64) positions
-      (fsb_qkv_rope_ring / fsb_window_attn_ring): the attention walks the same absolute 64-position tiles as over a
-      linear cache, so the result is the same; memory is fixed per slot and a stream has no length cap.
-    * upsampler + decoder: every causal conv keeps its own left context per slot, the last (taps - 1) * dilation rows
-      of its input in the form the conv reads it (Snake-activated where the Snake is fused upstream): ConvTranspose 1
-      row, ConvNeXt depthwise 6, the dilated k7 convs 6 * d, the final conv K - 1. A layer's input is a window
-      [stream][H + new rows][C]: fsb_window_fill puts the slot's history in rows 0..H-1 and the producer's new rows after
-      it, the consumer computes only the new rows (conv GEMM taps shifted by H, fsb_dwconv_ln_window), and
-      fsb_window_roll keeps the last H valid rows as the slot's next history. At stream start the history is zeros, as
-      the zero fill at negative time of the one-shot decode. The decoder's ResidualUnits run as their two conv GEMMs
-      (bit-identical to the fused kernel); the final conv runs over the window and its history rows are dropped.
-    * ragged pushes: the streams are padded to the largest frame count; padding rows follow a stream's valid rows, so
-      a causal layer never carries them into a valid row, and the roll takes valid rows only. Padding rows of the
-      transformer attend in a scratch sequence of their own. Slots outside a push are not touched.
-    * each (stream bucket, frame bucket) shape, powers of two, is captured into a CUDA graph the second time it is seen
-      (at most `max_graphs`; others run eagerly), on the calling thread.
-    * a push that fails leaves the state of its slots undefined: they refuse further pushes until closed.
-    """
+    A subclass sets `layers` (one (history rows, row width in bf16 units, rows per frame) per windowed conv input, in
+    execution order), `kv` (its transformers' ring K/V) and `_tfms` ((TfmConfig, rows per frame) per transformer), and
+    supplies the piece-specific parts of a push: `_check_piece`, `_frames`, `_describe` (host-side description of a
+    push), `_alloc_static` / `_stage` (the device buffers a pass reads), `_body` (the device work) and `_outputs`."""
+
+    _fill = "fsb_window_fill"  # the entry point that builds a layer's input window
 
     def __init__(self, dac: "DAC", slots: int, k_max: int, max_graphs: int):
-        t: TfmConfig = dac.post_tfm["cfg"]
-        if slots < 1 or k_max < 1:
-            raise ValueError(f"stream pool needs slots >= 1 and k_max >= 1 (got {slots}, {k_max})")
-        if not t.window_size or t.window_size <= 0:
-            raise ValueError("stream pool needs a window-limited post-transformer")
         self.dac, self.slots, self.k_max, self.max_graphs = dac, int(slots), int(k_max), int(max_graphs)
-        self.ring = _pad64(t.window_size + self.k_max + 63)
-        dev = dac.device
-        # slot `slots` is the scratch sequence of padding rows
-        n = (self.slots + 1) * t.n_head * (self.ring + 64) * t.head_dim
-        self.kv = [(torch.zeros(n, dtype=torch.bfloat16, device=dev), torch.zeros(n, dtype=torch.bfloat16, device=dev))
-                   for _ in dac.post_tfm["layers"]]
-        # one (H rows, C channels, rows per frame) per conv input of the upsampler + decoder, in execution order
-        self.layers = self._layer_geometry()
-        self.hist = [torch.zeros(max(1, self.slots * H * Cc), dtype=torch.bfloat16, device=dev)
+        self.hist = [torch.zeros(max(1, self.slots * H * Cc), dtype=torch.bfloat16, device=dac.device)
                      for H, Cc, _ in self.layers]
         self.rates = sorted({r for _, _, r in self.layers})
         self.pos = [0] * self.slots
         self.live = [False] * self.slots
         self.broken = [False] * self.slots
-        self._graphs: dict = {}  # (nb, kb) -> (CUDAGraph, static waveform)
+        self._graphs: dict = {}  # (nb, kb) -> (CUDAGraph, static result)
         self._seen: dict = {}
         self._gen = dac._ws_gen
-        self._static: dict = {}  # (nb, kb) -> (idx, meta) device buffers the pass reads
+        self._static: dict = {}  # (nb, kb) -> device buffers the pass reads
         self._shifts: dict = {}
-
-    def _layer_geometry(self) -> list:
-        dac, D = self.dac, self.dac.cfg.latent_dim
-        out, r = [], 1
-        for u in dac.up:
-            out.append((-min(u["conv"].shifts), D, r))
-            r *= u["f"]
-            out.append((u["cnx"]["k"] - 1, D, r))
-        out.append((-min(dac.dec_in.shifts), D, r))
-        cin = dac.cfg.decoder_dim
-        for blk in dac.dec_blocks:
-            out.append((-min(blk["up"].shifts), cin, r))
-            r *= blk["stride"]
-            cin //= 2
-            for ru in blk["res"]:
-                assert ru["c1"].taps == 1
-                out.append((-min(ru["c7"].shifts), cin, r))
-        out.append((dac.dec_out_k - 1, cin, r))
-        return out
 
     @property
     def state_bytes(self) -> int:
@@ -815,52 +872,27 @@ class DecodeStreamPool:
 
     @torch.inference_mode()
     def push(self, pieces: dict) -> dict:
-        """{slot: codes [1+n_codebooks, k]} (1 <= k <= k_max) of the next frames of each stream -> {slot: waveform fp32
-        [k * frame_length]}. The caller's tensors are not modified."""
-        dac, cfg = self.dac, self.dac.cfg
-        S_ = dac.n_stage
+        """{slot: next piece of that stream} -> {slot: its result} (the piece and result formats are the subclass's).
+        The caller's tensors are not modified."""
+        dac = self.dac
         items = list(pieces.items())
-        for slot, codes in items:
+        for slot, piece in items:
             self._check_slot(slot)
             if self.broken[slot]:
                 raise ValueError(f"slot {slot}: an earlier push failed, its state is lost; close the slot")
-            if codes.ndim != 2 or codes.shape[0] != S_:
-                raise ValueError(f"slot {slot}: codes must be [{S_}, k], got {tuple(codes.shape)}")
-            if not 1 <= codes.shape[1] <= self.k_max:
-                raise ValueError(f"slot {slot}: {codes.shape[1]} frames, a push takes 1 .. {self.k_max}")
+            self._check_piece(slot, piece)
         if not items:
             return {}
-        n = len(items)
-        ks = [int(c.shape[1]) for _, c in items]
-        nb = min(_pow2(n), self.slots)
+        ks = [self._frames(piece) for _, piece in items]
+        nb = min(_pow2(len(items)), self.slots)
         kb = min(_pow2(max(ks)), self.k_max)
-        FL = dac.frame_length
-        scratch = self.slots
         with dac._lock, torch.cuda.device(dac.device):
-            # ---- host-side description of the push: rows, positions, slots and valid rows per rate ----
-            row_seq = [scratch] * (nb * kb)
-            row_pos = [j for _ in range(nb) for j in range(kb)]
-            slot_of = [-1] * nb
-            valid = {r: [0] * nb for r in self.rates}
-            for i, ((slot, _), k) in enumerate(zip(items, ks)):
-                p = self.pos[slot]
-                slot_of[i] = slot
-                for j in range(k):
-                    row_seq[i * kb + j], row_pos[i * kb + j] = slot, p + j
-                for r in self.rates:
-                    valid[r][i] = k * r
-            meta_h = torch.tensor(row_seq + row_pos + slot_of + [v for r in self.rates for v in valid[r]],
-                                  dtype=torch.int32)
-            idx_h = torch.zeros(nb, S_, kb, dtype=torch.int32)
-            for i, (_, codes) in enumerate(items):
-                idx_h[i, :, : ks[i]] = codes.to(device="cpu", dtype=torch.int32)
-            idx_h[:, 0].clamp_(min=0, max=cfg.semantic_codebook_size - 1)  # rvq.py:354-359 (on our copy)
-            idx_h[:, 1:].clamp_(min=0, max=cfg.codebook_size - 1)
+            host = self._describe(items, ks, nb, kb)
             # ---- the RoPE table must cover every position before a graph captures its address ----
-            t: TfmConfig = dac.post_tfm["cfg"]
             top = max(self.pos[s] + k for (s, _), k in zip(items, ks))
-            rope_len = max(1024, _pow2(max(top, kb)))
-            dac._rope_table(rope_len, t.head_dim, t.rope_base)
+            rope_len = max(1024, _pow2(max(top, kb) * max(r for _, r in self._tfms)))
+            for t, _ in self._tfms:
+                dac._rope_table(rope_len, t.head_dim, t.rope_base)
             if self._gen != dac._ws_gen:  # a workspace a graph points into was re-allocated
                 self._graphs.clear()
                 self._seen.clear()
@@ -868,31 +900,29 @@ class DecodeStreamPool:
             key = (nb, kb)
             st = self._static.get(key)
             if st is None:
-                st = (torch.empty(nb * S_ * kb, dtype=torch.int32, device=dac.device),
-                      torch.empty(meta_h.numel(), dtype=torch.int32, device=dac.device))
+                st = self._alloc_static(nb, kb, host)
                 self._static[key] = st
             try:
-                st[0].copy_(idx_h.reshape(-1))
-                st[1].copy_(meta_h)
+                self._stage(st, items, ks, host)
                 hit = self._graphs.get(key)
                 if hit is not None:
                     hit[0].replay()
-                    wav = hit[1]
+                    res = hit[1]
                 else:
                     seen = self._seen.get(key, 0)
                     self._seen[key] = seen + 1
                     if seen == 0 or len(self._graphs) >= self.max_graphs:
-                        wav = self._body(nb, kb, st, rope_len)
+                        res = self._body(nb, kb, st, rope_len)
                     else:
                         torch.cuda.current_stream().synchronize()
                         graph = torch.cuda.CUDAGraph()
                         with torch.cuda.graph(graph, capture_error_mode="thread_local"):  # other threads keep running
-                            wav = self._body(nb, kb, st, rope_len)
+                            res = self._body(nb, kb, st, rope_len)
                         if self._gen != dac._ws_gen:
                             raise RuntimeError("stream pool: a workspace was re-allocated during graph capture")
-                        self._graphs[key] = (graph, wav)
+                        self._graphs[key] = (graph, res)
                         graph.replay()
-                out = {slot: wav[i, : k * FL].clone() for i, ((slot, _), k) in enumerate(zip(items, ks))}
+                out = self._outputs(res, items, ks)
             except BaseException:
                 for slot, _ in items:  # the device work may have advanced part of their state
                     self.broken[slot] = True
@@ -915,6 +945,134 @@ class DecodeStreamPool:
             snake.alpha.data_ptr() if snake is not None else None,
             snake.inv.data_ptr() if snake is not None else None, 0, _stream()))
 
+    def _windows(self, nb: int, slot_t: torch.Tensor, valid: dict, ws: str):
+        """A function (dense new rows [nb][n][row], n) -> (window of the next windowed layer, its history rows H): fills
+        the window from the slot's history and the new rows and rolls the slot's history (layers in execution order)."""
+        dac, L, chk = self.dac, self.dac.lib, _lib.check
+        fill = getattr(L, self._fill)
+        layer = iter(range(len(self.layers)))
+
+        def window(dense: torch.Tensor, n: int):
+            li = next(layer)
+            H, Cc, r = self.layers[li]
+            win = dac._buf(ws, nb * (H + n) * Cc)
+            chk(fill(self.hist[li].data_ptr(), dense.data_ptr(), win.data_ptr(), slot_t.data_ptr(), valid[r].data_ptr(),
+                     nb, H, n, Cc * 2, _stream()))
+            chk(L.fsb_window_roll(win.data_ptr(), self.hist[li].data_ptr(), slot_t.data_ptr(), valid[r].data_ptr(),
+                                  nb, H, n, Cc * 2, _stream()))
+            return win, H
+
+        return window
+
+
+class DecodeStreamPool(_StreamPool):
+    """Streaming `from_indices` of up to `slots` independent streams (one utterance each), decoded together; a push
+    computes only the new frames of the streams in it: push({slot: codes [1+n_codebooks, k]}, 1 <= k <= k_max) ->
+    {slot: waveform fp32 [k * frame_length]}.
+
+    * post-transformer: per slot and layer a K/V ring of R = round_up(window + k_max + 63, 64) positions
+      (fsb_qkv_rope_ring / fsb_window_attn_ring): the attention walks the same absolute 64-position tiles as over a
+      linear cache, so the result is the same; memory is fixed per slot and a stream has no length cap.
+    * upsampler + decoder: every causal conv keeps its own left context per slot, the last (taps - 1) * dilation rows
+      of its input in the form the conv reads it (Snake-activated where the Snake is fused upstream): ConvTranspose 1
+      row, ConvNeXt depthwise 6, the dilated k7 convs 6 * d, the final conv K - 1. A layer's input is a window
+      [stream][H + new rows][C]: fsb_window_fill puts the slot's history in rows 0..H-1 and the producer's new rows after
+      it, the consumer computes only the new rows (conv GEMM taps shifted by H, fsb_dwconv_ln_window), and
+      fsb_window_roll keeps the last H valid rows as the slot's next history. At stream start the history is zeros, as
+      the zero fill at negative time of the one-shot decode. The decoder's ResidualUnits run as their two conv GEMMs
+      (bit-identical to the fused kernel); the final conv runs over the window and its history rows are dropped.
+    * ragged pushes: the streams are padded to the largest frame count; padding rows follow a stream's valid rows, so
+      a causal layer never carries them into a valid row, and the roll takes valid rows only. Padding rows of the
+      transformer attend in a scratch sequence of their own. Slots outside a push are not touched.
+    * each (stream bucket, frame bucket) shape, powers of two, is captured into a CUDA graph the second time it is seen
+      (at most `max_graphs`; others run eagerly), on the calling thread.
+    * a push that fails leaves the state of its slots undefined: they refuse further pushes until closed.
+    """
+
+    def __init__(self, dac: "DAC", slots: int, k_max: int, max_graphs: int):
+        t: TfmConfig = dac.post_tfm["cfg"]
+        if slots < 1 or k_max < 1:
+            raise ValueError(f"stream pool needs slots >= 1 and k_max >= 1 (got {slots}, {k_max})")
+        if not t.window_size or t.window_size <= 0:
+            raise ValueError("stream pool needs a window-limited post-transformer")
+        self.dac = dac
+        self.ring = _pad64(t.window_size + int(k_max) + 63)
+        # slot `slots` is the scratch sequence of padding rows
+        n = (int(slots) + 1) * t.n_head * (self.ring + 64) * t.head_dim
+        self.kv = [(torch.zeros(n, dtype=torch.bfloat16, device=dac.device),
+                    torch.zeros(n, dtype=torch.bfloat16, device=dac.device)) for _ in dac.post_tfm["layers"]]
+        self._tfms = [(t, 1)]
+        # one (H rows, C channels, rows per frame) per conv input of the upsampler + decoder, in execution order
+        self.layers = self._layer_geometry()
+        super().__init__(dac, slots, k_max, max_graphs)
+
+    def _layer_geometry(self) -> list:
+        dac, D = self.dac, self.dac.cfg.latent_dim
+        out, r = [], 1
+        for u in dac.up:
+            out.append((-min(u["conv"].shifts), D, r))
+            r *= u["f"]
+            out.append((u["cnx"]["k"] - 1, D, r))
+        out.append((-min(dac.dec_in.shifts), D, r))
+        cin = dac.cfg.decoder_dim
+        for blk in dac.dec_blocks:
+            out.append((-min(blk["up"].shifts), cin, r))
+            r *= blk["stride"]
+            cin //= 2
+            for ru in blk["res"]:
+                assert ru["c1"].taps == 1
+                out.append((-min(ru["c7"].shifts), cin, r))
+        out.append((dac.dec_out_k - 1, cin, r))
+        return out
+
+    def _check_piece(self, slot: int, codes) -> None:
+        S_ = self.dac.n_stage
+        if codes.ndim != 2 or codes.shape[0] != S_:
+            raise ValueError(f"slot {slot}: codes must be [{S_}, k], got {tuple(codes.shape)}")
+        if not 1 <= codes.shape[1] <= self.k_max:
+            raise ValueError(f"slot {slot}: {codes.shape[1]} frames, a push takes 1 .. {self.k_max}")
+
+    @staticmethod
+    def _frames(codes) -> int:
+        return int(codes.shape[1])
+
+    def _describe(self, items: list, ks: list, nb: int, kb: int) -> tuple:
+        """Host-side description of a push: rows, positions, slots and valid rows per rate; the clamped codes."""
+        cfg, S_ = self.dac.cfg, self.dac.n_stage
+        scratch = self.slots
+        row_seq = [scratch] * (nb * kb)
+        row_pos = [j for _ in range(nb) for j in range(kb)]
+        slot_of = [-1] * nb
+        valid = {r: [0] * nb for r in self.rates}
+        for i, ((slot, _), k) in enumerate(zip(items, ks)):
+            p = self.pos[slot]
+            slot_of[i] = slot
+            for j in range(k):
+                row_seq[i * kb + j], row_pos[i * kb + j] = slot, p + j
+            for r in self.rates:
+                valid[r][i] = k * r
+        meta_h = torch.tensor(row_seq + row_pos + slot_of + [v for r in self.rates for v in valid[r]],
+                              dtype=torch.int32)
+        idx_h = torch.zeros(nb, S_, kb, dtype=torch.int32)
+        for i, (_, codes) in enumerate(items):
+            idx_h[i, :, : ks[i]] = codes.to(device="cpu", dtype=torch.int32)
+        idx_h[:, 0].clamp_(min=0, max=cfg.semantic_codebook_size - 1)  # rvq.py:354-359 (on our copy)
+        idx_h[:, 1:].clamp_(min=0, max=cfg.codebook_size - 1)
+        return idx_h, meta_h
+
+    def _alloc_static(self, nb: int, kb: int, host: tuple) -> tuple:
+        return (torch.empty(nb * self.dac.n_stage * kb, dtype=torch.int32, device=self.dac.device),
+                torch.empty(host[1].numel(), dtype=torch.int32, device=self.dac.device))
+
+    @staticmethod
+    def _stage(st: tuple, items: list, ks: list, host: tuple) -> None:
+        st[0].copy_(host[0].reshape(-1))
+        st[1].copy_(host[1])
+
+    def _outputs(self, wav: torch.Tensor, items: list, ks: list) -> dict:
+        FL = self.dac.frame_length
+        return {slot: wav[i, : k * FL].clone() for i, ((slot, _), k) in enumerate(zip(items, ks))}
+
     def _body(self, nb: int, kb: int, st: tuple, rope_len: int) -> torch.Tensor:
         """The device work of one push (eager or under capture): codes -> transformer (ring K/V) -> upsampler + decoder,
         each conv on a window of its slot's history + the new rows -> waveform [nb, kb * frame_length]."""
@@ -930,18 +1088,7 @@ class DecodeStreamPool:
                                z.data_ptr(), _stream()))
         x = dac._transformer(dac.post_tfm, z, nb, kb, "post", kv_cache=self.kv, cache_len=self.ring,
                              rows_at=(row_seq, row_pos), ring=True, rope_len=rope_len)
-        layer = iter(range(len(self.layers)))
-
-        def window(dense: torch.Tensor, n: int):
-            """The next layer's input window from its new rows `dense` [nb][n][C]; rolls the slot's history."""
-            li = next(layer)
-            H, Cc, r = self.layers[li]
-            win = dac._buf("pl_win", nb * (H + n) * Cc)
-            chk(L.fsb_window_fill(self.hist[li].data_ptr(), dense.data_ptr(), win.data_ptr(), slot_t.data_ptr(),
-                                  valid[r].data_ptr(), nb, H, n, Cc * 2, _stream()))
-            chk(L.fsb_window_roll(win.data_ptr(), self.hist[li].data_ptr(), slot_t.data_ptr(), valid[r].data_ptr(),
-                                  nb, H, n, Cc * 2, _stream()))
-            return win, H
+        window = self._windows(nb, slot_t, valid, "pl_win")
 
         n = kb
         for i, u in enumerate(dac.up):
@@ -995,6 +1142,214 @@ class DecodeStreamPool:
         chk(L.fsb_final_conv_tanh(win.data_ptr(), dac.dec_out_w.data_ptr(), dac.dec_out_b, nb, H + n, cin,
                                   dac.dec_out_k, wav.data_ptr(), _stream()))
         return wav[:, H:]
+
+
+class EncodeStreamPool(_StreamPool):
+    """Streaming `encode` of up to `slots` independent streams, encoded together; a push computes only the new frames of
+    the streams in it: push({slot: waveform fp32 [k * frame_length]}, 1 <= k <= k_max) -> {slot: codes int64
+    [n_stages, k]}. A stream's codes, concatenated, are bit-identical to `DAC.encode` of its whole waveform alone (a
+    last partial frame is zero-padded by the caller, which is exactly encode's right pad). The encoder is causal from
+    end to end, so every layer keeps only what its next rows read:
+
+    * first conv: the last K - 1 = 6 samples of the waveform, kept as 2 rows of 4 fp32 samples (16-byte rows for
+      fsb_window_fill / roll) and read by fsb_first_conv_window.
+    * encoder ResidualUnits: the dilated k7 conv keeps 6 * dilation rows of its Snake-activated input (6, 18, 54); the
+      k1 conv and the residual need none.
+    * strided `down` convs (k = 2 * stride, read as [T / stride][stride * C] rows, 2 taps): one row of that view; the
+      plain conv GEMM over the window computes them. `enc_out` (k3): 2 rows. The quantizer's downsample convs have
+      k = stride (one tap) and need no history. ConvNeXt depthwise convs: 6 rows.
+    * transformers: the encoder's (window 512 at 4 rows per frame) and `pre_module` (window 128 at 1 row per frame)
+      keep their K/V in rings of R = round_up(window + rows per frame * k_max + 63, 64) positions per slot and layer
+      (fsb_qkv_rope_ring / fsb_window_attn_ring), at absolute positions that grow without bound.
+    * ragged pushes, padding rows, the scratch sequence, graph capture and failed pushes as in DecodeStreamPool, except
+      that every window's padding rows are zeroed (fsb_window_fill_zero). The shared window buffer holds other layers'
+      rows before (the waveform window's fp32 samples read as bf16 can be Inf or NaN), and the tiled window attention
+      adds zero-weighted V rows of every run in a query tile into each row of the tile: a non-finite V in the scratch
+      sequence would turn valid rows into NaN, and the vector quantiser a NaN latent into an out-of-range code index.
+    """
+
+    _fill = "fsb_window_fill_zero"
+
+    def __init__(self, dac: "DAC", slots: int, k_max: int, n_quantizers: Optional[int], max_graphs: int):
+        if slots < 1 or k_max < 1:
+            raise ValueError(f"stream pool needs slots >= 1 and k_max >= 1 (got {slots}, {k_max})")
+        cfg, FL = dac.cfg, dac.frame_length
+        self.dac = dac
+        self.n_stage = dac.n_stage if n_quantizers is None else min(dac.n_stage, 1 + int(n_quantizers))
+        # the transformers in execution order, with their rows per frame; slot `slots` is the scratch sequence
+        tfms, r = [], FL
+        for blk in dac.enc_blocks:
+            r //= blk["stride"]
+            if blk["tfm"] is not None:
+                tfms.append((blk["tfm"], r))
+        tfms.append((dac.pre_tfm, r // int(math.prod(cfg.downsample_factor))))
+        self._tfms, self.rings, self.kv_t = [], [], []
+        for tf, r in tfms:
+            t: TfmConfig = tf["cfg"]
+            if not t.window_size or t.window_size <= 0:
+                raise ValueError("encode stream pool needs window-limited transformers")
+            if (int(slots) * int(k_max) * r > DAC.ONE_SHOT_MAX_ROWS):
+                raise ValueError(f"encode stream pool: slots x k_max x {r} transformer rows per frame = "
+                                 f"{int(slots) * int(k_max) * r} exceeds the {DAC.ONE_SHOT_MAX_ROWS} rows one launch takes")
+            R = _pad64(t.window_size + r * int(k_max) + 63)
+            n = (int(slots) + 1) * t.n_head * (R + 64) * t.head_dim
+            self._tfms.append((t, r))
+            self.rings.append(R)
+            self.kv_t.append([(torch.zeros(n, dtype=torch.bfloat16, device=dac.device),
+                               torch.zeros(n, dtype=torch.bfloat16, device=dac.device)) for _ in tf["layers"]])
+        self.kv = [kv for layers in self.kv_t for kv in layers]
+        self.layers = self._layer_geometry()
+        super().__init__(dac, slots, k_max, max_graphs)
+
+    def _layer_geometry(self) -> list:
+        """(H rows, row width in bf16 units, rows per frame) per windowed layer input, in execution order."""
+        dac, cfg = self.dac, self.dac.cfg
+        FL = dac.frame_length
+        out = [(-(-(dac.enc_in_w.shape[1] - 1) // 4), 8, FL // 4)]  # waveform: rows of 4 fp32 samples
+        r, c = FL, cfg.encoder_dim
+        for blk in dac.enc_blocks:
+            for ru in blk["res"]:
+                assert ru["c1"].taps == 1
+                out.append((-min(ru["c7"].shifts), c, r))
+            s = blk["stride"]
+            r //= s
+            out.append((-min(blk["down"].shifts), s * c, r))
+            c = blk["dim"]
+        out.append((-min(dac.enc_out.shifts), c, r))
+        for dn in dac.down:
+            assert dn["conv"].taps == 1  # kernel = stride: no history
+            r //= dn["f"]
+            out.append((dn["cnx"]["k"] - 1, cfg.latent_dim, r))
+        return out
+
+    def _check_piece(self, slot: int, wav) -> None:
+        FL = self.dac.frame_length
+        if not isinstance(wav, torch.Tensor) or wav.ndim != 1 or wav.dtype != torch.float32:
+            raise ValueError(f"slot {slot}: a piece must be a 1-D float32 waveform")
+        if wav.numel() % FL:
+            raise ValueError(f"slot {slot}: {wav.numel()} samples is not a whole number of {FL}-sample frames "
+                             "(zero-pad the last piece)")
+        if not 1 <= wav.numel() // FL <= self.k_max:
+            raise ValueError(f"slot {slot}: {wav.numel() // FL} frames, a push takes 1 .. {self.k_max}")
+
+    def _frames(self, wav) -> int:
+        return wav.numel() // self.dac.frame_length
+
+    def _describe(self, items: list, ks: list, nb: int, kb: int) -> torch.Tensor:
+        """(sequence, position) of every transformer row, then the slot of each stream and its valid rows per rate."""
+        scratch = self.slots
+        meta = []
+        for _, r in self._tfms:
+            n = kb * r
+            row_seq = [scratch] * (nb * n)
+            row_pos = [j for _ in range(nb) for j in range(n)]
+            for i, ((slot, _), k) in enumerate(zip(items, ks)):
+                p = self.pos[slot] * r
+                for j in range(k * r):
+                    row_seq[i * n + j], row_pos[i * n + j] = slot, p + j
+            meta += row_seq + row_pos
+        slot_of = [slot for slot, _ in items] + [-1] * (nb - len(items))
+        meta += slot_of
+        for r in self.rates:
+            meta += [k * r for k in ks] + [0] * (nb - len(items))
+        return torch.tensor(meta, dtype=torch.int32)
+
+    def _alloc_static(self, nb: int, kb: int, meta_h: torch.Tensor) -> tuple:
+        # zeros: the padding samples of a ragged push are never read into a valid row, but stay finite
+        return (torch.zeros(nb, kb * self.dac.frame_length, dtype=torch.float32, device=self.dac.device),
+                torch.empty(meta_h.numel(), dtype=torch.int32, device=self.dac.device))
+
+    @staticmethod
+    def _stage(st: tuple, items: list, ks: list, meta_h: torch.Tensor) -> None:
+        for i, (_, wav) in enumerate(items):
+            st[0][i, : wav.numel()].copy_(wav)
+        st[1].copy_(meta_h)
+
+    @staticmethod
+    def _outputs(codes: torch.Tensor, items: list, ks: list) -> dict:
+        return {slot: codes[i, :, :k].long() for i, ((slot, _), k) in enumerate(zip(items, ks))}
+
+    def _body(self, nb: int, kb: int, st: tuple, rope_len: int) -> torch.Tensor:
+        """The device work of one push (eager or under capture): waveform -> encoder -> quantizer downsample ->
+        pre_module -> residual VQ, each causal conv on a window of its slot's history + the new rows -> codes int32
+        [nb, n_stages, kb]. The layer walk is DAC._encode_one_shot's."""
+        dac, cfg = self.dac, self.dac.cfg
+        L, chk = dac.lib, _lib.check
+        FL, D = dac.frame_length, cfg.latent_dim
+        wav, meta = st
+        off, rows_at = 0, []
+        for _, r in self._tfms:
+            rows = nb * kb * r
+            rows_at.append((meta[off: off + rows], meta[off + rows: off + 2 * rows]))
+            off += 2 * rows
+        slot_t = meta[off: off + nb]
+        valid = {r: meta[off + nb * (1 + j): off + nb * (2 + j)] for j, r in enumerate(self.rates)}
+        window = self._windows(nb, slot_t, valid, "ep_win")
+        tfm_at = iter(range(len(self._tfms)))
+
+        def transformer(tf: dict, x: torch.Tensor, T: int) -> torch.Tensor:
+            ti = next(tfm_at)
+            return dac._transformer(tf, x, nb, T, "", kv_cache=self.kv_t[ti], cache_len=self.rings[ti],
+                                    rows_at=rows_at[ti], ring=True, rope_len=rope_len)
+
+        d0 = cfg.encoder_dim
+        Tc = kb * FL
+        win, H = window(wav, Tc // 4)
+        bufs = [dac._buf(f"ep_enc_{k}", nb * Tc * d0) for k in range(3)]
+        x, a, m = 0, 1, 2
+        r0 = dac.enc_blocks[0]["res"][0]
+        chk(L.fsb_first_conv_window(win.data_ptr(), dac.enc_in_w.data_ptr(), dac.enc_in_b.data_ptr(),
+                                    r0["s0"].alpha.data_ptr(), r0["s0"].inv.data_ptr(), nb, 4 * H + Tc, 4 * H, Tc, d0,
+                                    dac.enc_in_w.shape[1], bufs[x].data_ptr(), bufs[a].data_ptr(), _stream()))
+        c = d0
+        for bi, blk in enumerate(dac.enc_blocks):
+            for j, ru in enumerate(blk["res"]):
+                win, H = window(bufs[a], Tc)
+                self._gemm_win(ru["c7"], win, nb, H, Tc, c, out1=bufs[m], snake=ru["s1"])
+                nxt = blk["res"][j + 1]["s0"] if j < 2 else blk["s_out"]
+                dac._gemm(ru["c1"], bufs[m], nb, Tc, c, Tc, out0=bufs[x] if j < 2 else None, out1=bufs[a],
+                          snake=nxt, resid=bufs[x])
+            s, cout = blk["stride"], blk["dim"]
+            Tn = Tc // s
+            last = bi + 1 == len(dac.enc_blocks)
+            sn = dac.enc_out_snake if last else dac.enc_blocks[bi + 1]["res"][0]["s0"]
+            win, H = window(bufs[a], Tn)  # the [Tc / s][s * c] view
+            if blk["tfm"] is not None:
+                self._gemm_win(blk["down"], win, nb, H, Tn, s * c, out0=bufs[x])
+                n_out = transformer(blk["tfm"], bufs[x], Tn)
+                chk(L.fsb_snake(n_out.data_ptr(), sn.alpha.data_ptr(), sn.inv.data_ptr(), nb * Tn * cout, cout,
+                                bufs[a].data_ptr(), _stream()))
+                bufs[x][: nb * Tn * cout].copy_(n_out[: nb * Tn * cout])
+            else:
+                self._gemm_win(blk["down"], win, nb, H, Tn, s * c, out0=bufs[x], out1=bufs[m], snake=sn)
+                a, m = m, a
+            Tc, c = Tn, cout
+        win, H = window(bufs[a], Tc)
+        cur = dac._buf("ep_z", nb * Tc * D)
+        self._gemm_win(dac.enc_out, win, nb, H, Tc, c, out0=cur)
+        for i, dn in enumerate(dac.down):
+            f = dn["f"]
+            Tn = Tc // f
+            out = dac._buf(f"ep_down_{i}", nb * Tn * D)
+            dac._gemm(dn["conv"], cur, nb, Tn, f * D, Tn, out0=out)
+            cn = dn["cnx"]
+            win, H = window(out, Tn)
+            y = dac._buf("ep_cnx_y", nb * Tn * D)
+            h = dac._buf("ep_cnx_h", nb * Tn * 4 * D)
+            chk(L.fsb_dwconv_ln_window(win.data_ptr(), cn["dw"].data_ptr(), cn["dw_b"].data_ptr(), cn["ln_w"].data_ptr(),
+                                       cn["ln_b"].data_ptr(), nb, H + Tn, H, Tn, D, cn["k"], 1e-6, y.data_ptr(),
+                                       _stream()))
+            dac._gemm(cn["pw1"], y, nb, Tn, D, Tn, out0=h, act=1)
+            dac._gemm(cn["pw2"], h, nb, Tn, 4 * D, Tn, out0=out, gamma=cn["gamma"], resid=out)
+            cur, Tc = out, Tn
+        zq = transformer(dac.pre_tfm, cur, Tc)
+        # padding frames belong to no stream: quantise each stream's valid frames only
+        codes = torch.empty(nb, self.n_stage, Tc, dtype=torch.int32, device=dac.device)
+        chk(L.fsb_vq_encode_valid(zq.data_ptr(), dac.vq_in_w.data_ptr(), dac.vq_in_b.data_ptr(), dac.vq_cbn.data_ptr(),
+                                  dac.vq_cb_off.data_ptr(), dac.vq_sizes.data_ptr(), dac.vq_tab_ptrs.data_ptr(),
+                                  self.n_stage, cfg.codebook_dim, nb, Tc, D, valid[self._tfms[-1][1]].data_ptr(),
+                                  codes.data_ptr(), _stream()))
+        return codes
 
 
 class _SnakeView:

@@ -264,6 +264,12 @@ int fsb_final_conv_tanh(const void* d_a, const float* d_w, float bias, int B, in
 /* Encoder head: conv K taps 1->C on the fp32 waveform (modded_dac.py:683); raw and/or Snake'd output. */
 int fsb_first_conv(const float* d_wav, const float* d_w, const float* d_bias, const float* d_alpha,
                    const float* d_inv_alpha, int B, int T, int C, int K, void* d_raw, void* d_act, void* stream);
+/* fsb_first_conv over a stream window (EncodeStreamPool): output sample t of batch item b reads samples
+ * origin + t - (K-1) .. origin + t of d_wav [B][T_in] (fp32), so the origin samples before it are its carried history;
+ * outputs [B][T_out][C]. origin + T_out <= T_in; at least one of d_raw / d_act. */
+int fsb_first_conv_window(const float* d_wav, const float* d_w, const float* d_bias, const float* d_alpha,
+                          const float* d_inv_alpha, int B, int T_in, int origin, int T_out, int C, int K, void* d_raw,
+                          void* d_act, void* stream);
 int fsb_snake(const void* d_x, const float* d_alpha, const float* d_inv_alpha, long long n, int C, void* d_y,
               void* stream);
 /* One decoder ResidualUnit -- y = x + conv1(snake_1(conv7_dilated(a))), a = snake_0(x) -- as ONE kernel (dac
@@ -278,6 +284,11 @@ int fsb_res_unit(const void* d_a, const void* d_x, int B, int T, int C, int dila
 int fsb_vq_encode(const void* d_z, const float* d_in_w, const float* d_in_b, const float* d_cbn,
                   const int32_t* d_cb_off, const int32_t* d_sizes, const float* const* d_tabs, int S, int cd, int B,
                   int T, int D, int32_t* d_codes, void* stream);
+/* fsb_vq_encode of the first d_valid[b] frames of each batch item only (EncodeStreamPool: the frames after them are
+ * padding and may hold values that are not finite); the codes of the other frames are not written. */
+int fsb_vq_encode_valid(const void* d_z, const float* d_in_w, const float* d_in_b, const float* d_cbn,
+                        const int32_t* d_cb_off, const int32_t* d_sizes, const float* const* d_tabs, int S, int cd,
+                        int B, int T, int D, const int32_t* d_valid, int32_t* d_codes, void* stream);
 /* WindowLimitedTransformer glue (modded_dac.py:174-346) on fp32 GEMM results. */
 int fsb_resid_scale_norm(const float* d_y, int ld, const void* d_scale, const void* d_x_in, void* d_x_out,
                          const void* d_norm_w, void* d_n_out, int rows, int D, float eps, int round_bf16,
@@ -300,13 +311,19 @@ int fsb_qkv_rope_ring(const float* d_qkv, int rows, int H, int Hkv, int Dh, cons
 int fsb_window_attn_ring(const void* d_q, const void* d_k, const void* d_v, const int32_t* d_row_seq,
                          const int32_t* d_row_pos, int rows, int H, int Hkv, int Dh, int S, int window, int ring,
                          void* d_out, void* stream);
-/* Per-layer stream windows (DecodeStreamPool): a layer's input is viewed per stream as [H + n][row] with rows 0..H-1
+/* Per-layer stream windows (DecodeStreamPool, EncodeStreamPool): a layer's input is viewed per stream as [H + n][row] with rows 0..H-1
  * its carried causal history. fsb_window_fill writes win [nb][H + n][row]: rows 0..H-1 from state [slots][H][row] at
  * d_slot[i], rows H..H+d_valid[i]-1 from the producer's dense output [nb][n][row]; other rows are left as they are
  * (padding after the valid rows). fsb_window_roll writes the last H valid rows (window rows d_valid[i] ..
  * d_valid[i]+H-1) back to the slot's state. A negative slot skips the stream. row_bytes a multiple of 16. */
 int fsb_window_fill(const void* d_state, const void* d_dense, void* d_win, const int32_t* d_slot,
                     const int32_t* d_valid, int nb, int H, int n, int row_bytes, void* stream);
+/* fsb_window_fill that also zeroes every row it does not fill: the rows past a stream's valid rows, and all rows of a
+ * stream with a negative slot (EncodeStreamPool). Padding rows then never hold what the buffer held before, which may
+ * not be finite: the window attention multiplies a row's zero weights by the V rows of every run in its query tile, so
+ * a non-finite V in the scratch sequence would reach valid rows. */
+int fsb_window_fill_zero(const void* d_state, const void* d_dense, void* d_win, const int32_t* d_slot,
+                         const int32_t* d_valid, int nb, int H, int n, int row_bytes, void* stream);
 int fsb_window_roll(const void* d_win, void* d_state, const int32_t* d_slot, const int32_t* d_valid, int nb, int H,
                     int n, int row_bytes, void* stream);
 /* fsb_dwconv_ln over such a window: output row t = input row origin + t of x [B][T_in][C] (its history = the rows

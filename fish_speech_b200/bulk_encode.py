@@ -10,7 +10,10 @@ codes `[n_codebooks + 1, T]` (int64 in the reference; here too), files that alre
     throws away is not computed),
   * batches are formed from files of similar duration (sorted by length inside a window of the shard), so a padded
     batch wastes little compute, and capped by total padded seconds as well as by file count,
-  * a reader thread decodes and resamples the next batch while the GPU encodes the current one.
+  * a reader thread reads the next batches while the GPU encodes the current one. With a CUDA codec it only reads
+    (the raw frames of a PCM wav, the decoded array of any other file): conversion, down-mix, resampling to the
+    codec's rate and padding run on the device (fish_speech_b200.audio.load_batch); a codec on the CPU gets
+    converted, resampled waveforms as before.
 """
 from __future__ import annotations
 
@@ -25,6 +28,8 @@ from typing import Callable, Iterable, Optional, Sequence
 
 import numpy as np
 import torch
+
+from . import audio
 
 try:
     from loguru import logger
@@ -100,7 +105,18 @@ def resample(wav: torch.Tensor, sr: int, target: int) -> torch.Tensor:
 @dataclass
 class Clip:
     file: Path
-    wav: torch.Tensor  # [N] float32 at the codec's sample rate
+    wav: Optional[torch.Tensor]  # [N] float32 at the codec's sample rate (CPU codec)
+    pcm: Optional[audio.Pcm] = None  # the file as read, converted on the device (CUDA codec)
+    length: int = 0  # samples at the codec's sample rate
+
+    def __post_init__(self):
+        if self.wav is not None:
+            self.length = int(self.wav.numel())
+
+
+def _device_front_end(model) -> bool:
+    """Whether audio for `model` is converted and resampled on its device: a CUDA codec."""
+    return torch.device(model.device).type == "cuda"
 
 
 def plan_batches(lengths: Sequence[int], batch_size: int, max_padded_samples: int, window: int = 1024) -> list[list[int]]:
@@ -129,12 +145,15 @@ def encode_batch(clips: Sequence[Clip], model) -> float:
     if not clips:
         return 0.0
     device = model.device
-    lens = [int(c.wav.numel()) for c in clips]
-    audios = torch.zeros(len(clips), 1, max(lens), dtype=torch.float32)
-    for k, c in enumerate(clips):
-        audios[k, 0, : lens[k]] = c.wav
-    audios = audios.pin_memory().to(device, non_blocking=True) if torch.device(device).type == "cuda" else audios.to(device)
-    audio_lengths = torch.tensor(lens, device=device, dtype=torch.long)
+    lens = [c.length for c in clips]
+    if clips[0].pcm is not None:
+        audios, audio_lengths = audio.load_batch([c.pcm for c in clips], int(model.sample_rate), device)
+    else:
+        audios = torch.zeros(len(clips), 1, max(lens), dtype=torch.float32)
+        for k, c in enumerate(clips):
+            audios[k, 0, : lens[k]] = c.wav
+        audios = audios.pin_memory().to(device, non_blocking=True) if torch.device(device).type == "cuda" else audios.to(device)
+        audio_lengths = torch.tensor(lens, device=device, dtype=torch.long)
     indices, feature_lengths = model.encode(audios, audio_lengths)
     out = indices.cpu().numpy()
     for c, n, feat in zip(clips, feature_lengths.tolist(), out):
@@ -172,6 +191,16 @@ def batch_encode(model, audios_list: Sequence) -> list[torch.Tensor]:
     sample rate) -> one padded `model.encode` call -> per item its codes [n_codebooks, frames_i] on the host, padding
     frames cut off. (The reference runs this under fp16 autocast; the CUDA codec computes in bf16 / fp32 accumulate.)"""
     sr = int(model.sample_rate)
+    if not audios_list:
+        return []
+    device = model.device
+    if _device_front_end(model):
+        pcms = [audio.pcm_from_bytes(bytes(a)) if isinstance(a, (bytes, bytearray))
+                else audio.pcm_from_array(torch.as_tensor(a, dtype=torch.float32).reshape(-1), sr) for a in audios_list]
+        padded, lengths = audio.load_batch(pcms, sr, device)
+        features, feature_lengths = model.encode(padded, lengths)
+        features, feature_lengths = features.cpu(), feature_lengths.cpu()
+        return [f[..., : int(n)] for f, n in zip(features, feature_lengths)]
     audios = []
     for a in audios_list:
         if isinstance(a, (bytes, bytearray)):
@@ -179,9 +208,6 @@ def batch_encode(model, audios_list: Sequence) -> list[torch.Tensor]:
             audios.append(resample(wav, file_sr, sr)[None])
         else:
             audios.append(torch.as_tensor(a, dtype=torch.float32).reshape(1, -1))
-    if not audios:
-        return []
-    device = model.device
     lens = [int(x.shape[-1]) for x in audios]
     padded = torch.zeros(len(audios), 1, max(lens), dtype=torch.float32)
     for k, x in enumerate(audios):
@@ -195,11 +221,24 @@ def batch_encode(model, audios_list: Sequence) -> list[torch.Tensor]:
 def encode_files(files: Sequence[Path], model, batch_size: int = 64, max_batch_seconds: float = 1800.0,
                  reader: Callable[[Path], tuple[torch.Tensor, int]] = read_audio, prefetch: int = 2,
                  progress: Optional[Callable[[int, float], None]] = None) -> tuple[int, float]:
-    """Encode `files` with `model` (a DAC): a reader thread loads / down-mixes / resamples the clips of the next
-    batches while the current one is on the GPU. Unreadable files are logged and skipped, like the reference does
-    (extract_vq.py:97-104). Returns (files written, seconds of audio)."""
+    """Encode `files` with `model` (a DAC): a reader thread loads the clips of the next batches while the current one is
+    on the GPU. With a CUDA codec the reader only reads (`audio.read_pcm`, or `reader`'s waveform taken as it is) and
+    the device converts, down-mixes and resamples; otherwise the reader thread does that. Unreadable files are logged
+    and skipped, like the reference does (extract_vq.py:97-104). Returns (files written, seconds of audio)."""
     files = [Path(f) for f in files]
     sr = int(model.sample_rate)
+    on_device = _device_front_end(model)
+
+    def load(p: Path) -> Clip:
+        if not on_device:
+            wav, file_sr = reader(p)
+            return Clip(p, resample(wav.float().flatten(), file_sr, sr).contiguous())
+        if reader is read_audio:
+            pcm = audio.read_pcm(p)
+        else:
+            wav, file_sr = reader(p)
+            pcm = audio.pcm_from_array(wav.float().flatten(), file_sr)
+        return Clip(p, None, pcm, pcm.out_length(sr))
 
     def probe(p: Path) -> int:
         """Cheap length estimate for batch planning: file size (compressed formats sort roughly by duration too)."""
@@ -219,12 +258,11 @@ def encode_files(files: Sequence[Path], model, batch_size: int = 64, max_batch_s
                 clips: list[Clip] = []
                 for i in idxs:
                     try:
-                        wav, file_sr = reader(files[i])
-                        clips.append(Clip(files[i], resample(wav.float().flatten(), file_sr, sr).contiguous()))
+                        clips.append(load(files[i]))
                     except Exception as e:  # noqa: BLE001 - a bad file must not stop the shard
                         logger.error(f"Error reading {files[i]}: {e}")
                 # split again on true lengths if padding would exceed the cap
-                lens = [int(c.wav.numel()) for c in clips]
+                lens = [c.length for c in clips]
                 for sub in plan_batches(lens, batch_size, int(max_batch_seconds * sr)):
                     q.put([clips[j] for j in sub])
         finally:

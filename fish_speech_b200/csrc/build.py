@@ -8,7 +8,7 @@ from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 LIB = HERE.parent / "libfishb200.so"
-SOURCES = ["error.cu", "gemm_tc.cu", "lm_gemm.cu", "lm_kernels.cu", "attn_tile.cu", "lm_engine.cu", "codec_kernels.cu", "codec_resunit.cu", "api.cu"]
+SOURCES = ["error.cu", "gemm_tc.cu", "lm_gemm.cu", "lm_kernels.cu", "attn_tile.cu", "lm_engine.cu", "codec_kernels.cu", "codec_resunit.cu", "audio_kernels.cu", "api.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",

@@ -68,13 +68,14 @@ def main(argv=None):
         import soundfile as sf
         import torchaudio
 
+        from ...audio import resample
+
         model = load_model(config_name, checkpoint_path, device=device)
         if input_path.suffix in AUDIO_EXTENSIONS:
             audio, sr = torchaudio.load(str(input_path))
             if audio.shape[0] > 1:
                 audio = audio.mean(0, keepdim=True)
-            audio = torchaudio.functional.resample(audio, sr, model.sample_rate)
-            audios = audio[None].to(device)
+            audios = resample(audio.to(device), sr, model.sample_rate)[None]
             lengths = torch.tensor([audios.shape[2]], device=device, dtype=torch.long)
             indices, _ = model.encode(audios, lengths)
             if indices.ndim == 3:

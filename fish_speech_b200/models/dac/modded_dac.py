@@ -21,11 +21,12 @@ import ctypes as C
 import math
 import threading
 from dataclasses import dataclass, field
-from typing import Iterator, Optional
+from types import MappingProxyType
+from typing import Iterator, Mapping, Optional
 
 import torch
 
-from ... import _lib
+from ... import _lib, audio
 
 
 @dataclass
@@ -681,6 +682,7 @@ class DAC:
         """Streaming `encode` of up to `slots` independent streams at once: streams join and leave at any push, and one
         push encodes the new frames of every stream that has some in one batched (graph-replayed) pass, in memory that
         does not grow with a stream's length. Each stream's codes are bit-identical to `encode` of its waveform alone.
+        A stream opened with `open(sample_rate=sr)` takes audio at `sr` in pieces of any length and ends with `flush`.
         See EncodeStreamPool."""
         return EncodeStreamPool(self, slots, k_max, n_quantizers, max_graphs)
 
@@ -1161,6 +1163,13 @@ class EncodeStreamPool(_StreamPool):
     * transformers: the encoder's (window 512 at 4 rows per frame) and `pre_module` (window 128 at 1 row per frame)
       keep their K/V in rings of R = round_up(window + rows per frame * k_max + 63, 64) positions per slot and layer
       (fsb_qkv_rope_ring / fsb_window_attn_ring), at absolute positions that grow without bound.
+    * streams at other sample rates: a slot opened with `open(sample_rate=sr)` takes pieces of any length at `sr` (1-D
+      float32, or int16 PCM), and `flush(slot)` ends the stream. Each push resamples the new samples eagerly, before
+      the frame pass (fish_speech_b200.audio.StreamResampler, every such slot of the push in one launch), into a
+      per-slot carry of fewer than frame_length samples at the codec's rate; the whole frames go through the pass
+      below (in rounds of at most k_max frames) and the push returns every frame completed so far, possibly none.
+      `flush` pads the last partial frame with zeros, as `encode` pads. The codes are bit-identical to `encode` of the
+      whole clip resampled by `audio.resample`.
     * ragged pushes, padding rows, the scratch sequence, graph capture and failed pushes as in DecodeStreamPool, except
       that every window's padding rows are zeroed (fsb_window_fill_zero). The shared window buffer holds other layers'
       rows before (the waveform window's fp32 samples read as bf16 can be Inf or NaN), and the tiled window attention
@@ -1169,12 +1178,15 @@ class EncodeStreamPool(_StreamPool):
     """
 
     _fill = "fsb_window_fill_zero"
+    _rs: Mapping = MappingProxyType({})  # replaced per pool; no slot has a rate in a pool built without __init__
 
     def __init__(self, dac: "DAC", slots: int, k_max: int, n_quantizers: Optional[int], max_graphs: int):
         if slots < 1 or k_max < 1:
             raise ValueError(f"stream pool needs slots >= 1 and k_max >= 1 (got {slots}, {k_max})")
         cfg, FL = dac.cfg, dac.frame_length
         self.dac = dac
+        self._rs = {}     # slot -> StreamResampler, for the streams opened with a sample rate
+        self._carry = {}  # slot -> their fp32 samples at the codec's rate not yet in a frame (< frame_length)
         self.n_stage = dac.n_stage if n_quantizers is None else min(dac.n_stage, 1 + int(n_quantizers))
         # the transformers in execution order, with their rows per frame; slot `slots` is the scratch sequence
         tfms, r = [], FL
@@ -1234,6 +1246,112 @@ class EncodeStreamPool(_StreamPool):
 
     def _frames(self, wav) -> int:
         return wav.numel() // self.dac.frame_length
+
+    def open(self, sample_rate: Optional[int] = None) -> int:
+        """A new stream's slot. Without `sample_rate`, its pushes take whole frames of fp32 audio at the codec's rate;
+        with it, pieces of any length at `sample_rate` (1-D float32, or int16 PCM), ended by `flush`."""
+        if sample_rate is not None and int(sample_rate) <= 0:
+            raise ValueError(f"sample_rate must be positive (got {sample_rate})")
+        with self.dac._lock, torch.cuda.device(self.dac.device):
+            slot = super().open()
+            if sample_rate is not None:
+                self._rs[slot] = audio.StreamResampler(int(sample_rate), self.dac.sample_rate, self.dac.device)
+                self._carry[slot] = torch.empty(0, dtype=torch.float32, device=self.dac.device)
+            return slot
+
+    def close(self, slot: int) -> None:
+        with self.dac._lock:
+            super().close(slot)
+            if slot in self._rs:
+                del self._rs[slot], self._carry[slot]
+
+    def push(self, pieces: dict) -> dict:
+        """{slot: piece} -> {slot: codes int64 [n_stages, k]}. A slot opened without a sample rate takes 1 .. k_max
+        whole frames and gets their k codes; a slot opened with one takes any piece and gets the codes of the frames
+        it completed (k >= 0)."""
+        if not any(s in self._rs for s in pieces):
+            return super().push(pieces)
+        for slot, piece in pieces.items():
+            self._check_slot(slot)
+            if self.broken[slot]:
+                raise ValueError(f"slot {slot}: an earlier push failed, its state is lost; close the slot")
+            if slot not in self._rs:
+                self._check_piece(slot, piece)
+            else:
+                self._check_rated_piece(slot, piece)
+        with self.dac._lock, torch.cuda.device(self.dac.device):
+            try:
+                frames = self._resample_to_frames({s: p for s, p in pieces.items() if s in self._rs})
+                frames.update({s: p for s, p in pieces.items() if s not in self._rs})
+                return self._push_frames(frames)
+            except BaseException:
+                for slot in pieces:
+                    self.broken[slot] = True
+                raise
+
+    def flush(self, slot: int) -> torch.Tensor:
+        """End the stream of a slot opened with a sample rate: the rest of its samples, the last partial frame
+        zero-padded as `encode` pads it -> codes int64 [n_stages, k] (k >= 0). The slot then takes no more pushes
+        until it is closed and opened again. A slot opened without a rate has nothing pending: [n_stages, 0]."""
+        self._check_slot(slot)
+        if self.broken[slot]:
+            raise ValueError(f"slot {slot}: an earlier push failed, its state is lost; close the slot")
+        if slot not in self._rs:
+            return torch.empty(self.n_stage, 0, dtype=torch.int64, device=self.dac.device)
+        if self._rs[slot].counts.done:
+            raise ValueError(f"slot {slot}: the stream was already flushed")
+        with self.dac._lock, torch.cuda.device(self.dac.device):
+            try:
+                return self._push_frames(self._resample_to_frames({slot: None}))[slot]
+            except BaseException:
+                self.broken[slot] = True
+                raise
+
+    def _check_rated_piece(self, slot: int, piece) -> None:
+        if not isinstance(piece, torch.Tensor) or piece.ndim != 1 or piece.dtype not in (torch.float32, torch.int16):
+            raise ValueError(f"slot {slot}: a piece must be a 1-D float32 waveform or int16 PCM")
+        if self._rs[slot].counts.done:
+            raise ValueError(f"slot {slot}: the stream was flushed")
+
+    def _resample_to_frames(self, pieces: dict) -> dict:
+        """{slot: piece at the slot's rate, or None to flush} -> {slot: the whole frames now complete at the codec's
+        rate, fp32 [k * frame_length]}; the rest stays in the slot's carry."""
+        FL, dev = self.dac.frame_length, self.dac.device
+        todo = []
+        for slot, piece in pieces.items():
+            x = None
+            if piece is not None:
+                x = piece.to(dev)
+                if x.dtype == torch.int16:
+                    x = audio.pcm_to_mono(x, audio.PCM_S16)
+            todo.append((self._rs[slot], x))
+        frames = {}
+        for (slot, piece), y in zip(pieces.items(), audio.StreamResampler.push_many(todo)):
+            c = torch.cat((self._carry[slot], y))
+            if piece is None:
+                c = torch.nn.functional.pad(c, (0, -c.numel() % FL))  # encode's right pad
+            k = c.numel() // FL
+            frames[slot], self._carry[slot] = c[: k * FL], c[k * FL:]
+        return frames
+
+    def _push_frames(self, frames: dict) -> dict:
+        """{slot: fp32 [k * frame_length], any k >= 0} -> {slot: codes [n_stages, k]}: pushes of at most k_max frames."""
+        FL = self.dac.frame_length
+        out = {s: [] for s in frames}
+        done = dict.fromkeys(frames, 0)
+        while True:
+            rnd = {}
+            for s, f in frames.items():
+                k = min(self.k_max, f.numel() // FL - done[s])
+                if k > 0:
+                    rnd[s] = f[done[s] * FL: (done[s] + k) * FL]
+                    done[s] += k
+            if not rnd:
+                break
+            for s, c in super().push(rnd).items():
+                out[s].append(c)
+        return {s: torch.cat(v, dim=1) if v else torch.empty(self.n_stage, 0, dtype=torch.int64, device=self.dac.device)
+                for s, v in out.items()}
 
     def _describe(self, items: list, ks: list, nb: int, kb: int) -> torch.Tensor:
         """(sequence, position) of every transformer row, then the slot of each stream and its valid rows per rate."""

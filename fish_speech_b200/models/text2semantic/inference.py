@@ -272,10 +272,12 @@ def load_codec_model(codec_checkpoint_path, device, precision=torch.bfloat16):
 def encode_audio(audio_path, codec, device):
     import torchaudio
 
+    from ...audio import resample
+
     wav, sr = torchaudio.load(str(audio_path))
     if wav.shape[0] > 1:
         wav = wav.mean(dim=0, keepdim=True)
-    wav = torchaudio.functional.resample(wav.to(device), sr, codec.sample_rate)[0]
+    wav = resample(wav.to(device), sr, codec.sample_rate)[0]  # on a CUDA device: the codec front end's kernel
     audios = wav[None, None]
     audio_lengths = torch.tensor([len(wav)], device=device, dtype=torch.long)
     indices, feature_lengths = codec.encode(audios, audio_lengths)

@@ -333,6 +333,51 @@ int fsb_dwconv_ln_window(const void* d_x, const float* d_w, const float* d_bias,
                          void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Codec input front end (csrc/audio_kernels.cu): PCM at any sample rate -> the codec's mono fp32 input on the device.
+ *   replaces the numpy conversion + down-mix and torchaudio.functional.resample of the readers feeding DAC.encode
+ *   (tools/vqgan/extract_vq.py:108, fish_speech/models/text2semantic/inference.py:428).
+ * Descriptors are arrays in device memory, one per clip; a launch covers many clips (blockIdx.y = clip).
+ * ---------------------------------------------------------------------------------------------- */
+#define FSB_PCM_S16 0 /* little-endian int16:  x / 32768 */
+#define FSB_PCM_S32 1 /* little-endian int32:  x / 2147483648 */
+#define FSB_PCM_U8 2  /* unsigned 8-bit:       (x - 128) / 128 */
+#define FSB_PCM_F32 3 /* float32 as is */
+
+typedef struct {
+    long long src_off;  /* byte offset of the clip's first frame in d_src (any alignment) */
+    long long frames;   /* frames of `channels` interleaved samples */
+    long long channels;
+    long long format;   /* FSB_PCM_* */
+    long long dst_off;  /* element offset of the clip's mono output in d_dst */
+} fsb_pcm_clip;
+
+/* Mono fp32 of each clip: per frame the channel values (converted in fp32 as above) summed in order from 0.f, then
+ * divided by the channel count -- bit-identical to numpy's `x.astype(float32) / scale` and `.mean(axis=1)`.
+ * max_frames >= every clip's frames. */
+int fsb_pcm_to_mono(const void* d_src, const fsb_pcm_clip* d_clips, int B, long long max_frames, float* d_dst,
+                    void* stream);
+
+typedef struct {
+    long long x_off;    /* element offset in d_x of input sample x_start of the clip */
+    long long x_start;  /* d_x holds the clip's samples [x_start, x_end) from x_off on; samples < 0 or >= x_end are 0 */
+    long long x_end;
+    long long j0;       /* first output (absolute index in the clip's output) to compute */
+    long long out_off;  /* element offset in d_out of output j0 */
+    long long n_out;    /* outputs computed: j0 .. j0 + n_out - 1 */
+    long long n_fill;   /* elements written from out_off: the n_out outputs, then zeros (>= n_out) */
+    const float* w;     /* fp32 [taps][new_rate]: the non-zero taps of each phase; NULL = orig == new (a copy) */
+    const int32_t* span;/* int32 [new_rate][2]: phase p's first input offset from q * orig, and its tap count */
+    long long orig, new_rate; /* the two rates divided by their gcd */
+} fsb_resample_clip;
+
+/* torchaudio.functional.resample(x, orig, new) with its defaults (sinc_interp_hann, lowpass_filter_width 6,
+ * rolloff 0.99): output j = q * new + p is sum_m w[m][p] * x(q * orig + span[p][0] + m), m ascending over span[p][1]
+ * taps, fp64 fma from 0.0, rounded to fp32 once. The table is built by fish_speech_b200/audio.py. An output's bits depend only on the
+ * samples it reads, so a batch, a clip alone and a stream window that holds those samples agree bitwise. */
+int fsb_resample(const float* d_x, const fsb_resample_clip* d_clips, int B, long long max_fill, float* d_out,
+                 void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Unit-test hooks (used by tests/ only)
  * ---------------------------------------------------------------------------------------------- */
 /* out[j][i] (fp32, ld = m) = sum_k A[i][k] * B[j][k]; A [m,k], B [n,k] bf16 row-major, by the prefill / codec GEMM

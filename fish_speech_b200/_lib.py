@@ -82,6 +82,8 @@ def lib() -> C.CDLL:
     L.fsb_lm_slot_blob_bytes.restype = C.c_size_t
     L.fsb_lm_slot_save.argtypes = [vp, i32, vp, vp]
     L.fsb_lm_slot_restore.argtypes = [vp, i32, vp, vp]
+    # named buffers (include/fishb200.h), among them "kv_miss" int32 [max_batch]: 0, or 1 + the position at which a
+    # slot's live decode row met an unmapped KV page (engine.LmEngine.buffer gives each its shape)
     L.fsb_lm_buffer.argtypes = [vp, C.c_char_p, C.POINTER(vp), C.POINTER(C.c_size_t)]
     L.fsb_lm_set_sampler_noise.argtypes = [vp, vp, i32, i32]
     L.fsb_lm_copy_kv.argtypes = [vp, i32, i32, i32, vp]

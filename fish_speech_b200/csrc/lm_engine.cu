@@ -102,6 +102,7 @@ struct fsb_lm {
     // state
     int *cur_tok = nullptr, *out_tokens = nullptr, *n_out = nullptr, *pos = nullptr, *finished = nullptr;
     int *ras_window = nullptr, *iota = nullptr, *fpos = nullptr;
+    int* kv_miss = nullptr;  // per slot: 0, or 1 + the position at which decode attention first met an unmapped page
     unsigned long long* step = nullptr;
     // debug / test hooks
     float *slow_logits = nullptr, *fast_logits = nullptr;
@@ -241,9 +242,10 @@ int launch_decode_attn(const fsb_lm* h, const Stack& s, int l, const StepGemmPla
     AttnDecodeArgs aa = decode_attn_args(h, s, l, qkv, rows, row_seq, row_pos, kv_only);
     const int span = h->cfg.attn_split;
     const int bound = h->ctx_lcap > 0 ? h->ctx_lcap : s.S;
-    if (span <= 0 || s.bf16_math != 0 || bound <= span) return launch_attn_decode(aa, st);
+    int* kv_miss = s.kv_page ? h->kv_miss : nullptr;  // the paged slow stack only: the fast stack's cache is contiguous
+    if (span <= 0 || s.bf16_math != 0 || bound <= span) return launch_attn_decode(aa, st, kv_miss);
     aa.lcap = span;
-    return launch_attn_decode_split(aa, AttnSplit{h->q_d, h->span_ws, span, bound}, st);
+    return launch_attn_decode_split(aa, AttnSplit{h->q_d, h->span_ws, span, bound}, st, kv_miss);
 }
 
 // The first `upto` (GEMM, finalize) pairs of a layer after its attention: wo + residual add, w1|w3 + SwiGLU,
@@ -617,6 +619,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &h->slot_top_p, cfg->max_batch, "slot_top_p"));
     TRYC(dalloc(h, &h->slot_top_k, cfg->max_batch, "slot_top_k"));
     TRYC(dalloc(h, &h->slot_seed, cfg->max_batch, "slot_seed"));
+    TRYC(dalloc(h, &h->kv_miss, cfg->max_batch, "kv_miss"));
     TRYC(dalloc(h, &h->iota, RT));
     TRYC(dalloc(h, &h->fpos, static_cast<size_t>(C) * RT));
     TRYC(dalloc(h, &h->step, 1, "step"));

@@ -577,7 +577,8 @@ __global__ void __launch_bounds__(kAttnThreads) attn_kernel(AttnArgs a, float sc
 // SPLIT (attn_decode_split_kernel): a row of more than sp.span positions stops after the front end, its finished q heads
 // stored to sp.q for attn_span_kernel; every other row runs the code of SPLIT = false.
 template <int DH, int G, bool SPLIT>
-__device__ __forceinline__ void attn_decode_body(const AttnDecodeArgs a, const float scale, const int lcap, const AttnSplit sp) {
+__device__ __forceinline__ void attn_decode_body(const AttnDecodeArgs a, const float scale, const int lcap, const AttnSplit sp,
+                                                 int* kv_miss) {
     pdl_launch_dependents();
     const int row = blockIdx.y, g = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -655,7 +656,13 @@ __device__ __forceinline__ void attn_decode_body(const AttnDecodeArgs a, const f
         pt[j] = j < npre ? pg_pre : (ptab ? ptab[j] : j);  // j < npre: j == threadIdx.x
         unmapped |= pt[j] < 0;
     }
-    if (__syncthreads_or(unmapped)) return;  // unmapped history: nothing is written, nothing attended
+    if (__syncthreads_or(unmapped)) {  // unmapped history: nothing is written, nothing attended, the miss recorded
+        if (kv_miss != nullptr && g == 0 && threadIdx.x == 0) {
+            int* miss = kv_miss + a.row_seq[row];
+            if (*miss == 0) *miss = rpos + 1;
+        }
+        return;
+    }
     const bool split_row = SPLIT && wpos + 1 > sp.span;
     // (cos, sin) of this lane's rotary pair at the row's position: the same for q and k
     const uint32_t cs = *reinterpret_cast<const uint32_t*>(a.freqs + (static_cast<size_t>(wpos) * (DH / 2) + (d >> 1)) * 2);
@@ -718,14 +725,15 @@ __device__ __forceinline__ void attn_decode_body(const AttnDecodeArgs a, const f
 }
 
 template <int DH, int G>
-__global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArgs a, float scale, int lcap) {
-    attn_decode_body<DH, G, false>(a, scale, lcap, AttnSplit{});
+__global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(AttnDecodeArgs a, float scale, int lcap,
+                                                                   int* kv_miss) {
+    attn_decode_body<DH, G, false>(a, scale, lcap, AttnSplit{}, kv_miss);
 }
 
 template <int DH, int G>
 __global__ void __launch_bounds__(kAttnThreads) attn_decode_split_kernel(AttnDecodeArgs a, AttnSplit sp, float scale,
-                                                                         int lcap) {
-    attn_decode_body<DH, G, true>(a, scale, lcap, sp);
+                                                                         int lcap, int* kv_miss) {
+    attn_decode_body<DH, G, true>(a, scale, lcap, sp, kv_miss);
 }
 
 // A long row's page-table walk, shared by attn_span_kernel and attn_combine_kernel so that both take the same
@@ -1379,23 +1387,23 @@ int attn_init() {
 }
 
 template <int DH, int G>
-static int launch_attn_decode_t(const AttnDecodeArgs& a, cudaStream_t st) {
+static int launch_attn_decode_t(const AttnDecodeArgs& a, cudaStream_t st, int* kv_miss) {
     int lcap = a.S;
     if (a.lcap > 0 && a.lcap < lcap) lcap = a.lcap;
     const int pages = cdiv(a.S, kKvPage);  // page-table entries of one row (the identity when contiguous)
     lcap = attn_score_chunk<DH, G>(lcap, pages);
     const size_t smem = attn_smem_bytes<DH, G>(lcap, pages);
     const float scale = 1.0f / sqrtf(static_cast<float>(DH));
-    FSB_LAUNCH((attn_decode_kernel<DH, G>), dim3(a.Hkv, a.rows), dim3(kAttnThreads), smem, st, a, scale, lcap);
+    FSB_LAUNCH((attn_decode_kernel<DH, G>), dim3(a.Hkv, a.rows), dim3(kAttnThreads), smem, st, a, scale, lcap, kv_miss);
     return 0;
 }
 
-int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st) {
+int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st, int* kv_miss) {
     if (a.rows <= 0) return 0;
     const int G = a.H / a.Hkv;
     FSB_CHECK(a.H % a.Hkv == 0, "attention: H %% Hkv != 0");
 #define FSB_ATTN_CASE(DH_, G_) \
-    if (a.Dh == DH_ && G == G_) return launch_attn_decode_t<DH_, G_>(a, st);
+    if (a.Dh == DH_ && G == G_) return launch_attn_decode_t<DH_, G_>(a, st, kv_miss);
     FSB_ATTN_CASE(128, 1) FSB_ATTN_CASE(128, 2) FSB_ATTN_CASE(128, 4) FSB_ATTN_CASE(128, 8)
     FSB_ATTN_CASE(64, 1) FSB_ATTN_CASE(64, 2) FSB_ATTN_CASE(64, 4) FSB_ATTN_CASE(64, 8)
 #undef FSB_ATTN_CASE
@@ -1410,14 +1418,14 @@ static size_t attn_span_smem_bytes(int span) {
 }
 
 template <int DH, int G>
-static int launch_attn_decode_split_t(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st) {
+static int launch_attn_decode_split_t(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st, int* kv_miss) {
     int lcap = a.S;
     if (a.lcap > 0 && a.lcap < lcap) lcap = a.lcap;
     const int pages = cdiv(a.S, kKvPage);
     lcap = attn_score_chunk<DH, G>(lcap, pages);
     const float scale = 1.0f / sqrtf(static_cast<float>(DH));
     FSB_LAUNCH((attn_decode_split_kernel<DH, G>), dim3(a.Hkv, a.rows), dim3(kAttnThreads),
-               (attn_smem_bytes<DH, G>(lcap, pages)), st, a, sp, scale, lcap);
+               (attn_smem_bytes<DH, G>(lcap, pages)), st, a, sp, scale, lcap, kv_miss);
     if (a.kv_only) return 0;
     FSB_LAUNCH((attn_span_kernel<DH, G>), dim3(a.Hkv, a.rows, cdiv(sp.bound, sp.span)), dim3(kAttnThreads),
                (attn_span_smem_bytes<DH, G>(sp.span)), st, a, sp, scale);
@@ -1438,7 +1446,7 @@ int attn_split_max_span(int H, int Hkv, int Dh) {
     return 0;
 }
 
-int launch_attn_decode_split(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st) {
+int launch_attn_decode_split(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st, int* kv_miss) {
     if (a.rows <= 0) return 0;
     const int G = a.H / a.Hkv;
     FSB_CHECK(a.H % a.Hkv == 0, "attention: H %% Hkv != 0");
@@ -1448,7 +1456,7 @@ int launch_attn_decode_split(const AttnDecodeArgs& a, const AttnSplit& sp, cudaS
               attn_split_max_span(a.H, a.Hkv, a.Dh));
     FSB_CHECK(sp.bound > 0 && cdiv(sp.bound, sp.span) <= 65535, "attention: %d spans", cdiv(sp.bound, sp.span));
 #define FSB_ATTN_CASE(DH_, G_) \
-    if (a.Dh == DH_ && G == G_) return launch_attn_decode_split_t<DH_, G_>(a, sp, st);
+    if (a.Dh == DH_ && G == G_) return launch_attn_decode_split_t<DH_, G_>(a, sp, st, kv_miss);
     FSB_ATTN_CASE(128, 1) FSB_ATTN_CASE(128, 2) FSB_ATTN_CASE(128, 4) FSB_ATTN_CASE(128, 8)
     FSB_ATTN_CASE(64, 1) FSB_ATTN_CASE(64, 2) FSB_ATTN_CASE(64, 4) FSB_ATTN_CASE(64, 8)
 #undef FSB_ATTN_CASE

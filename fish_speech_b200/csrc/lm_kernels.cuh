@@ -155,7 +155,11 @@ struct AttnDecodeArgs {
     int kv_only;
     float eps;
 };
-int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st);
+// kv_miss: per sequence (row_seq) or null. A row with pos >= 0 that meets an unmapped page stores 1 + pos there if the
+// entry is still 0 (the CTA of KV group 0), so that the host learns that the row's attention and the tokens sampled
+// from it are void. A kernel argument of its own, not a field of AttnDecodeArgs: the span and combine kernels take
+// that struct and do not need it.
+int launch_attn_decode(const AttnDecodeArgs& a, cudaStream_t st, int* kv_miss = nullptr);
 
 // The same attention with the history of a LONG row -- more than `span` positions -- split over several CTAs, so that
 // one long context does not set the time of the whole launch. Three kernels instead of one:
@@ -179,7 +183,7 @@ constexpr int attn_span_floats(int G, int Dh) { return G * (Dh + 2); }
 // the longest span attn_span_kernel can hold in shared memory for this geometry (0: unsupported geometry)
 int attn_split_max_span(int H, int Hkv, int Dh);
 // a.lcap is the base kernel's score bound as for launch_attn_decode; the caller caps it at sp.span
-int launch_attn_decode_split(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st);
+int launch_attn_decode_split(const AttnDecodeArgs& a, const AttnSplit& sp, cudaStream_t st, int* kv_miss = nullptr);
 
 // h = rbf( rbf(silu(rbf(a))) * rbf(c) ): a = w1 feature i, c = w3 feature i of the fused GEMM result.
 // interleaved = 0: a = y[i], c = y[I + i];  1: the step-GEMM row order (w13_gate_row in lm_gemm.cuh)

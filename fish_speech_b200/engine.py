@@ -108,6 +108,12 @@ class KvPagePool:
         pages = np.concatenate([self.table[live].ravel(), *self.detached])
         return self.n_pages - len(np.unique(pages[pages >= 0]))
 
+    def row_pages(self, row: np.ndarray) -> tuple[int, int]:
+        """(pages `row` maps, pages no other row maps) of a slot's row (`table[slot]`) or a detached one: what a
+        request holds, and what it gives back to `available()` once it is retired or dropped."""
+        pages = row[row >= 0]
+        return len(pages), int(np.count_nonzero(self.ref[pages] == 1))
+
     # ---- mapping ------------------------------------------------------------------------------------------------
     def _unmap(self, slot: int, first: int):
         """Unmap pages first.. of `slot` (a row never maps one page twice)."""
@@ -390,6 +396,7 @@ class LmEngine:
             "slot_top_p": ((self.max_batch,), "<f4"),
             "slot_top_k": ((self.max_batch,), "<i4"),
             "slot_seed": ((self.max_batch,), "<i8"),
+            "kv_miss": ((self.max_batch,), "<i4"),
             "kv_page": ((self.max_batch, self.kv_pool.pages_per_slot), "<i4"),
             "slow_logits": ((self.max_batch, self.head_rows), "<f4"),
             "fast_logits": ((c.num_codebooks, self.max_batch, c.codebook_size), "<f4"),
@@ -497,6 +504,12 @@ class LmEngine:
         n_positions = min(int(n_positions), self.kv_len)
         self._reserve([(slot, n_positions, start)])
         self._wfrom[int(slot)] = int(start)
+
+    def grow_kv(self, ends: dict):
+        """ends: {slot: end} -- map pages for positions [covered end, end) of each live slot, which has written nothing
+        past what its pages cover; one page-table upload for all of them. Only retired rows are reclaimed."""
+        self._reserve([(int(s), int(e), self._covered.get(int(s), 0) * KV_PAGE) for s, e in ends.items()
+                       if kv_pages_for(e) > self._covered.get(int(s), 0)])
 
     def retire_slot(self, slot: int):
         """The slot's request is done: its pages stay mapped as a reusable prefix until the pool needs them."""

@@ -510,13 +510,16 @@ def serve_requests(model, input_queue: "queue.Queue", max_slots: int, frames_per
     FSB_SERVE_LIVE=n (n > max_slots) lets up to n requests be live at a time: streaming requests
     (`stream_frames`) are then paced at playback speed, one playback clock per request across its chunks, so
     that the scheduler parks the ones far ahead of their listener and gives their slots to the ones about to run
-    dry. A request dict may carry `cancel` (a threading.Event): once it is set the request in flight is taken out
+    dry. FSB_SERVE_KV_GROW=1 (with FSB_SERVE_KV_GB) lets requests take KV pages as they decode instead of reserving
+    prompt + budget at admission (ContinuousBatcher kv_growth). A request dict may carry `cancel` (a threading.Event): once it is set the request in flight is taken out
     of the scheduler, the plan ends and nothing more is put on its response queue."""
     from ...scheduler import Cancelled, ContinuousBatcher, SlotRequest, StreamClock
 
     if batcher is None:
         max_live = max(max_slots, int(os.environ.get("FSB_SERVE_LIVE", "0") or 0))
-        batcher = ContinuousBatcher(model, max_slots=max_slots, frames_per_poll=frames_per_poll, max_live=max_live)
+        grow = serve_kv_grow(os.environ.get("FSB_SERVE_KV_GROW"), os.environ.get("FSB_SERVE_KV_GB"))
+        batcher = ContinuousBatcher(model, max_slots=max_slots, frames_per_poll=frames_per_poll, max_live=max_live,
+                                    kv_growth=grow)
     paced = getattr(batcher, "max_live", 0) > getattr(batcher, "max_slots", 0)
     live = 0  # plans not yet exhausted
     waiting_queues: dict = {}  # id(plan) -> response queue of every plan that has a generate call in flight
@@ -677,6 +680,20 @@ def serve_attn_split(value: Optional[str]) -> int:
     return n
 
 
+def serve_kv_grow(value: Optional[str], kv_gb: Optional[str]) -> bool:
+    """FSB_SERVE_KV_GROW: 1 = requests take KV pages as they decode (ContinuousBatcher kv_growth); unset, empty or 0
+    = prompt + budget reserved at admission. Growth needs the bounded pool of FSB_SERVE_KV_GB: a ValueError naming
+    both variables without it, and one naming FSB_SERVE_KV_GROW for any other value."""
+    if value is None or value.strip() in ("", "0"):
+        return False
+    if value.strip() != "1":
+        raise ValueError(f"FSB_SERVE_KV_GROW={value!r} must be 0 or 1")
+    if not kv_gb:
+        raise ValueError("FSB_SERVE_KV_GROW=1 needs FSB_SERVE_KV_GB: growth shares a bounded KV page pool, and without "
+                         "FSB_SERVE_KV_GB every slot has its full capacity reserved")
+    return True
+
+
 def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool = False):
     """inference.py:736-799: the model lives in ONE daemon worker thread fed by a queue; `None` shuts
     it down; errors are returned as WrappedGenerateResponse(status="error", response=exc).
@@ -690,7 +707,10 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
     its pages fit; a pool that does not fit in free device memory raises a ValueError naming FSB_SERVE_KV_GB.
     FSB_ATTN_SPLIT=p (a multiple of 64; 0 or unset = off) makes a decode row whose context is longer than p positions
     split its attention into spans of p positions over several CTAs, so that one long conversation does not slow the
-    frames of every slot; requests that stay at or below p keep their bits, longer ones change in the last places."""
+    frames of every slot; requests that stay at or below p keep their bits, longer ones change in the last places.
+    FSB_SERVE_KV_GROW=1 (needs FSB_SERVE_KV_GB; else a ValueError naming both) maps a request's prompt and first frames
+    at admission and further pages as it decodes; a request that cannot get its next page safely waits parked."""
+    serve_kv_grow(os.environ.get("FSB_SERVE_KV_GROW"), os.environ.get("FSB_SERVE_KV_GB"))
     input_queue = queue.Queue()
     init_event = threading.Event()
     init_error: list = []

@@ -69,6 +69,10 @@ class SlotRequest:
     _parked: object = None  # engine.ParkedSlot while the request is live without a slot
     parks: int = 0
     resumes: int = 0
+    # KV growth (ContinuousBatcher kv_growth): times it waited parked for pages, and its longest such wait (seconds)
+    page_parks: int = 0
+    page_wait: float = 0.0
+    _short_since: float = 0.0
 
     def lead(self, now: float) -> float:
         """Frames the consumer holds beyond what it has played at `now` (negative: it is waiting for frames). An
@@ -131,15 +135,32 @@ def schedule_live(running: Sequence[SlotRequest], parked: Sequence[SlotRequest],
     return LivePlan(park, resume, admit, rest)
 
 
+def kv_safe(avail: int, claims) -> bool:
+    """Banker's rule over one resource, KV pages. `claims`: (need, alone) of every admitted request -- the pages it
+    may still take before it ends, and the pages only its row maps now. Safe when the requests can be ordered so that
+    each one's need fits in `avail` plus what those before it give back: a request that runs to its end takes its
+    need and then returns it together with `alone`, a net gain of `alone`. Smallest need first finds such an order
+    when one exists. A page shared with another row is not counted as returned, so a state called safe is safe."""
+    for need, alone in sorted(claims, key=lambda c: (c[0], -c[1])):
+        if need > avail:
+            return False
+        avail += alone
+    return True
+
+
 class ContinuousBatcher:
     def __init__(self, model, max_slots: int = 32, frames_per_poll: int = 8, min_free_to_admit: int = 1,
-                 max_live: Optional[int] = None, clock: Callable[[], float] = time.monotonic):
+                 max_live: Optional[int] = None, clock: Callable[[], float] = time.monotonic, kv_growth: bool = False):
         """`frames_per_poll`: decode frames between two looks at the device-side slot states (a finished slot
         idles for at most that many frames). `min_free_to_admit`: admissions wait until that many slots are
         free (or nothing is running) — every admission is one extra prefill pass + first frame that streams
         all weights for the new rows only, so grouping them trades admission latency for throughput.
         `max_live`: the most requests admitted at a time, running plus parked; the default, `max_slots`, means
-        nothing is ever parked. `clock`: the time source of the pacing policy (seconds)."""
+        nothing is ever parked. `clock`: the time source of the pacing policy (seconds).
+        `kv_growth`: on an engine whose page pool cannot hold every request at its full budget, a request maps its
+        prompt and one poll of frames at admission and takes further pages as it decodes, under the banker's rule
+        (kv_safe); one that cannot get its next page now waits parked until it can. Off: prompt + budget are
+        reserved at admission and a running request never waits (DESIGN.md §4b)."""
         from .models.text2semantic.inference import _ensure_engine
 
         if not 1 <= max_slots <= MAX_DECODE_BATCH:
@@ -176,6 +197,17 @@ class ContinuousBatcher:
         self._pos = eng.buffer("pos")
         self._ras = eng.buffer("ras_window")
         self._out = eng.buffer("out_tokens")
+        pool = getattr(eng, "kv_pool", None)
+        # growth only where page accounting is needed at all (the `paged` test of _admit)
+        self.kv_growth = bool(kv_growth) and pool is not None and (
+            pool.n_pages < pool.slots * pool.pages_per_slot or self.max_live > self.max_slots)
+        self.short: list[SlotRequest] = []  # parked for pages (kv_growth), in the order they were parked
+        self._kv = None  # kv_growth: (avail, {request: [need, alone]}) while one step is being scheduled
+        if self.kv_growth:
+            self._miss = eng.buffer("kv_miss")
+            self._miss.zero_()
+            # unused slots idle at position -1, as retired ones do: at position 0 over no page they would record a miss
+            self._pos.fill_(-1)
 
     def close(self):
         """Give the engine back to the one-request-at-a-time entry points."""
@@ -223,7 +255,7 @@ class ContinuousBatcher:
         return req
 
     def idle(self) -> bool:
-        return not self.waiting and not self.active and not self.parked
+        return not self.waiting and not self.active and not self.parked and not self.short
 
     def _free_slots(self) -> list[int]:
         return [s for s in range(self.max_slots) if s not in self.active]
@@ -237,7 +269,11 @@ class ContinuousBatcher:
         self.parked.append(req)
 
     def _resume(self, req: SlotRequest, s: int):
-        self.parked.remove(req)
+        if any(r is req for r in self.short):
+            self.short.remove(req)
+            req.page_wait = max(req.page_wait, self.clock() - req._short_since)
+        else:
+            self.parked.remove(req)
         parked, req._parked = req._parked, None
         self.eng.resume_slot(s, parked)
         req.slot = s
@@ -246,18 +282,110 @@ class ContinuousBatcher:
         self._len[s] = parked.ctx_len
 
     def _schedule(self):
-        """One scheduling decision (schedule_live) carried out: park, resume, admit, fill."""
-        plan = schedule_live(list(self.active.values()), self.parked, self.waiting, self.clock(), self.max_slots,
-                             self.max_live, self.frames_per_poll)
+        """One scheduling decision (schedule_live) carried out: park, resume, admit, fill. With kv_growth, requests
+        parked for pages resume first, and every resume and admission needs a safe grant of its pages."""
+        if self.kv_growth:
+            self._kv = self._kv_state()
+            self._grants = {}  # slot -> end granted to a request resumed in this step
+            self._resume_short()
+        plan = schedule_live(list(self.active.values()), self.parked, [] if self.short else self.waiting,
+                             self.clock(), self.max_slots, self.max_live, self.frames_per_poll)
         for req in plan.park:
             self._park(req)
         free = self._free_slots()
         for req in plan.resume:
+            if self.kv_growth:
+                end = self._grant(req)
+                if end is None:  # due, but short of pages: it waits with those parked for pages
+                    self._to_short(req)
+                    continue
+                self._grants[free[0]] = end
             self._resume(req, free.pop(0))
         self._admit(plan.admit)
         free = self._free_slots()
-        for req in plan.fill[:len(free)]:
+        for req in plan.fill:
+            if not free:
+                break
+            if self.kv_growth:
+                end = self._grant(req)
+                if end is None:
+                    continue
+                self._grants[free[0]] = end
             self._resume(req, free.pop(0))
+
+    # ---- KV growth (kv_growth) -------------------------------------------------------------------------------------
+    def _kv_state(self):
+        """(pages available, {request: [need, alone]}) over every admitted request, running or parked."""
+        pool = self.eng.kv_pool
+        claims = {}
+        for r in [*self.active.values(), *self.parked, *self.short]:
+            held, alone = pool.row_pages(pool.table[r.slot] if r._parked is None else r._parked.row)
+            claims[r] = [kv_pages_for(int(r.prompt.size(1)) + r._limit) - held, alone]
+        return pool.available(), claims
+
+    def _target(self, req: SlotRequest) -> int:
+        """Positions `req` has mapped once the next poll's frames are written: they write from its next position,
+        context length - 1, on; never past prompt + budget."""
+        ctx = self._len[req.slot] if req._parked is None else req._parked.ctx_len
+        return min(ctx - 1 + self.frames_per_poll, int(req.prompt.size(1)) + req._limit)
+
+    def _grant(self, req: SlotRequest) -> Optional[int]:
+        """The end of `req`'s next poll (_target) when the pages it takes leave the state safe (they are counted as
+        taken from then on), else None."""
+        pool = self.eng.kv_pool
+        end = self._target(req)
+        held, _ = pool.row_pages(pool.table[req.slot] if req._parked is None else req._parked.row)
+        g = kv_pages_for(end) - held
+        if g <= 0:
+            return end
+        avail, claims = self._kv
+        need, alone = claims[req]
+        trial = dict(claims)
+        trial[req] = [need - g, alone + g]
+        if g > avail or not kv_safe(avail - g, trial.values()):
+            return None
+        claims[req] = trial[req]
+        self._kv = (avail - g, claims)
+        return end
+
+    def _resume_short(self):
+        """Requests parked for pages take free slots, in FIFO order, each once its grant is safe. One whose grant is not
+        safe yet lets the next one try: the first request of the safe order may be behind it."""
+        free = self._free_slots()
+        for req in list(self.short):
+            if not free:
+                break
+            end = self._grant(req)
+            if end is not None:
+                self._resume(req, free.pop(0))
+                self._grants[req.slot] = end
+
+    def _to_short(self, req: SlotRequest):
+        self.parked.remove(req)
+        self.short.append(req)
+        req.page_parks += 1
+        req._short_since = self.clock()
+
+    def _grow(self):
+        """Pages for the positions the next poll writes, for every running request, granted in safety order (smallest
+        need first); a request whose grant would make the state unsafe is parked for pages before the frames run.
+        One page-table upload for all grants (LmEngine.grow_kv)."""
+        ends, short = dict(self._grants), []
+        claims = self._kv[1]
+        for req in sorted((r for r in self.active.values() if r.slot not in ends), key=lambda r: claims[r][0]):
+            end = self._grant(req)
+            if end is None:
+                short.append(req)
+            else:
+                ends[req.slot] = end
+        for req in short:
+            self._park(req)
+            self._to_short(req)
+        if short:  # the slots they left may serve a request parked for pages whose grant is safe
+            self._resume_short()
+            ends.update(self._grants)
+        self.eng.grow_kv(ends)
+        self._kv = None
 
     def cancel(self, req: SlotRequest) -> bool:
         """Take `req` out wherever it is: waiting, running or parked. A running request's slot idles from the next
@@ -270,8 +398,8 @@ class ContinuousBatcher:
             self.waiting.remove(req)
         elif self.active.get(req.slot) is req:
             self._vacate([req])
-        elif req._parked is not None and any(r is req for r in self.parked):
-            self.parked.remove(req)
+        elif req._parked is not None and any(r is req for r in self.parked + self.short):
+            (self.short if any(r is req for r in self.short) else self.parked).remove(req)
             parked, req._parked = req._parked, None
             self.eng.drop_parked(parked)
         else:
@@ -319,9 +447,18 @@ class ContinuousBatcher:
                 # FIFO: the head of the queue waits until its pages fit, and nothing overtakes it
                 if head.reuse_prefix and head._host_prompt is None:  # one device -> host copy per request
                     head._host_prompt = head.prompt.detach().to("cpu", torch.int32)
-                need = self.eng.kv_pages_needed(head._host_prompt, T + head._limit, free[0], busy=slots,
-                                                reuse=head.reuse_prefix)
-                if need > pages:
+                end = T + (min(self.frames_per_poll, head._limit) if self.kv_growth else head._limit)
+                need = self.eng.kv_pages_needed(head._host_prompt, end, free[0], busy=slots, reuse=head.reuse_prefix)
+                if self.kv_growth:
+                    # growth: it maps its prompt and one poll of frames, if the state with it admitted is safe (it is
+                    # counted as giving nothing back: its prefix may be shared)
+                    avail, claims = self._kv
+                    claim = [kv_pages_for(T + head._limit) - kv_pages_for(end), 0]
+                    if need > avail or not kv_safe(avail - need, [*claims.values(), claim]):
+                        break
+                    claims[head] = claim
+                    self._kv = (avail - need, claims)
+                elif need > pages:
                     break
                 pages -= need
             req = head
@@ -351,14 +488,19 @@ class ContinuousBatcher:
             self._len[r.slot] = int(r.prompt.size(1)) + 1
         self.eng.set_context_bound_exact(max(self._len.values()) + 1)
         # paged KV: every request's pages (prompt + budget) are reserved before its prefill
-        kw = dict(kv_end=[int(r.prompt.size(1)) + r._limit for r in batch]) if pool is not None else {}
+        # (with kv_growth: the prompt and the first poll's frames)
+        kw = dict(kv_end=[int(r.prompt.size(1)) + (min(self.frames_per_poll, r._limit) if self.kv_growth else r._limit)
+                          for r in batch]) if pool is not None else {}
         if any(r.reuse_prefix for r in batch) and hasattr(self.eng, "prefill_reusing"):
             self.eng.prefill_reusing([r.prompt for r in batch], slots, None, do_sample=True, **kw)
         else:
             self.eng.prefill([r.prompt for r in batch], slots, None, do_sample=True, **kw)
 
     def _retire(self) -> list[SlotRequest]:
-        st = torch.stack([self._state.to(torch.int32), self._n_out]).cpu()  # one small D2H copy (synchronises)
+        rows = [self._state.to(torch.int32), self._n_out] + ([self._miss] if self.kv_growth else [])
+        st = torch.stack(rows).cpu()  # one small D2H copy (synchronises)
+        if self.kv_growth:
+            self._fail_missed(st[2])
         for s, req in self.active.items():
             # frames of a streaming request leave as soon as they are final: all but the newest one (the last frame of
             # a request -- <|im_end|> or the one at the budget -- is never part of what generate_long keeps)
@@ -389,10 +531,28 @@ class ContinuousBatcher:
                 req.on_done(req)
         return finished
 
+    def _fail_missed(self, miss: torch.Tensor):
+        """Requests whose decode attention met an unmapped page (the "kv_miss" buffer) sampled from a void attention:
+        each fails alone, with the slot and position; its neighbours continue."""
+        bad = [r for s, r in self.active.items() if int(miss[s]) != 0]
+        if not bad:
+            return
+        for r in bad:
+            r.error = RuntimeError(f"slot {r.slot}: decode attention met an unmapped KV page at position "
+                                   f"{int(miss[r.slot]) - 1}; the request's tokens are void")
+        self._miss[torch.tensor([r.slot for r in bad], dtype=torch.long, device=self._miss.device)] = 0
+        self._vacate(bad)
+        for r in bad:
+            r.done.set()
+            if r.on_done is not None:
+                r.on_done(r)
+
     def step(self) -> list[SlotRequest]:
         """Park / resume paced requests and admit waiting ones into free slots (schedule_live), run
         `frames_per_poll` frames, retire what finished."""
         self._schedule()
+        if self.kv_growth:
+            self._grow()
         if not self.active:
             return []
         k = self.frames_per_poll

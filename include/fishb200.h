@@ -199,6 +199,9 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
  *   the slot-control arrays listed at fsb_lm_set_slot_control, "kv_page" int32 [max_batch][ceil(kv_len / 64)]
  *   (page of each 64-position block of each slot, -1 = not mapped; read by the kernels at run time, so a captured
  *   decode graph stays valid when the caller remaps pages between calls),
+ *   "kv_miss" int32 [max_batch] (0, or 1 + the position of a slot's live decode row the first time the slow-stack
+ *   decode attention found a page it reads or appends to unmapped: that row attended to nothing and its tokens are
+ *   void; zeroed at create, never cleared by the library: the caller zeroes a slot's entry when it reuses the slot),
  *   debug only: "slow_logits" f32 [max_batch][head_rows], "fast_logits" f32 [C][max_batch][codebook_size];
  *   the decode state (for fsb_lm_test_layer_gemms), RT = the decode row tile (32 for max_batch <= 32, else 64):
  *   "x_slow" / "x_fast" bf16 [RT][dim] / [RT][fast_dim] residual streams, "ssq_slow" / "ssq_fast" f32 [RT][32] their

@@ -1,4 +1,5 @@
-"""Codec input front end: PCM at any sample rate -> the codec's mono fp32 input, on the device.
+"""Codec input and output front ends on the device: PCM at any sample rate -> the codec's mono fp32 input, and the
+decoder's fp32 44.1 kHz output -> the client's sample rate and sample format.
 
 * `resample(x, orig_freq, new_freq)`: `torchaudio.functional.resample` with its defaults (sinc_interp_hann,
   lowpass_filter_width 6, rolloff 0.99). On a CUDA float32 tensor it runs `fsb_resample` (csrc/audio_kernels.cu); on
@@ -10,6 +11,9 @@
 * `StreamResampler`: the same resampler over a signal that arrives in pieces. Each push emits the outputs whose filter
   window is complete and keeps on the device the input history the next outputs read; `flush` emits the tail against
   zero right-padding. The concatenated outputs are bit-identical to `resample` of the whole signal.
+* `convert_out` / `OutputStream`: the same resampler run from the decoder's rate to the client's, with the sample
+  format (float32, int16 PCM as `inference_engine.utils.pcm16`, or G.711 mu-law) fused into the same launch
+  (`fsb_audio_out`), one-shot and streamed with the same bits.
 
 The filter table is built on the host in float64 from torchaudio's formula (`filter_table`) and cast to fp32 once per
 rate pair and device. Taps where the Hann window is zero are dropped, so each output is one fixed sequence of fp64
@@ -417,15 +421,8 @@ class StreamResampler:
                         rs.counts.push(x.numel())
                         plan.append(x)
                     continue
-                h0, hist = rs._h0, rs._hist
-                segs.append(hist)
-                n_win = hist.numel()
-                if x is None:
-                    j0, n = rs.counts.flush()
-                else:
-                    segs.append(x)
-                    n_win += x.numel()
-                    j0, n, _ = rs.counts.push(x.numel())
+                seg, h0, n_win, j0, n = rs._take(x)
+                segs += seg
                 plan.append((rs, off, h0, n_win, j0, n))
                 off += n_win
             win = torch.cat(segs) if segs else None
@@ -447,7 +444,170 @@ class StreamResampler:
                 rs, x_off, h0, n_win, j0, n = pl
                 res.append(out[rows[k][4]: rows[k][4] + n])
                 k += 1
-                keep = rs.counts.keep_from() if not rs.counts.done else rs.counts.received
-                rs._hist = win[x_off + keep - h0: x_off + n_win]
-                rs._h0 = keep
+                rs._retain(win, x_off, h0, n_win)
+            return res
+
+    def _take(self, x: Optional[torch.Tensor]) -> tuple:
+        """Advance the counts by a piece (None: the flush) -> (window pieces [history, piece], input index of the
+        window's first sample, window length, first output, outputs now ready)."""
+        segs, h0, n_win = [self._hist], self._h0, self._hist.numel()
+        if x is None:
+            j0, n = self.counts.flush()
+        else:
+            segs.append(x)
+            n_win += x.numel()
+            j0, n, _ = self.counts.push(x.numel())
+        return segs, h0, n_win, j0, n
+
+    def _retain(self, win: torch.Tensor, x_off: int, h0: int, n_win: int) -> None:
+        """Keep, of this stream's window at win[x_off: x_off + n_win], the samples the next outputs read."""
+        keep = self.counts.keep_from() if not self.counts.done else self.counts.received
+        self._hist = win[x_off + keep - h0: x_off + n_win]
+        self._h0 = keep
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# output front end: the decoder's fp32 waveform -> the client's rate and sample format (fsb_audio_out)
+# ---------------------------------------------------------------------------------------------------------------------
+CODEC_RATE = 44100  # the decoder's output rate (CodecConfig.sample_rate)
+# sample format name -> (fsb_audio_out_row.format, include/fishb200.h FSB_OUT_*; element dtype)
+OUTPUT_FORMATS = {"float32": (0, torch.float32), "pcm16": (1, torch.int16), "mulaw": (2, torch.uint8)}
+
+
+def output_format(sample_format: Optional[str]) -> str:
+    """The format name a request's `sample_format` stands for: None is float32."""
+    fmt = "float32" if sample_format is None else str(sample_format)
+    if fmt not in OUTPUT_FORMATS:
+        raise ValueError(f"sample_format must be one of {sorted(OUTPUT_FORMATS)} (got {sample_format!r})")
+    return fmt
+
+
+def _launch_out(x: torch.Tensor, rows: list, out: torch.Tensor) -> None:
+    """rows: per output row (x_off, x_start, x_end, j0, out byte offset, n_out, table or None, format code) -> one
+    fsb_audio_out launch into the bytes of `out`."""
+    desc = []
+    for x_off, x_start, x_end, j0, out_off, n_out, tab, code in rows:
+        if tab is None:
+            w_ptr, s_ptr, o, n = 0, 0, 1, 1
+        else:
+            w_ptr, s_ptr, o, n = tab[0].data_ptr(), tab[1].data_ptr(), tab[2], tab[3]
+        desc.append([x_off, x_start, x_end, j0, out_off, n_out, w_ptr, s_ptr, o, n, code])
+    d = torch.tensor(desc, dtype=torch.int64).to(x.device)
+    _lib.check(_lib.lib().fsb_audio_out(x.data_ptr(), d.data_ptr(), len(rows), max(r[5] for r in rows),
+                                        out.data_ptr(), _stream(x.device)))
+
+
+def convert_out(wav: torch.Tensor, sample_rate: Optional[int] = None, sample_format: Optional[str] = None,
+                orig_freq: int = CODEC_RATE) -> torch.Tensor:
+    """A CUDA fp32 waveform [..., N] at `orig_freq` -> [..., M] at `sample_rate` in `sample_format` (float32, pcm16 =
+    int16, mulaw = uint8), every row in one fsb_audio_out launch. M is torchaudio's length; the float32 samples are
+    the bits of `resample`, pcm16 is utils.pcm16 of them and mulaw G.711 of that. With no rate and no format (or the
+    waveform's own rate in float32) the waveform itself is returned."""
+    fmt = output_format(sample_format)
+    rate = int(orig_freq) if sample_rate is None else int(sample_rate)
+    if rate <= 0:
+        raise ValueError(f"sample_rate must be positive (got {sample_rate})")
+    if wav.device.type != "cuda" or wav.dtype != torch.float32:
+        raise TypeError(f"convert_out takes a CUDA float32 waveform (got {wav.dtype} on {wav.device})")
+    if rate == int(orig_freq) and fmt == "float32":
+        return wav
+    code, dtype = OUTPUT_FORMATS[fmt]
+    shape = wav.shape
+    n = int(shape[-1])
+    x = wav.reshape(-1, n).contiguous()
+    rows = x.shape[0]
+    with torch.cuda.device(x.device):
+        identity = rate == int(orig_freq)
+        tab = None if identity else _device_table(orig_freq, rate, x.device)
+        out_n = n if identity else filter_table(int(orig_freq), rate).total(n)
+        out = torch.empty(rows, out_n, dtype=dtype, device=x.device)
+        if rows and out_n:
+            es = out.element_size()
+            _launch_out(x, [(r * n, 0, n, 0, r * out_n * es, out_n, tab, code) for r in range(rows)], out)
+    return out.reshape(*shape[:-1], out_n)
+
+
+class OutputStream(StreamResampler):
+    """`convert_out` over a waveform that arrives in pieces: `push(piece)` -> the converted samples now complete,
+    `flush()` -> the rest (the filter's look-ahead holds back up to about 6 input samples per output phase). The
+    concatenated results are bit-identical to `convert_out` of the whole waveform. History is kept as
+    `StreamResampler` keeps it; at the input rate there is none, and float32 there passes pieces through."""
+
+    def __init__(self, sample_rate: Optional[int] = None, sample_format: Optional[str] = None, device="cuda",
+                 orig_freq: int = CODEC_RATE):
+        rate = int(orig_freq) if sample_rate is None else int(sample_rate)
+        if rate <= 0:
+            raise ValueError(f"sample_rate must be positive (got {sample_rate})")
+        super().__init__(orig_freq, rate, device)
+        self.sample_format = output_format(sample_format)
+        self._code, self.dtype = OUTPUT_FORMATS[self.sample_format]
+
+    @property
+    def sample_rate(self) -> int:
+        return self.new_freq
+
+    def push(self, x: torch.Tensor) -> torch.Tensor:
+        return OutputStream.push_many([(self, x)])[0]
+
+    def flush(self) -> torch.Tensor:
+        return OutputStream.push_many([(self, None)])[0]
+
+    @staticmethod
+    def push_many(items: list) -> list:
+        """[(stream, fp32 piece on its device, or None to flush)] -> their converted samples, every stream (of any
+        rate and format) in one launch (the streams must share a device)."""
+        if not items:
+            return []
+        dev = items[0][0].device
+        with torch.cuda.device(dev):
+            segs, plan, off = [], [], 0
+            for st, x in items:
+                if st.device != dev:
+                    raise ValueError("push_many: streams on different devices")
+                if x is not None:
+                    x = x.reshape(-1)
+                    if x.dtype != torch.float32 or x.device != dev:
+                        raise ValueError("a piece must be float32 on the stream's device")
+                if st.identity and st._code == 0:  # float32 at the input rate: the piece itself
+                    if x is None:
+                        st.counts.flush()
+                    else:
+                        st.counts.push(x.numel())
+                    plan.append(x if x is not None else torch.empty(0, dtype=torch.float32, device=dev))
+                    continue
+                if st.identity:  # quantise only: output j is input j, no history
+                    r0 = st.counts.received
+                    seg, h0, n_win, j0 = ([] if x is None else [x]), r0, (0 if x is None else x.numel()), r0
+                    if x is None:
+                        st.counts.flush()
+                    else:
+                        st.counts.push(n_win)
+                    n = n_win
+                else:
+                    seg, h0, n_win, j0, n = st._take(x)
+                segs += seg
+                plan.append((st, off, h0, n_win, j0, n))
+                off += n_win
+            win = torch.cat(segs) if segs else None
+            rows, ob = [], 0
+            for pl in plan:
+                if isinstance(pl, tuple):
+                    st, x_off, h0, n_win, j0, n = pl
+                    rows.append((x_off, h0, st.counts.received, j0, ob, n, st._tab, st._code))
+                    ob += -(-n * st.dtype.itemsize // 16) * 16  # every row's bytes 16-aligned: a view of any dtype
+            out = torch.empty(max(16, ob), dtype=torch.uint8, device=dev)
+            live = [r for r in rows if r[5] > 0]
+            if live:
+                _launch_out(win, live, out)
+            res, k = [], 0
+            for pl in plan:
+                if not isinstance(pl, tuple):
+                    res.append(pl)
+                    continue
+                st, x_off, h0, n_win, j0, n = pl
+                b = rows[k][4]
+                res.append(out[b: b + n * st.dtype.itemsize].view(st.dtype))
+                k += 1
+                if not st.identity:
+                    st._retain(win, x_off, h0, n_win)
             return res

@@ -31,3 +31,7 @@ except Exception:
         top_p: float = 0.8
         repetition_penalty: float = 1.1
         temperature: float = 0.8
+        # extensions of ours: the audio handed out, converted on the device (audio.convert_out). None: the codec's
+        # fp32 at 44.1 kHz, as the reference hands it out
+        sample_rate: Optional[int] = None
+        sample_format: Optional[str] = None  # "float32", "pcm16" (int16) or "mulaw" (uint8, G.711)

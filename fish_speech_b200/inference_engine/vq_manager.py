@@ -28,9 +28,10 @@ class VQManager:
         logger.info(f"VQ features: {codes.shape}")
         return self._codec().from_indices(codes[None])[0].squeeze()
 
-    def open_decode_stream(self, max_frames: int = 4096) -> DecodeStream:
-        """Incremental decoder for one utterance: `.push(codes[None])` as frames arrive (models/dac/modded_dac.py)."""
-        return self._codec().open_decode_stream(batch=1, max_frames=max_frames)
+    def open_decode_stream(self, max_frames: int = 4096, **conversion) -> DecodeStream:
+        """Incremental decoder for one utterance: `.push(codes[None])` as frames arrive (models/dac/modded_dac.py);
+        `sample_rate=` / `sample_format=` convert what it returns (and then `.flush()` ends it)."""
+        return self._codec().open_decode_stream(batch=1, max_frames=max_frames, **conversion)
 
     def encode_reference(self, reference_audio, enable_reference_audio) -> Optional[torch.Tensor]:
         """Reference clip (bytes or path) -> prompt codes [C, T], or None when reference audio is off."""

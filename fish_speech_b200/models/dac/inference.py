@@ -55,6 +55,18 @@ def load_model(config_name, checkpoint_path, device="cuda") -> DAC:
     return model
 
 
+def write_wav(path: Path, samples: np.ndarray, sample_rate: int, sample_format: str) -> None:
+    """A mono WAV file of samples already in `sample_format` (audio.OUTPUT_FORMATS), written as they are."""
+    from ...inference_engine.utils import WAVE_OF_FORMAT, wav_chunk_header
+
+    bits, tag = WAVE_OF_FORMAT[sample_format]
+    data = np.ascontiguousarray(samples).astype(samples.dtype.newbyteorder("<")).tobytes()
+    head = bytearray(wav_chunk_header(sample_rate=sample_rate, bit_depth=bits, format_tag=tag))
+    head[4:8] = (len(head) - 8 + len(data)).to_bytes(4, "little")  # RIFF size
+    head[40:44] = len(data).to_bytes(4, "little")  # data size
+    Path(path).write_bytes(bytes(head) + data)
+
+
 def main(argv=None):
     import click
 
@@ -64,11 +76,17 @@ def main(argv=None):
     @click.option("--config-name", default="modded_dac_vq")
     @click.option("--checkpoint-path", default="checkpoints/openaudio-s1-mini/codec.pth")
     @click.option("--device", "-d", default="cuda")
-    def _main(input_path, output_path, config_name, checkpoint_path, device):
+    @click.option("--output-sample-rate", type=int, default=None,
+                  help="Sample rate of the written audio (default: the codec's), resampled on the device.")
+    @click.option("--output-format", type=click.Choice(["float", "pcm16", "mulaw"]), default=None,
+                  help="Samples of the written WAV, converted on the device: float (32-bit IEEE), pcm16 (16-bit PCM, "
+                       "clipped to [-1, 1] and scaled by 32767) or mulaw (8-bit G.711). Default: the codec's float "
+                       "waveform, written by soundfile as before.")
+    def _main(input_path, output_path, config_name, checkpoint_path, device, output_sample_rate, output_format):
         import soundfile as sf
         import torchaudio
 
-        from ...audio import resample
+        from ...audio import convert_out, resample
 
         model = load_model(config_name, checkpoint_path, device=device)
         if input_path.suffix in AUDIO_EXTENSIONS:
@@ -89,7 +107,16 @@ def main(argv=None):
         if indices.ndim == 2:
             indices = indices.unsqueeze(0)
         fake = model.from_indices(indices)
-        sf.write(output_path, fake[0, 0].float().cpu().numpy(), model.sample_rate)
+        rate = model.sample_rate if output_sample_rate is None else int(output_sample_rate)
+        if output_sample_rate is None and output_format is None:
+            sf.write(output_path, fake[0, 0].float().cpu().numpy(), model.sample_rate)
+        else:
+            fmt = {None: "float32", "float": "float32"}.get(output_format, output_format)
+            out = convert_out(fake[0, 0].float(), rate, fmt, orig_freq=model.sample_rate).cpu().numpy()
+            if output_format is None:  # a rate alone: the float waveform, written by soundfile as before
+                sf.write(output_path, out, rate)
+            else:
+                write_wav(output_path, out, rate, fmt)
         logger.info(f"Saved audio to {output_path}")
 
     return _main(argv, standalone_mode=False) if argv is not None else _main()

@@ -492,10 +492,13 @@ class DAC:
             cur = out
         return self._decoder(cur, B, Tc)
 
-    def open_decode_stream(self, batch: int = 1, max_frames: int = 4096, conv_context: int = 16) -> "DecodeStream":
+    def open_decode_stream(self, batch: int = 1, max_frames: int = 4096, conv_context: int = 16,
+                           sample_rate: Optional[int] = None, sample_format: Optional[str] = None) -> "DecodeStream":
         """Incremental `from_indices` (SURVEY §8(f).3): push code frames as the LM emits them, get their samples back.
-        The codec is causal (rvq.py:395-398 asserts it), so what a frame sounds like never depends on later frames."""
-        return DecodeStream(self, batch, max_frames, conv_context)
+        The codec is causal (rvq.py:395-398 asserts it), so what a frame sounds like never depends on later frames.
+        With a `sample_rate` or `sample_format` (see audio.convert_out) the samples come converted, and `flush()` at
+        the end returns the ones the resampler's look-ahead held back."""
+        return DecodeStream(self, batch, max_frames, conv_context, sample_rate, sample_format)
 
     def open_stream_pool(self, slots: int, k_max: int = 32, max_graphs: int = 8) -> "DecodeStreamPool":
         """Streaming decode of up to `slots` independent streams at once: streams join and leave at any push, and one
@@ -765,8 +768,13 @@ class DecodeStream:
       as long as conv_context covers the receptive field (tests compare with the one-shot decode).
     """
 
-    def __init__(self, dac: "DAC", batch: int, max_frames: int, conv_context: int):
+    def __init__(self, dac: "DAC", batch: int, max_frames: int, conv_context: int,
+                 sample_rate: Optional[int] = None, sample_format: Optional[str] = None):
         self.dac, self.B, self.S, self.ctx = dac, int(batch), int(max_frames), int(conv_context)
+        # one output converter per row, when a rate or format is asked for
+        self.out = None if sample_rate is None and sample_format is None else [
+            audio.OutputStream(sample_rate, sample_format, dac.device, orig_freq=dac.sample_rate)
+            for _ in range(self.B)]
         t: TfmConfig = dac.post_tfm["cfg"]
         dev = dac.device
         n = self.B * t.n_head * self.S * t.head_dim
@@ -777,11 +785,30 @@ class DecodeStream:
 
     @torch.inference_mode()
     def push(self, indices: torch.Tensor) -> torch.Tensor:
-        """codes [B, 1+n_codebooks, k] of the next k frames -> waveform [B, 1, k * frame_length] (fp32)."""
+        """codes [B, 1+n_codebooks, k] of the next k frames -> waveform [B, 1, k * frame_length] (fp32), or with a
+        rate or format the samples of each row converted so far [B, 1, m]."""
+        wav = self._push(indices)
+        return wav if self.out is None else self._convert([w for w in wav[:, 0]])
+
+    @torch.inference_mode()
+    def flush(self) -> torch.Tensor:
+        """End of the stream: [B, 1, m], the converted samples pushes held back ([B, 1, 0] fp32 without conversion)."""
+        if self.out is None:
+            return torch.zeros(self.B, 1, 0, dtype=torch.float32, device=self.dac.device)
+        return self._convert([None] * self.B)
+
+    def _convert(self, pieces: list) -> torch.Tensor:
+        with self.dac._lock, torch.cuda.device(self.dac.device):
+            ys = audio.OutputStream.push_many(list(zip(self.out, pieces)))
+        return torch.stack(ys)[:, None]
+
+    def _push(self, indices: torch.Tensor) -> torch.Tensor:
         dac, cfg = self.dac, self.dac.cfg
         B, S_, k = indices.shape
         if B != self.B:
             raise ValueError(f"stream was opened for batch {self.B}, got {B}")
+        if self.out is not None and self.out[0].counts.done:
+            raise ValueError("the stream was flushed")
         if k == 0:
             return torch.zeros(B, 1, 0, dtype=torch.float32, device=dac.device)
         if self.pos + k > self.S:
@@ -1006,7 +1033,67 @@ class DecodeStreamPool(_StreamPool):
         self._tfms = [(t, 1)]
         # one (H rows, C channels, rows per frame) per conv input of the upsampler + decoder, in execution order
         self.layers = self._layer_geometry()
+        self._out: dict = {}  # slot -> audio.OutputStream, for slots opened with a sample rate or format
         super().__init__(dac, slots, k_max, max_graphs)
+
+    def open(self, sample_rate: Optional[int] = None, sample_format: Optional[str] = None) -> int:
+        """A new stream's slot. Without a rate or format its pushes return fp32 at the codec's rate, as always; with
+        either, they return the samples converted so far (audio.OutputStream: torchaudio's resampler, then float32,
+        pcm16 = int16 or mulaw = uint8), and `flush(slot)` returns the rest."""
+        conv = sample_rate is not None or sample_format is not None
+        if conv:  # check the arguments before a slot is taken
+            out = audio.OutputStream(sample_rate, sample_format, self.dac.device, orig_freq=self.dac.sample_rate)
+        with self.dac._lock, torch.cuda.device(self.dac.device):
+            slot = super().open()
+            if conv:
+                self._out[slot] = out
+            return slot
+
+    def close(self, slot: int) -> None:
+        with self.dac._lock:
+            super().close(slot)
+            self._out.pop(slot, None)
+
+    def push(self, pieces: dict) -> dict:
+        """{slot: codes [1+n_codebooks, k]} -> {slot: audio}: fp32 [k * frame_length] for a slot opened without a rate
+        or format; the samples converted so far for one opened with them. The frames of every slot run in one pass
+        (a captured graph per bucket, whatever the slots' formats); then every converted slot's samples are
+        converted in one fsb_audio_out launch."""
+        for slot in pieces:
+            st = self._out.get(slot)
+            if st is not None and st.counts.done:
+                raise ValueError(f"slot {slot}: the stream was flushed")
+        out = super().push(pieces)
+        conv = [s for s in out if s in self._out]
+        if conv:
+            with torch.inference_mode(), self.dac._lock, torch.cuda.device(self.dac.device):
+                try:
+                    ys = audio.OutputStream.push_many([(self._out[s], out[s]) for s in conv])
+                except BaseException:
+                    for s in conv:
+                        self.broken[s] = True
+                    raise
+            out.update(zip(conv, ys))
+        return out
+
+    def flush(self, slot: int) -> torch.Tensor:
+        """End the stream of a slot opened with a rate or format: the samples the filter's look-ahead held back (its
+        window closed with zeros, as the one-shot conversion closes it). The slot then takes no more pushes until it is
+        closed and opened again. A slot opened without either has nothing pending: fp32 [0]."""
+        self._check_slot(slot)
+        if self.broken[slot]:
+            raise ValueError(f"slot {slot}: an earlier push failed, its state is lost; close the slot")
+        st = self._out.get(slot)
+        if st is None:
+            return torch.empty(0, dtype=torch.float32, device=self.dac.device)
+        if st.counts.done:
+            raise ValueError(f"slot {slot}: the stream was already flushed")
+        with torch.inference_mode(), self.dac._lock, torch.cuda.device(self.dac.device):
+            try:
+                return st.flush()
+            except BaseException:
+                self.broken[slot] = True
+                raise
 
     def _layer_geometry(self) -> list:
         dac, D = self.dac, self.dac.cfg.latent_dim

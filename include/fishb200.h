@@ -381,6 +381,33 @@ int fsb_resample(const float* d_x, const fsb_resample_clip* d_clips, int B, long
                  void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Codec output front end (csrc/audio_kernels.cu): the decoder's fp32 44.1 kHz waveform -> the client's rate and sample
+ * format, on the device, in one pass.
+ *   replaces the per-segment `(audio * 32768).astype(np.int16)` of the serving shell (tools/server/inference.py:32-33)
+ *   and any resampling a client would do on the host.
+ * ---------------------------------------------------------------------------------------------- */
+#define FSB_OUT_F32 0   /* float32: the fp32 value y itself */
+#define FSB_OUT_PCM16 1 /* int16: trunc(min(max(y, -1), 1) * 32767.0f), the product rounded to nearest (not fused);
+                           NaN -> 0. Equal to inference_engine/utils.py:pcm16. */
+#define FSB_OUT_MULAW 2 /* uint8: G.711 mu-law (bias 132, 8 segments) of that int16, as audioop.lin2ulaw */
+
+typedef struct {
+    long long x_off, x_start, x_end; /* as fsb_resample_clip: d_x[x_off ..] holds input samples [x_start, x_end) */
+    long long j0;       /* first output (absolute index in the row's output) to compute */
+    long long out_off;  /* BYTE offset in d_out of output j0, aligned to the format's size */
+    long long n_out;    /* outputs computed: j0 .. j0 + n_out - 1 */
+    const float* w;     /* as fsb_resample_clip; NULL = no resampling (output j is input j) */
+    const int32_t* span;
+    long long orig, new_rate;
+    long long format;   /* FSB_OUT_* */
+} fsb_audio_out_row;
+
+/* Each output y is what fsb_resample computes for it (the same fp64 sum, rounded to fp32 once), stored in the row's
+ * format. Rows of different rates and formats share a launch; max_out >= every row's n_out. */
+int fsb_audio_out(const float* d_x, const fsb_audio_out_row* d_rows, int B, long long max_out, void* d_out,
+                  void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Unit-test hooks (used by tests/ only)
  * ---------------------------------------------------------------------------------------------- */
 /* out[j][i] (fp32, ld = m) = sum_k A[i][k] * B[j][k]; A [m,k], B [n,k] bf16 row-major, by the prefill / codec GEMM

@@ -121,6 +121,7 @@ def lib() -> C.CDLL:
     L.fsb_op_step_gemm_tile.argtypes = [vp, i32, i32, vp, i32, i32, vp, vp, C.c_float, i32, i32, vp, i32p, vp]
     L.fsb_lm_test_layer_gemms.argtypes = [vp, i32, i32, i32, i32, vp]
     L.fsb_lm_test_layer_attn.argtypes = [vp, i32, i32, i32, i32, vp]
+    L.fsb_lm_test_prefill_stage.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]
     L.fsb_pcm_to_mono.argtypes = [vp, vp, i32, ll, vp, vp]
     L.fsb_resample.argtypes = [vp, vp, i32, ll, vp, vp]
     L.fsb_audio_out.argtypes = [vp, vp, i32, ll, vp, vp]

@@ -275,69 +275,114 @@ int run_stack_decode(fsb_lm* h, Stack& s, int rows, const int* row_seq, const in
     return 0;
 }
 
-// ---- prefill: the same stack over `rows` token rows with wide-N tensor-core GEMMs and consumer kernels.
-// On entry xn_p = attention_norm_0(xres_p). ----
-int run_stack_prefill(fsb_lm* h, Stack& s, int rows, const int* row_seq, const int* row_pos, cudaStream_t st) {
+EmbedArgs embed_args(fsb_lm* h, const int* tokens, bf16* x, float* ssq, int rows) {
+    const fsb_lm_config& c = h->cfg;
+    EmbedArgs ea{};
+    ea.tokens = tokens;
+    ea.emb = h->emb; ea.cb_emb = h->cb_emb; ea.x = x; ea.ssq = ssq;
+    ea.rows = rows; ea.D = h->slow.D; ea.C = c.num_codebooks; ea.cs = c.codebook_size; ea.vocab = c.vocab_size;
+    ea.sem_begin = c.semantic_begin_id; ea.sem_end = c.semantic_end_id;
+    ea.scale = c.scale_codebook_embeddings;
+    return ea;
+}
+
+// ---- prefill: the same stack over `rows` token rows with wide-N tensor-core GEMMs and consumer kernels. ----
+// The stages of one prefill layer, in launch order (fsb_lm_test_prefill_stage runs any one of them).
+enum PrefillStage { kPfEmbed = 0, kPfQkv, kPfAttn, kPfWo, kPfW13, kPfW2, kPfStages };
+
+// The prologue: xres_p = embed(tokens), xn_p = attention_norm_0(xres_p).
+int prefill_embed(fsb_lm* h, const int* tokens, int rows, cudaStream_t st) {
+    Stack& s = h->slow;
+    FSB_TRY(launch_embed(embed_args(h, tokens, h->xres_p, nullptr, rows), st));
+    ResidNormArgs r{};
+    r.x_in = h->xres_p;
+    r.norm_w = s.w[0].attn_norm; r.n_out = h->xn_p;
+    r.rows = rows; r.D = s.D; r.eps = h->cfg.norm_eps;
+    return launch_resid_norm(r, st);
+}
+
+// One stage (kPfQkv .. kPfW2) of slow layer l: one place for run_stack_prefill and fsb_lm_test_prefill_stage, so that
+// the test hook launches exactly what prefill launches.
+int prefill_stage(fsb_lm* h, int l, int stage, int rows, const int* row_seq, const int* row_pos, cudaStream_t st) {
+    Stack& s = h->slow;
     const float eps = h->cfg.norm_eps;
-    const int Nqkv = (s.H + 2 * s.Hkv) * s.Dh;
-    for (int l = 0; l < s.nl; ++l) {
-        const LayerW& w = s.w[l];
-        PrefillLayer& P = s.pf[l];
-        FSB_TRY(launch_rows_of(P.qkv, P.qkv_wide, rows, st));
-        QkvPrepArgs qa{};
-        qa.y = h->ws; qa.ld = Nqkv;
-        qa.bias = w.bqkv;
-        qa.q_norm = s.qk_norm ? w.q_norm : nullptr;
-        qa.k_norm = s.qk_norm ? w.k_norm : nullptr;
-        qa.freqs = s.freqs;
-        qa.row_seq = row_seq;
-        qa.row_pos = row_pos;
-        qa.q = h->q_p;
-        qa.kcache = s.kcache + l * s.cache_layer_stride;
-        qa.vcache = s.vcache + l * s.cache_layer_stride;
-        qa.kv_page = s.kv_page;
-        qa.kv_page_ld = s.kv_page_ld;
-        qa.rows = rows; qa.H = s.H; qa.Hkv = s.Hkv; qa.Dh = s.Dh; qa.S = s.S;
-        qa.eps = eps;
-        FSB_TRY(launch_qkv_prep(qa, st));
-        AttnArgs aa{};
-        aa.q = h->q_p;
-        aa.kcache = qa.kcache;
-        aa.vcache = qa.vcache;
-        aa.kv_page = s.kv_page;
-        aa.kv_page_ld = s.kv_page_ld;
-        aa.row_seq = row_seq;
-        aa.row_pos = row_pos;
-        aa.out = h->attn_p;
-        aa.rows = rows; aa.H = s.H; aa.Hkv = s.Hkv; aa.Dh = s.Dh; aa.S = s.S;
-        aa.window = 0;
-        aa.lcap = h->ctx_lcap;
-        aa.bf16_math = 0;
-        FSB_TRY(launch_attn(aa, st));
-        FSB_TRY(launch_rows_of(P.wo, rows, st));
-        ResidNormArgs r1{};
-        r1.y = h->ws; r1.ld = s.D;
-        r1.bias = w.bo;
-        r1.x_in = h->xres_p; r1.x_out = h->xres_p;
-        r1.norm_w = w.ffn_norm; r1.n_out = h->xn_p;
-        r1.rows = rows; r1.D = s.D; r1.eps = eps;
-        FSB_TRY(launch_resid_norm(r1, st));
-        FSB_TRY(launch_rows_of(P.w13, P.w13_wide, rows, st));
-        SwigluArgs sa{};
-        sa.y = h->ws; sa.ld = s.n13;
-        sa.h = h->h_p; sa.rows = rows; sa.I = s.I;
-        sa.interleaved = 1;
-        FSB_TRY(launch_swiglu(sa, st));
-        FSB_TRY(launch_rows_of(P.w2, rows, st));
-        ResidNormArgs r2{};
-        r2.y = h->ws; r2.ld = s.D;
-        r2.x_in = h->xres_p; r2.x_out = h->xres_p;
-        // the final norm is applied by the head GEMM's normalise-on-load on the last-token rows only
-        r2.norm_w = (l + 1 < s.nl) ? s.w[l + 1].attn_norm : nullptr;
-        r2.n_out = h->xn_p;
-        r2.rows = rows; r2.D = s.D; r2.eps = eps;
-        FSB_TRY(launch_resid_norm(r2, st));
+    const LayerW& w = s.w[l];
+    PrefillLayer& P = s.pf[l];
+    switch (stage) {
+        case kPfQkv: {
+            FSB_TRY(launch_rows_of(P.qkv, P.qkv_wide, rows, st));
+            QkvPrepArgs qa{};
+            qa.y = h->ws; qa.ld = (s.H + 2 * s.Hkv) * s.Dh;
+            qa.bias = w.bqkv;
+            qa.q_norm = s.qk_norm ? w.q_norm : nullptr;
+            qa.k_norm = s.qk_norm ? w.k_norm : nullptr;
+            qa.freqs = s.freqs;
+            qa.row_seq = row_seq;
+            qa.row_pos = row_pos;
+            qa.q = h->q_p;
+            qa.kcache = s.kcache + l * s.cache_layer_stride;
+            qa.vcache = s.vcache + l * s.cache_layer_stride;
+            qa.kv_page = s.kv_page;
+            qa.kv_page_ld = s.kv_page_ld;
+            qa.rows = rows; qa.H = s.H; qa.Hkv = s.Hkv; qa.Dh = s.Dh; qa.S = s.S;
+            qa.eps = eps;
+            return launch_qkv_prep(qa, st);
+        }
+        case kPfAttn: {
+            AttnArgs aa{};
+            aa.q = h->q_p;
+            aa.kcache = s.kcache + l * s.cache_layer_stride;
+            aa.vcache = s.vcache + l * s.cache_layer_stride;
+            aa.kv_page = s.kv_page;
+            aa.kv_page_ld = s.kv_page_ld;
+            aa.row_seq = row_seq;
+            aa.row_pos = row_pos;
+            aa.out = h->attn_p;
+            aa.rows = rows; aa.H = s.H; aa.Hkv = s.Hkv; aa.Dh = s.Dh; aa.S = s.S;
+            aa.window = 0;
+            aa.lcap = h->ctx_lcap;
+            aa.bf16_math = 0;
+            return launch_attn(aa, st);
+        }
+        case kPfWo: {
+            FSB_TRY(launch_rows_of(P.wo, rows, st));
+            ResidNormArgs r1{};
+            r1.y = h->ws; r1.ld = s.D;
+            r1.bias = w.bo;
+            r1.x_in = h->xres_p; r1.x_out = h->xres_p;
+            r1.norm_w = w.ffn_norm; r1.n_out = h->xn_p;
+            r1.rows = rows; r1.D = s.D; r1.eps = eps;
+            return launch_resid_norm(r1, st);
+        }
+        case kPfW13: {
+            FSB_TRY(launch_rows_of(P.w13, P.w13_wide, rows, st));
+            SwigluArgs sa{};
+            sa.y = h->ws; sa.ld = s.n13;
+            sa.h = h->h_p; sa.rows = rows; sa.I = s.I;
+            sa.interleaved = 1;
+            return launch_swiglu(sa, st);
+        }
+        case kPfW2: {
+            FSB_TRY(launch_rows_of(P.w2, rows, st));
+            ResidNormArgs r2{};
+            r2.y = h->ws; r2.ld = s.D;
+            r2.x_in = h->xres_p; r2.x_out = h->xres_p;
+            // the final norm is applied by the head GEMM's normalise-on-load on the last-token rows only
+            r2.norm_w = (l + 1 < s.nl) ? s.w[l + 1].attn_norm : nullptr;
+            r2.n_out = h->xn_p;
+            r2.rows = rows; r2.D = s.D; r2.eps = eps;
+            return launch_resid_norm(r2, st);
+        }
     }
+    set_error("prefill: no stage %d", stage);
+    return 1;
+}
+
+// On entry xn_p = attention_norm_0(xres_p) (prefill_embed).
+int run_stack_prefill(fsb_lm* h, int rows, const int* row_seq, const int* row_pos, cudaStream_t st) {
+    for (int l = 0; l < h->slow.nl; ++l)
+        for (int stage = kPfQkv; stage < kPfStages; ++stage)
+            FSB_TRY(prefill_stage(h, l, stage, rows, row_seq, row_pos, st));
     return 0;
 }
 
@@ -446,17 +491,6 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
     fe.rows = rows; fe.ncols = C + 1; fe.T_cap = c.max_frames;
     FSB_TRY(launch_frame_end(fe, st));
     return 0;
-}
-
-EmbedArgs embed_args(fsb_lm* h, const int* tokens, bf16* x, float* ssq, int rows) {
-    const fsb_lm_config& c = h->cfg;
-    EmbedArgs ea{};
-    ea.tokens = tokens;
-    ea.emb = h->emb; ea.cb_emb = h->cb_emb; ea.x = x; ea.ssq = ssq;
-    ea.rows = rows; ea.D = h->slow.D; ea.C = c.num_codebooks; ea.cs = c.codebook_size; ea.vocab = c.vocab_size;
-    ea.sem_begin = c.semantic_begin_id; ea.sem_end = c.semantic_end_id;
-    ea.scale = c.scale_codebook_embeddings;
-    return ea;
 }
 
 int decode_one_frame(fsb_lm* h, int batch, const fsb_sampling& sp, cudaStream_t st) {
@@ -573,7 +607,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
             return 1;            \
         }                        \
     } while (0)
-    TRYC(dalloc(h, &h->ws, h->ws_floats));
+    TRYC(dalloc(h, &h->ws, h->ws_floats, "ws_prefill"));
     TRYC(dalloc(h, &h->step_ws, h->step_ws_floats));
     TRYC(dalloc(h, &s.xres, static_cast<size_t>(RT) * s.D, "x_slow"));
     TRYC(dalloc(h, &s.ssq, static_cast<size_t>(RT) * kSsqStride, "ssq_slow"));
@@ -588,11 +622,11 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
                     "attn_span_ws"));
     TRYC(dalloc(h, &h->attn_d, static_cast<size_t>(RT) * Qm, "attn"));
     TRYC(dalloc(h, &h->h_d, static_cast<size_t>(RT) * Im, "ffn_h"));
-    TRYC(dalloc(h, &h->xres_p, static_cast<size_t>(R) * s.D));
-    TRYC(dalloc(h, &h->xn_p, static_cast<size_t>(R) * s.D));
-    TRYC(dalloc(h, &h->q_p, static_cast<size_t>(R) * s.H * s.Dh));
-    TRYC(dalloc(h, &h->attn_p, static_cast<size_t>(R) * s.H * s.Dh));
-    TRYC(dalloc(h, &h->h_p, static_cast<size_t>(R) * s.I));
+    TRYC(dalloc(h, &h->xres_p, static_cast<size_t>(R) * s.D, "x_prefill"));
+    TRYC(dalloc(h, &h->xn_p, static_cast<size_t>(R) * s.D, "xn_prefill"));
+    TRYC(dalloc(h, &h->q_p, static_cast<size_t>(R) * s.H * s.Dh, "q_prefill"));
+    TRYC(dalloc(h, &h->attn_p, static_cast<size_t>(R) * s.H * s.Dh, "attn_prefill"));
+    TRYC(dalloc(h, &h->h_p, static_cast<size_t>(R) * s.I, "h_prefill"));
     s.kv_page_ld = cdiv(s.S, kKvPage);
     s.n_pages = cfg->kv_pages > 0 ? cfg->kv_pages : cfg->max_batch * s.kv_page_ld;
     s.cache_layer_stride = static_cast<size_t>(s.n_pages) * s.Hkv * kKvPage * s.Dh;
@@ -714,13 +748,8 @@ int fsb_lm_prefill(fsb_lm* h, const int32_t* d_tokens, const int32_t* d_row_slot
     FSB_CHECK(rows >= 1 && rows <= std::max(c.max_rows, 128), "prefill: rows=%d exceeds max_rows=%d", rows, c.max_rows);
     FSB_CHECK(nseq >= 1 && nseq <= c.max_batch, "prefill: nseq=%d out of range", nseq);
     Stack& s = h->slow;
-    FSB_TRY(launch_embed(embed_args(h, d_tokens, h->xres_p, nullptr, rows), st));
-    ResidNormArgs r{};
-    r.x_in = h->xres_p;
-    r.norm_w = s.w[0].attn_norm; r.n_out = h->xn_p;
-    r.rows = rows; r.D = s.D; r.eps = c.norm_eps;
-    FSB_TRY(launch_resid_norm(r, st));
-    FSB_TRY(run_stack_prefill(h, s, rows, d_row_slot, d_row_pos, st));
+    FSB_TRY(prefill_embed(h, d_tokens, rows, st));
+    FSB_TRY(run_stack_prefill(h, rows, d_row_slot, d_row_pos, st));
     if (!do_sample) return 0;
     FSB_CHECK(sp != nullptr || h->slot_control, "prefill: sampling parameters required");
     const fsb_sampling sp_none{1.f, 1.f, 1, 0};
@@ -932,6 +961,23 @@ int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only
     const StepGemmPlan& qkv = s.dec[layer].qkv;
     FSB_TRY(step_gemm_launch(qkv, rows, st));
     return launch_decode_attn(h, s, layer, qkv, rows, h->iota, h->pos, kv_only != 0, st);
+}
+
+int fsb_lm_test_prefill_stage(fsb_lm* h, int layer, int stage, int rows, const int32_t* d_tokens,
+                              const int32_t* d_row_seq, const int32_t* d_row_pos, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(h != nullptr, "test_prefill_stage: null handle");
+    const int R = std::max(h->cfg.max_rows, 128);
+    FSB_CHECK(stage >= kPfEmbed && stage < kPfStages, "test_prefill_stage: stage=%d outside [0, %d)", stage, kPfStages);
+    FSB_CHECK(rows >= 1 && rows <= R, "test_prefill_stage: rows=%d outside [1, %d]", rows, R);
+    if (stage == kPfEmbed) {
+        FSB_CHECK(d_tokens != nullptr, "test_prefill_stage: the embed stage needs tokens");
+        return prefill_embed(h, d_tokens, rows, st);
+    }
+    FSB_CHECK(layer >= 0 && layer < h->slow.nl, "test_prefill_stage: layer=%d outside [0, %d)", layer, h->slow.nl);
+    FSB_CHECK((stage != kPfQkv && stage != kPfAttn) || (d_row_seq != nullptr && d_row_pos != nullptr),
+              "test_prefill_stage: stage %d needs the rows' sequences and positions", stage);
+    return prefill_stage(h, layer, stage, rows, d_row_seq, d_row_pos, st);
 }
 
 int fsb_lm_test_sample(fsb_lm* h, int fast, int cb_index, int rows, const int32_t* d_row_slot, const float* d_logits,

@@ -382,6 +382,7 @@ class LmEngine:
         c = self.cfg
         C1 = c.num_codebooks + 1
         rt = self.row_tile
+        R = max(self.max_rows, 128)
         shapes = {
             "out_tokens": ((self.max_batch, C1, self.max_frames), "<i4"),
             "n_out": ((self.max_batch,), "<i4"),
@@ -416,6 +417,14 @@ class LmEngine:
             "v_slow": ((c.n_layer, self._K.kv_pages, c.n_local_heads, KV_PAGE, c.head_dim), "<u2"),
             "k_fast": ((c.n_fast_layer, self.max_batch, c.fast_n_local_heads, c.num_codebooks, c.fast_head_dim), "<u2"),
             "v_fast": ((c.n_fast_layer, self.max_batch, c.fast_n_local_heads, c.num_codebooks, c.fast_head_dim), "<u2"),
+            # prefill workspaces (include/fishb200.h fsb_lm_test_prefill_stage), R = max(max_rows, 128) token rows;
+            # "ws_prefill" is flat: the last prefill GEMM's fp32 result [rows][n_out] at row stride n_out
+            "x_prefill": ((R, c.dim), "<u2"),
+            "xn_prefill": ((R, c.dim), "<u2"),
+            "q_prefill": ((R, c.n_head, c.head_dim), "<u2"),
+            "attn_prefill": ((R, c.n_head * c.head_dim), "<u2"),
+            "h_prefill": ((R, c.intermediate_size), "<u2"),
+            "ws_prefill": ((nbytes.value // 4,), "<f4"),
         }
         shape, ts = shapes[name]
         with torch.cuda.device(self.device):
@@ -472,6 +481,23 @@ class LmEngine:
         _lib.check(self.lib.fsb_lm_test_sample(self.h, int(codebook > 0), int(codebook), logits.shape[0],
                                                None if rs is None else rs.data_ptr(), logits.data_ptr(),
                                                int(bool(use_ras)), None if sp is None else C.byref(sp), _stream()))
+
+    PREFILL_STAGES = ("embed", "qkv", "attn", "wo", "w13", "w2")
+
+    def test_prefill_stage(self, stage: str, rows: int, layer: int = 0, tokens: Optional[torch.Tensor] = None,
+                           row_seq: Optional[torch.Tensor] = None, row_pos: Optional[torch.Tensor] = None):
+        """Test hook (include/fishb200.h fsb_lm_test_prefill_stage): one stage of slow layer `layer` of the prefill
+        over `rows` token rows, on the prefill buffers as they are. tokens int32 [rows][C+1] (embed); row_seq / row_pos
+        int32 [rows] (qkv, attn). Returns after the stage has finished."""
+        def dev(t):
+            return None if t is None else t.to(device=self.device, dtype=torch.int32).contiguous()
+
+        tok, seq, pos = dev(tokens), dev(row_seq), dev(row_pos)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.fsb_lm_test_prefill_stage(
+                self.h, int(layer), self.PREFILL_STAGES.index(stage), int(rows), *(
+                    None if t is None else t.data_ptr() for t in (tok, seq, pos)), _stream()))
+            torch.cuda.current_stream().synchronize()
 
     # ---- paged slow KV cache (KvPagePool) --------------------------------------------------------------------------
     def _forget_slot(self, slot: int):

@@ -211,7 +211,13 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
  *   stride H*Dh), "ffn_h" bf16 [RT * max I] (the w2 operand: rows at stride I of the stack being run);
  *   the KV caches (for fsb_lm_test_layer_attn and the copy tests): "k_slow" / "v_slow" bf16
  *   [n_layer][kv_pages][n_kv_head][64][head_dim] (the page pool), "k_fast" / "v_fast" bf16
- *   [n_fast_layer][max_batch][fast_n_kv_head][num_codebooks][fast_head_dim] (one contiguous block per slot) */
+ *   [n_fast_layer][max_batch][fast_n_kv_head][num_codebooks][fast_head_dim] (one contiguous block per slot);
+ *   the prefill workspaces (for fsb_lm_test_prefill_stage), R = max(max_rows, 128) token rows: "x_prefill" /
+ *   "xn_prefill" bf16 [R][dim] (the residual stream and its normed copy, the next GEMM's operand), "q_prefill" bf16
+ *   [R][n_head][head_dim], "attn_prefill" bf16 [R][n_head*head_dim], "h_prefill" bf16 [R][intermediate] and
+ *   "ws_prefill" f32, flat: the fp32 result of the prefill GEMM run last, [rows][n_out] at a row stride of n_out
+ *   ((n_head + 2 n_kv_head) * head_dim for qkv, dim for wo and w2, ceil(intermediate / 64) * 128 for w1|w3, whose
+ *   columns are in the interleaved row order of the fused matrix) */
 int fsb_lm_buffer(fsb_lm* h, const char* name, void** d_ptr, size_t* bytes);
 
 /* Measurement hook for bench.py: launch every weight-streaming step GEMM of one decode frame `reps` times
@@ -452,6 +458,22 @@ int fsb_lm_test_layer_gemms(fsb_lm* h, int fast, int layer, int rows, int upto, 
  * row. kv_only != 0 stops after the append, as the fast stack's pass 0 does. Outputs: "attn" (rows at stride H*Dh)
  * and the caches "k_*" / "v_*". rows in [1, max_batch]. */
 int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only, void* stream);
+
+/* Runs one stage of slow layer `layer` of the prefill for `rows` token rows exactly as fsb_lm_prefill does (the
+ * handle's own plans, the narrow / wide GEMM choice, the "kv_page" table and the context bound), on the fsb_lm_buffer
+ * prefill workspaces as the caller left them:
+ *   stage 0 (embed; `layer` ignored): d_tokens int32 [rows][C+1] -> "x_prefill", "xn_prefill" (attention_norm of 0)
+ *   stage 1 (qkv): qkv GEMM of "xn_prefill" -> "ws_prefill"; bias, qk-norm, RoPE -> "q_prefill" and the K/V of each
+ *           row appended at (d_row_seq[i], d_row_pos[i]) through the page table ("k_slow" / "v_slow")
+ *   stage 2 (attention): "q_prefill" against the caches -> "attn_prefill" (a row whose history has an unmapped page
+ *           reads zeros)
+ *   stage 3 (wo): wo GEMM of "attn_prefill" -> "ws_prefill"; "x_prefill" += it + bo; "xn_prefill" = ffn_norm(x)
+ *   stage 4 (w1|w3): GEMM of "xn_prefill" -> "ws_prefill"; SwiGLU -> "h_prefill"
+ *   stage 5 (w2): w2 GEMM of "h_prefill" -> "ws_prefill"; "x_prefill" += it; "xn_prefill" = the next layer's
+ *           attention_norm(x), untouched on the last layer.
+ * d_row_seq / d_row_pos int32 [rows] (stages 1 and 2). rows in [1, max(max_rows, 128)]. */
+int fsb_lm_test_prefill_stage(fsb_lm* h, int layer, int stage, int rows, const int32_t* d_tokens,
+                              const int32_t* d_row_seq, const int32_t* d_row_pos, void* stream);
 
 /* Runs the sampler (csrc/lm_kernels.cu sample_kernel) on its own for `rows` batch rows, with the arguments a decode
  * frame gives it: the slow head's (fast = 0, cb_index = 0; use_ras != 0 as in a decode frame, 0 as in the prefill's) or

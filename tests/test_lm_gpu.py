@@ -194,18 +194,43 @@ def test_batch_invariance_and_ragged_prompts():
         assert dec >= 0.6 * n * cfg.num_codebooks, f"seq {i}: {eq}/{n} frames identical, {ties} near-ties, {dec} decisions"
 
 
+class _PrefillCalls:
+    """Stands in for an engine's library handle and counts its fsb_lm_prefill calls (one per prefill pass)."""
+
+    def __init__(self, lib):
+        self._lib, self.calls = lib, 0
+
+    def __getattr__(self, name):
+        f = getattr(self._lib, name)
+        if name != "fsb_lm_prefill":
+            return f
+
+        def counted(*args):
+            self.calls += 1
+            return f(*args)
+        return counted
+
+
 def test_prefill_chunking_equals_single_pass():
-    """max_rows smaller than the prompt: time-split prefill must give the same continuation."""
-    cfg = O.tiny_config()
+    """max_rows smaller than the prompt: a 150-row prompt prefilled 48 rows at a time (pieces start at 48, 96 and 144,
+    so the page edges at 64 and 128 fall inside pieces) must give the continuation of a single pass."""
+    cfg = O.tiny_config(max_seq_len=256)
     w = O.make_weights(cfg, seed=41, head_gain=8.0)
-    p = make_prompt(cfg, 41, 70)
-    a = _gen(build_model(cfg, w, max_rows=2048), p, 6, temperature=0.7, top_p=0.7, top_k=1)
-    b = _gen(build_model(cfg, w, max_rows=128), p, 6, temperature=0.7, top_p=0.7, top_k=1)  # 70 < 128: one pass
+    T = 150
+    p = make_prompt(cfg, 41, T)
+    passes = []
+    for max_rows in (2048, 48):
+        model = build_model(cfg, w, max_rows=max_rows)
+        model.engine.lib = calls = _PrefillCalls(model.engine.lib)
+        passes.append((_gen(model, p, 6, temperature=0.7, top_p=0.7, top_k=1), calls.calls))
+        model.engine.close()
+    (a, n_one), (b, n_chunked) = passes
+    assert n_one == 1 and n_chunked == 4, f"prefill passes: {n_one} with max_rows 2048, {n_chunked} with 48"
     assert torch.equal(a, b)
     st = O.setup(cfg, w)
     traces = []
     ref = O.generate(st, p, 6, temperature=0.7, top_p=0.7, top_k=1, traces=traces, noise=False)
-    assert_tokens_match(a, ref, traces, cfg, 70, "chunked prefill")
+    assert_tokens_match(a, ref, traces, cfg, T, "chunked prefill")
 
 
 def test_s2pro_layer_geometry_greedy():

@@ -218,6 +218,15 @@ def batch_encode(model, audios_list: Sequence) -> list[torch.Tensor]:
     return [f[..., : int(n)] for f, n in zip(features, feature_lengths)]
 
 
+@torch.inference_mode()
+def batch_vqgan_decode(model, features: Sequence) -> list[np.ndarray]:
+    """tools/server/model_utils.py:59-86: codes of several utterances ([1 + n_codebooks, T_i] each, any integer dtype)
+    -> per item its waveform, float32 numpy [1, T_i * frame_length], in input order. Instead of padded micro-batches,
+    the items share `model.from_indices_list`'s decode pool, each bit-identical to `model.from_indices` of that item
+    alone. A malformed item raises ValueError naming it."""
+    return [w.cpu().numpy()[None] for w in model.from_indices_list(features)]
+
+
 def encode_files(files: Sequence[Path], model, batch_size: int = 64, max_batch_seconds: float = 1800.0,
                  reader: Callable[[Path], tuple[torch.Tensor, int]] = read_audio, prefetch: int = 2,
                  progress: Optional[Callable[[int, float], None]] = None) -> tuple[int, float]:

@@ -22,7 +22,7 @@ import math
 import threading
 from dataclasses import dataclass, field
 from types import MappingProxyType
-from typing import Iterator, Mapping, Optional
+from typing import Iterator, Mapping, Optional, Sequence
 
 import torch
 
@@ -117,6 +117,7 @@ class DAC:
         self._bufs: dict = {}
         self._graphs: dict = {}   # (B, S, T) -> (CUDAGraph, static index buffer, static waveform) of from_indices
         self._graph_seen: dict = {}
+        self._dec_pool: Optional["DecodeStreamPool"] = None  # the streamed from_indices' pool, opened on first use
         self._ws_gen = 0  # bumped whenever a workspace or the RoPE table is re-allocated (stream pools drop their graphs)
         # decoder ResidualUnits as one kernel each (csrc/codec_resunit.cu); False = two conv GEMM launches per unit
         self._fused_units = True
@@ -437,12 +438,23 @@ class DAC:
     # -------------------------------------------------------------------------------------------
     # decode
     # -------------------------------------------------------------------------------------------
+    # from_indices decodes through a DecodeStreamPool when the one-shot pass would not fit (see from_indices): this many
+    # batch rows side by side, in pieces of this many frames (about 12 s at 44.1 kHz). Measured on an H100 (700 W,
+    # tools/decode_long.py, BASELINE.md): at 5 minutes, 256-frame pieces decode one row 18 % faster than 128-frame ones
+    # (0.77 GB peak), and four rows 5 % faster at 2.8 GB; 512 frames gain 9 % for one row and nothing for four, at
+    # twice the memory.
+    DECODE_STREAM_FRAMES = 256
+    DECODE_STREAM_SLOTS = 4
+
     @torch.inference_mode()
     def from_indices(self, indices: torch.Tensor) -> torch.Tensor:
         """modded_dac.py:925-927: codes [B, 1+n_codebooks, T] -> waveform [B, 1, T*frame_length] (fp32).
         Like the reference (rvq.py:354-359) the caller's tensor is clamped in place.
         The ~190 launches of one decode are captured into a CUDA graph the second time a (B, T) shape is seen and
-        replayed from then on: the layer walk below costs more host time than the GPU needs for short utterances."""
+        replayed from then on: the layer walk below costs more host time than the GPU needs for short utterances.
+        When the one-shot pass's workspaces fit in free device memory and its post-transformer rows (B x T) fit its
+        launches (ONE_SHOT_MAX_ROWS), it runs as it always has; otherwise the batch is decoded through a
+        DecodeStreamPool in pieces of DECODE_STREAM_FRAMES frames, in bounded memory and with the same samples."""
         cfg = self.cfg
         # one caller at a time per DAC object: the layers share persistent workspaces (the reference's nn.Module
         # allocates per call and may be driven from two host threads, e.g. TTSInferenceEngine + a batch encoder)
@@ -457,6 +469,11 @@ class DAC:
                 g_idx.copy_(indices.reshape(-1))
                 graph.replay()
                 return g_wav.clone().view(B, 1, -1)
+            # only a shape without a captured graph pays for the memory probe: one with a graph fit in one shot
+            need = self._decode_one_shot_bytes(B, T)
+            fits = need + need // 20 + self.ONE_SHOT_MARGIN_BYTES <= self._free_device_bytes()
+            if not fits or B * T > self.ONE_SHOT_MAX_ROWS:
+                return self._from_indices_streamed(indices)
             seen = self._graph_seen.get(key, 0)
             self._graph_seen[key] = seen + 1
             if seen == 0 or len(self._graphs) >= 4:
@@ -492,6 +509,88 @@ class DAC:
             cur = out
         return self._decoder(cur, B, Tc)
 
+    def _decode_one_shot_bytes(self, B: int, T: int) -> int:
+        """Bytes the one-shot from_indices of B x T frames would allocate: its int32 codes, the waveform and the copy a
+        graph replay returns, plus every named workspace that is not already large enough (a workspace that grows is
+        allocated before the old one is released). The decoder's three bf16 buffers (393 KB per frame each for the
+        S2-Pro geometry) dominate."""
+        cfg = self.cfg
+        D, rows = cfg.latent_dim, B * T
+        need = rows * self.n_stage * 4 + 2 * rows * self.frame_length * 4
+        need += self._grow_bytes("q_z", rows * D) + self._tfm_bytes(self.post_tfm["cfg"], rows)
+        Tc = T
+        for i, f in enumerate(reversed(cfg.downsample_factor)):
+            Tc *= f
+            need += self._grow_bytes(f"up_{i}", B * Tc * D)
+            need += self._grow_bytes("cnx_y", B * Tc * D) + self._grow_bytes("cnx_h", B * Tc * 4 * D)
+        return need + sum(self._grow_bytes(f"dec_{k}", self._decoder_numel(B, Tc)) for k in range(3))
+
+    def _from_indices_streamed(self, indices: torch.Tensor) -> torch.Tensor:
+        """from_indices of clamped codes through the decode pool, row by row, into one [B, 1, T*frame_length] output."""
+        B, _, T = indices.shape
+        wav = torch.empty(B, 1, T * self.frame_length, dtype=torch.float32, device=self._device)
+        codes = indices.to(device="cpu", dtype=torch.int32)
+        self._decode_streamed(list(codes), list(wav[:, 0]))
+        return wav
+
+    @torch.inference_mode()
+    def from_indices_list(self, codes: Sequence) -> list:
+        """Ragged batch decode: codes of any number of utterances, each [1+n_codebooks, T_i] of any integer dtype (torch
+        or numpy, T_i >= 1) -> per utterance its waveform fp32 [T_i * frame_length] on the device, in input order. Each
+        equals from_indices of that utterance alone, bit for bit. The utterances share the decode pool's slots: one
+        takes a slot as soon as an earlier one is done, so none is padded to a longer one beyond one push. Unlike
+        from_indices, the caller's codes are not modified."""
+        cfg, S = self.cfg, self.n_stage
+        items = []
+        for i, c in enumerate(codes):
+            c = torch.as_tensor(c)
+            if c.dtype.is_floating_point or c.dtype.is_complex or c.dtype == torch.bool:
+                raise ValueError(f"item {i}: codes must be integers, got {c.dtype}")
+            if c.ndim != 2 or c.shape[0] != S:
+                raise ValueError(f"item {i}: codes must be [{S}, frames], got {tuple(c.shape)}")
+            if c.shape[1] == 0:
+                raise ValueError(f"item {i}: no frames")
+            c = c.to(device="cpu", dtype=torch.int64)
+            items.append(torch.cat([c[:1].clamp(0, cfg.semantic_codebook_size - 1),  # rvq.py:354-359, on a copy
+                                    c[1:].clamp(0, cfg.codebook_size - 1)]).to(torch.int32))
+        with self._lock, torch.cuda.device(self._device):
+            outs = [torch.empty(c.shape[1] * self.frame_length, dtype=torch.float32, device=self._device) for c in items]
+            self._decode_streamed(items, outs)
+        return outs
+
+    def _decode_streamed(self, items: list, outs: list) -> None:
+        """Decode items[i] (clamped codes int32 [S, T_i] on the host) into outs[i] (fp32 [T_i * frame_length]) through
+        the decode pool: up to DECODE_STREAM_SLOTS items side by side, each pushed in pieces of up to
+        DECODE_STREAM_FRAMES frames; the next item takes the slot of one that is done."""
+        FL, k = self.frame_length, self.DECODE_STREAM_FRAMES
+        if self._dec_pool is None:  # kept: later calls replay the graphs it captured
+            self._dec_pool = self.open_stream_pool(self.DECODE_STREAM_SLOTS, k_max=k)
+        pool = self._dec_pool
+        todo = iter(range(len(items)))
+        live: dict = {}  # slot -> [item, frames decoded]
+        try:
+            while True:
+                while len(live) < pool.slots:
+                    i = next(todo, None)
+                    if i is None:
+                        break
+                    live[pool.open()] = [i, 0]
+                if not live:
+                    return
+                pieces = {s: items[i][:, f: f + k] for s, (i, f) in live.items()}
+                for s, wav in pool.push(pieces).items():
+                    i, f = live[s]
+                    n = pieces[s].shape[1]
+                    outs[i][f * FL: (f + n) * FL].copy_(wav)
+                    if f + n == items[i].shape[1]:
+                        pool.close(s)
+                        del live[s]
+                    else:
+                        live[s][1] = f + n
+        finally:
+            for s in live:
+                pool.close(s)
+
     def open_decode_stream(self, batch: int = 1, max_frames: int = 4096, conv_context: int = 16,
                            sample_rate: Optional[int] = None, sample_format: Optional[str] = None) -> "DecodeStream":
         """Incremental `from_indices` (SURVEY §8(f).3): push code frames as the LM emits them, get their samples back.
@@ -520,16 +619,19 @@ class DAC:
         return (self._fused_units and c7.taps == 7 and c1.taps == 1 and c7.bias is not None and c1.bias is not None
                 and c7.kpad == _pad64(c) and c1.kpad == _pad64(c) and bool(self.lib.fsb_res_unit_supported(c)))
 
+    def _decoder_numel(self, B: int, T: int) -> int:
+        """Elements of each of the decoder's buffers for B x T latent rows: its largest activation."""
+        cfg = self.cfg
+        numel = max(B * (T * math.prod(cfg.decoder_rates[: i + 1])) * (cfg.decoder_dim // 2 ** (i + 1))
+                    for i in range(len(cfg.decoder_rates)))
+        return max(numel, B * T * cfg.decoder_dim)
+
     def _decoder(self, z: torch.Tensor, B: int, T: int) -> torch.Tensor:
         """Decoder.forward (modded_dac.py:760-801) on z = flat [B][T][latent] bf16."""
         cfg = self.cfg
         c = cfg.decoder_dim
-        # largest activation: after the last transposed conv
         t_full = T * cfg.hop_length
-        numel = max(B * (T * math.prod(cfg.decoder_rates[: i + 1])) * (cfg.decoder_dim // 2 ** (i + 1))
-                    for i in range(len(cfg.decoder_rates)))
-        numel = max(numel, B * T * c)
-        bufs = [self._buf(f"dec_{k}", numel) for k in range(3)]
+        bufs = [self._buf(f"dec_{k}", self._decoder_numel(B, T)) for k in range(3)]
         free = [0, 1, 2]
 
         def take():
@@ -584,11 +686,13 @@ class DAC:
     # -------------------------------------------------------------------------------------------
     # encode
     # -------------------------------------------------------------------------------------------
-    # encode routes to the streamed path when its one-shot workspaces would not fit in free device memory with a margin
-    # of this plus 5 % of the estimate left over (the caching allocator's rounding, the small buffers the estimate omits)
-    ENCODE_MARGIN_BYTES = 512 << 20
+    # encode and from_indices route to the streamed path when their one-shot workspaces would not fit in free device
+    # memory with a margin of this plus 5 % of the estimate left over (the caching allocator's rounding, the small
+    # buffers the estimate omits)
+    ONE_SHOT_MARGIN_BYTES = 512 << 20
     # the transformers' row-wise glue kernels launch one CTA row per token row (grid.y), so one pass takes at most this
-    # many rows per transformer: for the S2-Pro encoder transformer (4 rows per frame) about 12.7 minutes of audio
+    # many rows per transformer: for the S2-Pro encoder transformer (4 rows per frame) about 12.7 minutes of audio, for
+    # the post-transformer of from_indices (1 row per frame) about 50 minutes
     ONE_SHOT_MAX_ROWS = 65535
     ENCODE_STREAM_FRAMES = 128  # frames per push of the streamed path (about 6 s at 44.1 kHz)
     ENCODE_STREAM_SLOTS = 4  # batch rows encoded side by side by the streamed path
@@ -605,7 +709,7 @@ class DAC:
             N = math.ceil(length / self.frame_length) * self.frame_length
             need = self._encode_one_shot_bytes(B, N)
             rows = max(r for _, r in self._encode_one_shot_tfm_rows(B, N))
-            fits = need + need // 20 + self.ENCODE_MARGIN_BYTES <= self._free_device_bytes()
+            fits = need + need // 20 + self.ONE_SHOT_MARGIN_BYTES <= self._free_device_bytes()
             if fits and rows <= self.ONE_SHOT_MAX_ROWS:
                 return self._encode_one_shot(audio_data, audio_lengths, n_quantizers)
             return self._encode_streamed(audio_data, audio_lengths, n_quantizers)
@@ -620,11 +724,7 @@ class DAC:
         named workspace that is not already large enough (a workspace that grows is allocated before the old one is
         released). The bf16 encoder activations (3 x B x N x encoder_dim) dominate."""
         cfg = self.cfg
-
-        def grow(name: str, numel: int, elt: int = 2, dtype=torch.bfloat16) -> int:
-            b = self._bufs.get(name)
-            return 0 if b is not None and b.numel() >= numel and b.dtype == dtype else max(numel, 1) * elt
-
+        grow = self._grow_bytes
         need = 2 * B * N * 4  # the padded fp32 waveform (and the input's conversion to it)
         need += sum(grow(f"enc_{k}", B * N * cfg.encoder_dim) for k in range(3))
         T = N // self.hop_length
@@ -634,13 +734,21 @@ class DAC:
             T //= f
             need += grow(f"down_{i}", B * T * D) + grow("cnx_y", B * T * D) + grow("cnx_h", B * T * 4 * D)
         for tf, rows in self._encode_one_shot_tfm_rows(B, N):
-            t: TfmConfig = tf["cfg"]
-            HD = t.n_head * t.head_dim
-            need += grow("tf_ws", rows * max(3 * HD, 2 * t.intermediate_size, t.dim), 4, torch.float32)
-            need += grow("tf_n", rows * t.dim) + sum(grow(f"tf_{k}", rows * HD) for k in ("q", "k", "v", "att"))
-            need += grow("tf_h", rows * t.intermediate_size) + 3 * rows * 4  # + row (sequence, position), arange
+            need += self._tfm_bytes(tf["cfg"], rows)
         need += B * self.n_stage * T * (4 + 8)  # int32 codes and their int64 copy
         return need
+
+    def _grow_bytes(self, name: str, numel: int, elt: int = 2, dtype=torch.bfloat16) -> int:
+        """Bytes `_buf(name, numel, dtype)` would allocate: 0 when the workspace is already large enough."""
+        b = self._bufs.get(name)
+        return 0 if b is not None and b.numel() >= numel and b.dtype == dtype else max(numel, 1) * elt
+
+    def _tfm_bytes(self, t: TfmConfig, rows: int) -> int:
+        """Bytes the workspaces of `_transformer` over `rows` rows would allocate."""
+        grow, HD = self._grow_bytes, t.n_head * t.head_dim
+        need = grow("tf_ws", rows * max(3 * HD, 2 * t.intermediate_size, t.dim), 4, torch.float32)
+        need += grow("tf_n", rows * t.dim) + sum(grow(f"tf_{k}", rows * HD) for k in ("q", "k", "v", "att"))
+        return need + grow("tf_h", rows * t.intermediate_size) + 3 * rows * 4  # + row (sequence, position), arange
 
     def _encode_one_shot_tfm_rows(self, B: int, N: int) -> list:
         """(transformer, rows) of every transformer the one-shot encode of B x N padded samples runs."""

@@ -75,6 +75,10 @@ def lib() -> C.CDLL:
     L.fsb_lm_destroy.restype = None
     L.fsb_lm_prefill.argtypes = [vp, vp, vp, vp, i32, vp, vp, i32, i32, C.POINTER(Sampling), vp]
     L.fsb_lm_decode.argtypes = [vp, i32, i32, C.POINTER(Sampling), i32, vp]
+    L.fsb_lm_set_decode_tile.argtypes = [vp, i32]
+    L.fsb_lm_decode_tile.argtypes = [vp]
+    L.fsb_lm_graph_captures.argtypes = [vp]
+    L.fsb_lm_graph_captures.restype = C.c_longlong
     L.fsb_lm_reset.argtypes = [vp, vp]
     L.fsb_lm_set_context_bound.argtypes = [vp, i32]
     L.fsb_lm_set_slot_control.argtypes = [vp, i32]

@@ -10,7 +10,9 @@
 //   decode state       residual streams x_slow / x_fast [RT][D] + their per-128-feature sums of squares
 //                      (fp32 [RT][32]); q / attention / SwiGLU operands [RT][*]; logits fp32 [max_batch][n]
 //   step_ws            fp32 stream-K partials of the step GEMMs: [slot][tile][RT rows][128 features]
-// RT = the decode row tile: 32 for max_batch <= 32 (the 32-row step GEMM), 64 above (the 64-row one).
+// RT = the decode row tile: 32 for max_batch <= 32 (the 32-row step GEMM), 64 above (the 64-row one). An RT = 64
+// engine also holds the 32-row plans of every step GEMM (same weights, same stream-K schedule, the first 32 rows of
+// the same operand buffers) and runs a frame of <= 32 rows on them: the same bits in less time.
 //   prefill workspaces [max_rows][*] operands + ws fp32 [max_rows][N]
 //
 // One decode frame (inference.py:96-181) = embed, 36 x {qkv GEMM (norm on load), attention (finishes qkv: bias /
@@ -55,7 +57,8 @@ struct Stack {
     bool qk_norm = false;
     int bf16_math = 0;
     std::vector<LayerW> w;
-    std::vector<StepLayer> dec;     // decode: fused step GEMMs
+    std::vector<StepLayer> dec;     // decode: fused step GEMMs at the engine's row tile RT
+    std::vector<StepLayer> dec32;   // RT = 64 only: the same GEMMs at the 32-row tile
     std::vector<PrefillLayer> pf;   // prefill: BN=128 tiles, fp32 result + consumer kernels (slow only)
     bf16 *kcache = nullptr, *vcache = nullptr;
     int* kv_page = nullptr;  // slow stack: page table [max_batch][kv_page_ld] of the paged cache; fast stack: contiguous
@@ -65,6 +68,26 @@ struct Stack {
     bf16* xres = nullptr;  // decode residual stream [RT][D]
     float* ssq = nullptr;  // its per-tile sums of squares [RT][kSsqStride]
 };
+
+// The step GEMM plans one decode frame runs: the engine's RT plans or, on an RT = 64 engine, the 32-row ones.
+struct FramePlans {
+    int tile;
+    const std::vector<StepLayer>* slow;
+    const std::vector<StepLayer>* fast;
+    const StepGemmPlan *head, *fast_out, *proj;
+    const StepFinalize* proj_out;
+};
+
+// One captured decode frame and what its capture depended on (fsb_lm_decode's graph cache).
+struct DecodeGraph {
+    cudaGraphExec_t exec = nullptr;
+    int batch = -1, tile = 0, lcap = -1, kernels = 0;
+    bool slot_control = false;
+    const float* noise = nullptr;
+    fsb_sampling sampling{};
+    unsigned long long used = 0;  // last use, for least-recently-used eviction
+};
+constexpr int kGraphCache = 16;  // captured frames kept per engine
 
 }  // namespace
 
@@ -77,7 +100,6 @@ struct fsb_lm {
     float* slot_top_p = nullptr;
     int* slot_top_k = nullptr;
     unsigned long long* slot_seed = nullptr;
-    bool graph_slot_control = false;
     fsb_lm_config cfg;
     int num_sms = 0;
     int step_ctas = 0;
@@ -89,6 +111,10 @@ struct fsb_lm {
     int head_rows = 0;
     StepGemmPlan head_plan, fast_out_plan, proj_plan;
     StepFinalize proj_out;  // fast_project_in's bias, no residual add, into the fast residual stream
+    StepGemmPlan head_plan32, fast_out_plan32, proj_plan32;  // RT = 64 only: the 32-row plans
+    StepFinalize proj_out32;
+    int force_tile = 0;      // fsb_lm_set_decode_tile: 0 = by the frame's row count, else 32 or 64
+    int last_tile = 0;       // row tile of the last decode frame
     bool has_proj = false;
     // decode workspaces
     bf16 *q_d = nullptr, *attn_d = nullptr, *h_d = nullptr, *hid_d = nullptr;
@@ -109,13 +135,10 @@ struct fsb_lm {
     const float* noise_u = nullptr;
     int noise_draws = 0, noise_ld = 0;
     int ctx_lcap = 0;  // score-buffer bound for the slow attention (0 = capacity)
-    int graph_lcap = -1;
-    // decode graph cache
-    cudaGraphExec_t graph_exec = nullptr;
-    int graph_batch = -1;
-    int graph_kernels = 0;  // kernels inside one captured frame
-    const float* graph_noise = nullptr;
-    fsb_sampling graph_sampling{};
+    // decode graph cache: one captured frame per (rows, tile, context bound, slot control, noise, sampling)
+    std::vector<DecodeGraph> graphs;
+    unsigned long long graph_uses = 0;
+    long long graph_captures = 0;
     std::vector<void*> owned;
     std::map<std::string, std::pair<void*, size_t>> named;
 };
@@ -178,21 +201,47 @@ int launch_rows_of(const GemmPlan& plan, const GemmPlan& wide, int rows, cudaStr
     return (rows >= 512 && tiles_wide >= 2 * sms) ? launch_rows_of(wide, rows, st) : launch_rows_of(plan, rows, st);
 }
 
-// Step GEMM over the weight `w` [n_out, K]; operand X = act, used as it is.
-int make_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, int K, const bf16* act) {
-    return step_plan_init(plan, w, n_out, K, act, false, h->rt, h->step_ctas, kStepStages, h->step_ws,
+// Step GEMM over the weight `w` [n_out, K]; operand X = act, used as it is. `rt`: the row tile, h->rt or (on an
+// RT = 64 engine) 32, whose plan reads the first 32 rows of the same operand buffer.
+int make_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, int K, const bf16* act, int rt) {
+    return step_plan_init(plan, w, n_out, K, act, false, rt, h->step_ctas, kStepStages, h->step_ws,
                           h->step_ws_floats);
 }
 
 // Step GEMM over the weight `w` [n_out, s.D]; operand X = stack s's residual stream, RMSNorm'd with norm_w on load.
-int make_norm_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, const Stack& s, const bf16* norm_w) {
-    FSB_TRY(step_plan_init(plan, w, n_out, s.D, s.xres, true, h->rt, h->step_ctas, kStepStages, h->step_ws,
+int make_norm_step_plan(fsb_lm* h, StepGemmPlan* plan, const bf16* w, int n_out, const Stack& s, const bf16* norm_w,
+                        int rt) {
+    FSB_TRY(step_plan_init(plan, w, n_out, s.D, s.xres, true, rt, h->step_ctas, kStepStages, h->step_ws,
                            h->step_ws_floats));
     plan->p.x_ssq = s.ssq;
     plan->p.norm_w = norm_w;
     plan->p.x_nt = cdiv(s.D, 128);
     plan->p.eps = h->cfg.norm_eps;
     return 0;
+}
+
+// A 32-row plan of an RT = 64 engine must cut its GEMM into the same stream-K ranges as the 64-row plan (the
+// schedule is a function of the unit count and the CTA count): then every output element is the same sum of the same
+// MMAs at either tile, and a frame's bits do not depend on which tile ran it.
+int check_same_schedule(const StepGemmPlan& a, const StepGemmPlan& b) {
+    FSB_CHECK(a.grid.x == b.grid.x && a.p.tiles == b.p.tiles && a.p.K == b.p.K && a.max_parts == b.max_parts,
+              "fsb_lm_create: the %d- and %d-row step GEMM plans of a %dx%d weight differ in schedule (%u vs %u CTAs, "
+              "%d vs %d partial slots)", a.rt, b.rt, a.p.n_out, a.p.K, a.grid.x, b.grid.x, a.max_parts, b.max_parts);
+    return 0;
+}
+
+FramePlans frame_plans(const fsb_lm* h, int tile) {
+    if (tile == h->rt)
+        return FramePlans{tile, &h->slow.dec, &h->fast.dec, &h->head_plan, &h->fast_out_plan, &h->proj_plan,
+                          &h->proj_out};
+    return FramePlans{tile, &h->slow.dec32, &h->fast.dec32, &h->head_plan32, &h->fast_out_plan32, &h->proj_plan32,
+                      &h->proj_out32};
+}
+
+// The row tile of a decode frame over `batch` rows: the forced one, else 32 where the engine has 32-row plans.
+int frame_tile(const fsb_lm* h, int batch) {
+    if (h->force_tile != 0) return h->force_tile;
+    return (h->rt == kStepRowsMax && batch <= kStepRows) ? kStepRows : h->rt;
 }
 
 SlotCtl slot_ctl(const fsb_lm* h) {
@@ -262,10 +311,10 @@ int run_layer_gemms(const StepLayer& P, int rows, int upto, cudaStream_t st) {
 
 // ---- decode: one transformer stack over the batch rows, eight kernels per layer: qkv GEMM, attention, then the
 // three (GEMM, finalize) pairs. ----
-int run_stack_decode(fsb_lm* h, Stack& s, int rows, const int* row_seq, const int* row_pos, bool stop_after_kv,
-                     cudaStream_t st) {
+int run_stack_decode(fsb_lm* h, Stack& s, const std::vector<StepLayer>& dec, int rows, const int* row_seq,
+                     const int* row_pos, bool stop_after_kv, cudaStream_t st) {
     for (int l = 0; l < s.nl; ++l) {
-        StepLayer& P = s.dec[l];
+        const StepLayer& P = dec[l];
         FSB_TRY(step_gemm_launch(P.qkv, rows, st));
         const bool kv_only = stop_after_kv && l == s.nl - 1;  // fast pass 0 only fills the KV cache (inference.py:147)
         FSB_TRY(launch_decode_attn(h, s, l, P.qkv, rows, row_seq, row_pos, kv_only, st));
@@ -431,17 +480,17 @@ SampleArgs frame_sample_args(const fsb_lm* h, int p, const StepPartials& parts, 
 }
 
 // Head + sampling + fast passes + bookkeeping for `rows` sequences whose last residual-stream rows (un-normed)
-// are in slow.xres[0..rows) with their sums of squares in slow.ssq. inference.py:114-181.
-int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const int* set_pos_rows,
-                   const int* row_pos_src, const fsb_sampling& sp, cudaStream_t st) {
+// are in slow.xres[0..rows) with their sums of squares in slow.ssq, on the plans `fp`. inference.py:114-181.
+int run_frame_tail(fsb_lm* h, const FramePlans& fp, int rows, const int* row_slot, bool use_ras,
+                   const int* set_pos_rows, const int* row_pos_src, const fsb_sampling& sp, cudaStream_t st) {
     const fsb_lm_config& c = h->cfg;
     const int C = c.num_codebooks;
     const int* slots = row_slot ? row_slot : h->iota;
     Stack& s = h->slow;
     Stack& f = h->fast;
     // ---- slow head over the selectable rows (the final norm is applied on load) ----
-    FSB_TRY(step_gemm_launch(h->head_plan, rows, st));
-    FSB_TRY(launch_sample(frame_sample_args(h, 0, step_plan_partials(h->head_plan), rows, row_slot, use_ras, sp), st));
+    FSB_TRY(step_gemm_launch(*fp.head, rows, st));
+    FSB_TRY(launch_sample(frame_sample_args(h, 0, step_plan_partials(*fp.head), rows, row_slot, use_ras, sp), st));
 
     // ---- fast pass 0 input: hidden = norm(x) (norm_fastlayer_input) [-> fast_project_in]  (llama.py:459-461, 819-828)
     RowsArgs hr{};
@@ -452,8 +501,8 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
     if (h->has_proj) {
         hr.y = h->hid_d;
         FSB_TRY(launch_rows(hr, st));
-        FSB_TRY(step_gemm_launch(h->proj_plan, rows, st));  // fast_project_in
-        FSB_TRY(step_finalize_launch(h->proj_out, rows, st));
+        FSB_TRY(step_gemm_launch(*fp.proj, rows, st));  // fast_project_in
+        FSB_TRY(step_finalize_launch(*fp.proj_out, rows, st));
     } else {
         hr.y = f.xres;
         hr.ssq = f.ssq;
@@ -472,10 +521,10 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
             er.rows = rows; er.D = f.D; er.eps = c.norm_eps;
             FSB_TRY(launch_rows(er, st));
         }
-        FSB_TRY(run_stack_decode(h, f, rows, slots, h->fpos + p * h->rt, p == 0, st));
+        FSB_TRY(run_stack_decode(h, f, *fp.fast, rows, slots, h->fpos + p * h->rt, p == 0, st));
         if (p == 0) continue;
-        FSB_TRY(step_gemm_launch(h->fast_out_plan, rows, st));
-        FSB_TRY(launch_sample(frame_sample_args(h, p, step_plan_partials(h->fast_out_plan), rows, row_slot, false, sp),
+        FSB_TRY(step_gemm_launch(*fp.fast_out, rows, st));
+        FSB_TRY(launch_sample(frame_sample_args(h, p, step_plan_partials(*fp.fast_out), rows, row_slot, false, sp),
                               st));
     }
     FrameEndArgs fe{};
@@ -493,11 +542,13 @@ int run_frame_tail(fsb_lm* h, int rows, const int* row_slot, bool use_ras, const
     return 0;
 }
 
-int decode_one_frame(fsb_lm* h, int batch, const fsb_sampling& sp, cudaStream_t st) {
+// One frame over rows [0, batch) on the plans of row tile `tile` (batch <= tile).
+int decode_one_frame(fsb_lm* h, int batch, int tile, const fsb_sampling& sp, cudaStream_t st) {
     Stack& s = h->slow;
+    const FramePlans fp = frame_plans(h, tile);
     FSB_TRY(launch_embed(embed_args(h, h->cur_tok, s.xres, s.ssq, batch), st));
-    FSB_TRY(run_stack_decode(h, s, batch, h->iota, h->pos, false, st));
-    return run_frame_tail(h, batch, nullptr, true, nullptr, nullptr, sp, st);
+    FSB_TRY(run_stack_decode(h, s, *fp.slow, batch, h->iota, h->pos, false, st));
+    return run_frame_tail(h, fp, batch, nullptr, true, nullptr, nullptr, sp, st);
 }
 
 size_t step_ws_bound(int n_out, int ctas, int rt) {
@@ -674,20 +725,36 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
         }
     }
     // ---- GEMM plans, and the finalize after each GEMM whose consumer is another GEMM ----
+    // the decode plans of one layer at row tile `rt`
+    auto build_step = [&](Stack& st, StepLayer& P, const LayerW& lw, int rt) -> int {
+        const int Nqkv = (st.H + 2 * st.Hkv) * st.Dh;
+        FSB_TRY(make_norm_step_plan(h, &P.qkv, lw.wqkv, Nqkv, st, lw.attn_norm, rt));
+        FSB_TRY(make_step_plan(h, &P.wo, lw.wo, st.D, st.H * st.Dh, h->attn_d, rt));
+        P.wo_out = step_finalize_resid(P.wo, lw.bo, st.xres, st.xres, st.ssq);
+        FSB_TRY(make_norm_step_plan(h, &P.w13, lw.w13, st.n13, st, lw.ffn_norm, rt));
+        P.w13_out = step_finalize_swiglu(P.w13, h->h_d, st.I);
+        FSB_TRY(make_step_plan(h, &P.w2, lw.w2, st.D, st.I, h->h_d, rt));
+        P.w2_out = step_finalize_resid(P.w2, nullptr, st.xres, st.xres, st.ssq);
+        return 0;
+    };
+    const bool two_tiles = RT == kStepRowsMax;
     auto build = [&](Stack& st, bool with_prefill) -> int {
         st.dec.resize(st.nl);
+        if (two_tiles) st.dec32.resize(st.nl);
         if (with_prefill) st.pf.resize(st.nl);
         const int Nqkv = (st.H + 2 * st.Hkv) * st.Dh;
         for (int l = 0; l < st.nl; ++l) {
             const LayerW& lw = st.w[l];
             StepLayer& P = st.dec[l];
-            FSB_TRY(make_norm_step_plan(h, &P.qkv, lw.wqkv, Nqkv, st, lw.attn_norm));
-            FSB_TRY(make_step_plan(h, &P.wo, lw.wo, st.D, st.H * st.Dh, h->attn_d));
-            P.wo_out = step_finalize_resid(P.wo, lw.bo, st.xres, st.xres, st.ssq);
-            FSB_TRY(make_norm_step_plan(h, &P.w13, lw.w13, st.n13, st, lw.ffn_norm));
-            P.w13_out = step_finalize_swiglu(P.w13, h->h_d, st.I);
-            FSB_TRY(make_step_plan(h, &P.w2, lw.w2, st.D, st.I, h->h_d));
-            P.w2_out = step_finalize_resid(P.w2, nullptr, st.xres, st.xres, st.ssq);
+            FSB_TRY(build_step(st, P, lw, RT));
+            if (two_tiles) {
+                StepLayer& Q = st.dec32[l];
+                FSB_TRY(build_step(st, Q, lw, kStepRows));
+                FSB_TRY(check_same_schedule(Q.qkv, P.qkv));
+                FSB_TRY(check_same_schedule(Q.wo, P.wo));
+                FSB_TRY(check_same_schedule(Q.w13, P.w13));
+                FSB_TRY(check_same_schedule(Q.w2, P.w2));
+            }
             if (with_prefill) {
                 FSB_TRY(make_prefill_plan(h, &st.pf[l].qkv, lw.wqkv, Nqkv, st.D, h->xn_p, R));
                 FSB_TRY(make_prefill_plan(h, &st.pf[l].wo, lw.wo, st.D, st.H * st.Dh, h->attn_p, R));
@@ -701,11 +768,23 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     };
     TRYC(build(s, true));
     TRYC(build(f, false));
-    TRYC(make_norm_step_plan(h, &h->head_plan, h->head_w, h->head_rows, s, h->norm_w));
-    TRYC(make_norm_step_plan(h, &h->fast_out_plan, h->fast_out_w, cfg->codebook_size, f, h->fast_norm_w));
+    TRYC(make_norm_step_plan(h, &h->head_plan, h->head_w, h->head_rows, s, h->norm_w, RT));
+    TRYC(make_norm_step_plan(h, &h->fast_out_plan, h->fast_out_w, cfg->codebook_size, f, h->fast_norm_w, RT));
     if (h->has_proj) {
-        TRYC(make_step_plan(h, &h->proj_plan, h->fast_proj_w, f.D, s.D, h->hid_d));
+        TRYC(make_step_plan(h, &h->proj_plan, h->fast_proj_w, f.D, s.D, h->hid_d, RT));
         h->proj_out = step_finalize_resid(h->proj_plan, h->fast_proj_b, nullptr, f.xres, f.ssq);
+    }
+    if (two_tiles) {
+        TRYC(make_norm_step_plan(h, &h->head_plan32, h->head_w, h->head_rows, s, h->norm_w, kStepRows));
+        TRYC(check_same_schedule(h->head_plan32, h->head_plan));
+        TRYC(make_norm_step_plan(h, &h->fast_out_plan32, h->fast_out_w, cfg->codebook_size, f, h->fast_norm_w,
+                                 kStepRows));
+        TRYC(check_same_schedule(h->fast_out_plan32, h->fast_out_plan));
+        if (h->has_proj) {
+            TRYC(make_step_plan(h, &h->proj_plan32, h->fast_proj_w, f.D, s.D, h->hid_d, kStepRows));
+            TRYC(check_same_schedule(h->proj_plan32, h->proj_plan));
+            h->proj_out32 = step_finalize_resid(h->proj_plan32, h->fast_proj_b, nullptr, f.xres, f.ssq);
+        }
     }
 #undef TRYC
     *out = h;
@@ -714,9 +793,10 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
 
 void fsb_lm_destroy(fsb_lm* h) {
     if (!h) return;
-    if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+    for (DecodeGraph& g : h->graphs) cudaGraphExecDestroy(g.exec);
     auto free_plans = [](Stack& st) {
         for (auto& p : st.dec) { step_plan_free(&p.qkv); step_plan_free(&p.wo); step_plan_free(&p.w13); step_plan_free(&p.w2); }
+        for (auto& p : st.dec32) { step_plan_free(&p.qkv); step_plan_free(&p.wo); step_plan_free(&p.w13); step_plan_free(&p.w2); }
         for (auto& p : st.pf) { gemm_plan_free(&p.qkv); gemm_plan_free(&p.wo); gemm_plan_free(&p.w13); gemm_plan_free(&p.w2); gemm_plan_free(&p.qkv_wide); gemm_plan_free(&p.w13_wide); }
     };
     free_plans(h->slow);
@@ -724,6 +804,9 @@ void fsb_lm_destroy(fsb_lm* h) {
     step_plan_free(&h->head_plan);
     step_plan_free(&h->fast_out_plan);
     if (h->has_proj) step_plan_free(&h->proj_plan);
+    step_plan_free(&h->head_plan32);
+    step_plan_free(&h->fast_out_plan32);
+    step_plan_free(&h->proj_plan32);
     for (void* p : h->owned) cudaFree(p);
     delete h;
 }
@@ -764,7 +847,7 @@ int fsb_lm_prefill(fsb_lm* h, const int32_t* d_tokens, const int32_t* d_row_slot
     g.rows = nseq; g.D = s.D; g.eps = c.norm_eps;
     FSB_TRY(launch_rows(g, st));
     // the reference resets the RAS window per generate() call and prefill uses no RAS
-    return run_frame_tail(h, nseq, d_slots, false, d_last_rows, d_row_pos, *sp, st);
+    return run_frame_tail(h, frame_plans(h, h->rt), nseq, d_slots, false, d_last_rows, d_row_pos, *sp, st);
 }
 
 int fsb_lm_set_slot_control(fsb_lm* h, int enable) {
@@ -819,19 +902,26 @@ int fsb_lm_decode(fsb_lm* h, int batch, int nframes, const fsb_sampling* sp, int
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     FSB_CHECK(batch >= 1 && batch <= h->cfg.max_batch, "decode: batch=%d out of range", batch);
     FSB_CHECK(sp != nullptr || h->slot_control, "decode: sampling parameters required");
+    const int tile = frame_tile(h, batch);
+    FSB_CHECK(batch <= tile, "decode: batch=%d does not fit the forced %d-row tile", batch, tile);
     const fsb_sampling sp_none{1.f, 1.f, 1, 0};
     if (sp == nullptr || h->slot_control) sp = &sp_none;  // per-slot parameters: one graph for every mix of requests
+    h->last_tile = tile;
     if (!use_graph) {
-        for (int i = 0; i < nframes; ++i) FSB_TRY(decode_one_frame(h, batch, *sp, st));
+        for (int i = 0; i < nframes; ++i) FSB_TRY(decode_one_frame(h, batch, tile, *sp, st));
         return 0;
     }
-    const bool same = h->graph_exec && h->graph_batch == batch && h->graph_lcap == h->ctx_lcap &&
-                      h->graph_slot_control == h->slot_control && h->graph_noise == h->noise_u &&
-                      memcmp(&h->graph_sampling, sp, sizeof(fsb_sampling)) == 0;
-    if (!same) {
-        if (h->graph_exec) {
-            cudaGraphExecDestroy(h->graph_exec);
-            h->graph_exec = nullptr;
+    DecodeGraph* hit = nullptr;
+    for (DecodeGraph& g : h->graphs)
+        if (g.batch == batch && g.tile == tile && g.lcap == h->ctx_lcap && g.slot_control == h->slot_control &&
+            g.noise == h->noise_u && memcmp(&g.sampling, sp, sizeof(fsb_sampling)) == 0)
+            hit = &g;
+    if (hit == nullptr) {
+        if (static_cast<int>(h->graphs.size()) >= kGraphCache) {  // make room: drop the least recently used frame
+            auto lru = std::min_element(h->graphs.begin(), h->graphs.end(),
+                                        [](const DecodeGraph& a, const DecodeGraph& b) { return a.used < b.used; });
+            cudaGraphExecDestroy(lru->exec);
+            h->graphs.erase(lru);
         }
         // capture on a private stream so the caller's stream mode does not matter
         cudaStream_t cs;
@@ -841,10 +931,10 @@ int fsb_lm_decode(fsb_lm* h, int batch, int nframes, const fsb_sampling* sp, int
         int rc = 1;
         const int launches_before = g_launch_count;
         if (e == cudaSuccess) {
-            rc = decode_one_frame(h, batch, *sp, cs);
+            rc = decode_one_frame(h, batch, tile, *sp, cs);
             e = cudaStreamEndCapture(cs, &g);
         }
-        h->graph_kernels = g_launch_count - launches_before;
+        const int kernels = g_launch_count - launches_before;
         g_launch_count = launches_before;  // captured, not launched
         if (e != cudaSuccess || rc != 0 || g == nullptr) {
             if (rc == 0) set_error("decode: graph capture failed: %s", cudaGetErrorString(e));
@@ -860,19 +950,40 @@ int fsb_lm_decode(fsb_lm* h, int batch, int nframes, const fsb_sampling* sp, int
             set_error("decode: cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
             return 1;
         }
-        h->graph_exec = ge;
-        h->graph_batch = batch;
-        h->graph_lcap = h->ctx_lcap;
-        h->graph_slot_control = h->slot_control;
-        h->graph_noise = h->noise_u;
-        h->graph_sampling = *sp;
+        ++h->graph_captures;
+        DecodeGraph d;
+        d.exec = ge;
+        d.batch = batch;
+        d.tile = tile;
+        d.lcap = h->ctx_lcap;
+        d.kernels = kernels;
+        d.slot_control = h->slot_control;
+        d.noise = h->noise_u;
+        d.sampling = *sp;
+        h->graphs.push_back(d);
+        hit = &h->graphs.back();
     }
+    hit->used = ++h->graph_uses;
     for (int i = 0; i < nframes; ++i) {
-        FSB_CUDA(cudaGraphLaunch(h->graph_exec, st));
-        g_launch_count += h->graph_kernels;
+        FSB_CUDA(cudaGraphLaunch(hit->exec, st));
+        g_launch_count += hit->kernels;
     }
     return 0;
 }
+
+int fsb_lm_set_decode_tile(fsb_lm* h, int tile) {
+    FSB_CHECK(h != nullptr, "set_decode_tile: null handle");
+    FSB_CHECK(tile == 0 || tile == kStepRows || tile == kStepRowsMax, "set_decode_tile: tile=%d must be 0, %d or %d",
+              tile, kStepRows, kStepRowsMax);
+    FSB_CHECK(tile <= h->rt, "set_decode_tile: tile=%d exceeds the engine's %d-row tile (max_batch=%d)", tile, h->rt,
+              h->cfg.max_batch);
+    h->force_tile = tile;
+    return 0;
+}
+
+int fsb_lm_decode_tile(fsb_lm* h) { return h ? h->last_tile : 0; }
+
+long long fsb_lm_graph_captures(fsb_lm* h) { return h ? h->graph_captures : 0; }
 
 int fsb_lm_bench_gemms(fsb_lm* h, int reps, double* weight_bytes_per_rep, int* launches_per_rep, void* stream) {
     // Every weight-streaming step GEMM of one decode frame (36 slow layers x 4, head, 10 fast passes x

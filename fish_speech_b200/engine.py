@@ -372,6 +372,22 @@ class LmEngine:
         except Exception:
             pass
 
+    # ---- decode row tile (include/fishb200.h fsb_lm_set_decode_tile) -------------------------------------------------
+    def set_decode_tile(self, tile: int) -> None:
+        """Test hook: 0 = each frame runs the 32-row step GEMMs when it decodes <= 32 rows (the default), 32 or 64 =
+        that tile for every frame. The tiles give the same bits; only the frame time differs."""
+        _lib.check(self.lib.fsb_lm_set_decode_tile(self.h, int(tile)))
+
+    @property
+    def decode_tile(self) -> int:
+        """Row tile of the last `decode` call (0 before the first)."""
+        return int(self.lib.fsb_lm_decode_tile(self.h))
+
+    @property
+    def graph_captures(self) -> int:
+        """Decode frames captured into CUDA graphs since the engine was created."""
+        return int(self.lib.fsb_lm_graph_captures(self.h))
+
     # -------------------------------------------------------------------------------------------
     def buffer(self, name: str) -> torch.Tensor:
         """Zero-copy torch view of a named device buffer of the handle."""

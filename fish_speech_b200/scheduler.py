@@ -12,6 +12,11 @@ Paced requests (`SlotRequest.pace`, frames per second the consumer plays) let an
 than it has slots: a slot produces frames several times faster than they are heard, so a stream that is far
 enough ahead of its playback is parked between two polls (its K/V stays in its pool pages, nothing is copied) and
 its slot serves a stream that is about to run dry; `schedule_live` is the whole policy.
+
+Compact rows (`ContinuousBatcher(compact_rows=True)`): a frame decodes rows [0, 1 + highest live slot) instead of
+every slot, and when the live requests fit in 32 rows the ones above them move down between two polls (the same park /
+resume, no K/V copied), so that an engine of more than 32 slots runs its 32-row step GEMMs whenever load allows;
+`compact_moves` is the whole policy.
 """
 from __future__ import annotations
 
@@ -22,7 +27,7 @@ from typing import Callable, NamedTuple, Optional, Sequence
 
 import torch
 
-from .engine import MAX_DECODE_BATCH, bf16_round, kv_pages_for
+from .engine import MAX_DECODE_BATCH, STEP_ROWS, bf16_round, kv_pages_for
 
 
 class Cancelled(Exception):
@@ -73,6 +78,7 @@ class SlotRequest:
     page_parks: int = 0
     page_wait: float = 0.0
     _short_since: float = 0.0
+    moves: int = 0  # compact_rows: times it was moved to a lower slot
 
     def lead(self, now: float) -> float:
         """Frames the consumer holds beyond what it has played at `now` (negative: it is waiting for frames). An
@@ -135,6 +141,19 @@ def schedule_live(running: Sequence[SlotRequest], parked: Sequence[SlotRequest],
     return LivePlan(park, resume, admit, rest)
 
 
+def compact_moves(running: Sequence[int], free: Sequence[int], rows: int = STEP_ROWS) -> list:
+    """(from slot, to slot) moves that put every running request into slots [0, rows): a pure function of the slots
+    the running requests hold and the free ones. Only when all of them fit there (at most `rows` running): each one at
+    or above `rows`, lowest first, goes to the lowest free slot below `rows`. Otherwise, or when none is above, no move.
+    Every move goes downward."""
+    running = sorted(int(s) for s in running)
+    if len(running) > rows:
+        return []
+    high = [s for s in running if s >= rows]
+    low = sorted(int(s) for s in free if int(s) < rows)
+    return list(zip(high, low))
+
+
 def kv_safe(avail: int, claims) -> bool:
     """Banker's rule over one resource, KV pages. `claims`: (need, alone) of every admitted request -- the pages it
     may still take before it ends, and the pages only its row maps now. Safe when the requests can be ordered so that
@@ -150,7 +169,8 @@ def kv_safe(avail: int, claims) -> bool:
 
 class ContinuousBatcher:
     def __init__(self, model, max_slots: int = 32, frames_per_poll: int = 8, min_free_to_admit: int = 1,
-                 max_live: Optional[int] = None, clock: Callable[[], float] = time.monotonic, kv_growth: bool = False):
+                 max_live: Optional[int] = None, clock: Callable[[], float] = time.monotonic, kv_growth: bool = False,
+                 compact_rows: bool = False):
         """`frames_per_poll`: decode frames between two looks at the device-side slot states (a finished slot
         idles for at most that many frames). `min_free_to_admit`: admissions wait until that many slots are
         free (or nothing is running) — every admission is one extra prefill pass + first frame that streams
@@ -160,7 +180,12 @@ class ContinuousBatcher:
         `kv_growth`: on an engine whose page pool cannot hold every request at its full budget, a request maps its
         prompt and one poll of frames at admission and takes further pages as it decodes, under the banker's rule
         (kv_safe); one that cannot get its next page now waits parked until it can. Off: prompt + budget are
-        reserved at admission and a running request never waits (DESIGN.md §4b)."""
+        reserved at admission and a running request never waits (DESIGN.md §4b).
+        `compact_rows`: each frame decodes rows [0, 1 + highest live slot) rather than all `max_slots`, and at a poll
+        boundary, when the running requests fit in 32 rows, those in slots >= 32 move to the lowest free slots below 32
+        (compact_moves; LmEngine.park_slot / resume_slot: a small state blob and a page-table row, no K/V copied). An
+        engine of more than 32 slots then runs its 32-row step GEMMs, with the same bits. Off: every frame decodes
+        all `max_slots` rows and a request never changes slot unless it is parked."""
         from .models.text2semantic.inference import _ensure_engine
 
         if not 1 <= max_slots <= MAX_DECODE_BATCH:
@@ -173,6 +198,8 @@ class ContinuousBatcher:
         if self.max_live < max_slots:
             raise ValueError(f"max_live must be >= max_slots ({max_slots}), got {max_live}")
         self.clock = clock
+        self.compact_rows = bool(compact_rows)
+        self.moves = 0  # compact_rows: requests moved to a lower slot
         self.parked: list[SlotRequest] = []  # admitted, between two polls without a slot (SlotRequest._parked)
         self.frames_per_poll = int(frames_per_poll)
         self.min_free_to_admit = max(1, int(min_free_to_admit))
@@ -280,6 +307,23 @@ class ContinuousBatcher:
         req.resumes += 1
         self.active[s] = req
         self._len[s] = parked.ctx_len
+
+    def _move(self, req: SlotRequest, s: int):
+        """Continue the running `req` in the free slot `s`: its per-slot state and page-table row go along, so it keeps
+        its pages, RAS window, random stream and playback clock."""
+        frm = req.slot
+        parked = self.eng.park_slot(frm, self._len.pop(frm))
+        del self.active[frm]
+        self.eng.resume_slot(s, parked)
+        req.slot = s
+        self.active[s] = req
+        self._len[s] = parked.ctx_len
+        req.moves += 1
+        self.moves += 1
+
+    def _compact(self):
+        for frm, to in compact_moves(list(self.active), self._free_slots()):
+            self._move(self.active[frm], to)
 
     def _schedule(self):
         """One scheduling decision (schedule_live) carried out: park, resume, admit, fill. With kv_growth, requests
@@ -555,13 +599,17 @@ class ContinuousBatcher:
             self._grow()
         if not self.active:
             return []
+        if self.compact_rows:
+            self._compact()  # after the grants: a moved request takes the pages granted to its row along
         k = self.frames_per_poll
         for s in self._len:
             self._len[s] += k
         self.eng.set_context_bound_exact(min(max(self._len.values()) + 1, self.eng.kv_len))
         # every slot row is decoded: idle and frozen rows cost one attention position and nothing else
-        # (the GEMMs stream the weights once for the engine's 32- or 64-row tile whatever the number of live rows)
-        self.eng.decode(self.max_slots, k, None, use_graph=True)
+        # (the GEMMs stream the weights once for the engine's 32- or 64-row tile whatever the number of live rows);
+        # compact_rows: only rows up to the highest live slot, on the 32-row tile when that is at most 32 rows
+        rows = 1 + max(self.active) if self.compact_rows else self.max_slots
+        self.eng.decode(rows, k, None, use_graph=True)
         self.frames_run += k
         self.slot_frames += k * len(self.active)
         return self._retire()

@@ -140,6 +140,20 @@ int fsb_lm_prefill(fsb_lm* h, const int32_t* d_tokens, const int32_t* d_row_slot
 int fsb_lm_decode(fsb_lm* h, int batch, int nframes, const fsb_sampling* s, int use_graph,
                   void* stream);
 
+/* Row tile of the decode frames. An engine of 33..64 slots holds the step GEMM plans of both tiles: the 64-row plans
+ * and 32-row plans with the same stream-K schedule over the first 32 rows of the same buffers (fsb_lm_create fails if
+ * the schedules differ). fsb_lm_decode runs a frame of batch <= 32 rows on the 32-row plans and a larger one on the
+ * 64-row plans; every output element is the same sum of the same MMAs at either tile, so only the time differs.
+ * Decode graphs are kept per (batch, tile, context bound, slot control, noise, sampling), up to 16 per engine, so
+ * changing the row count or the tile between calls replays a captured frame once it has been seen.
+ * fsb_lm_set_decode_tile (test hook): 0 = by the row count (default), 32 or 64 = that tile for every frame (64 needs
+ * an engine of more than 32 slots; a decode of more rows than a forced 32-row tile holds fails).
+ * fsb_lm_decode_tile: the tile of the last fsb_lm_decode call (0 before the first). fsb_lm_graph_captures: decode
+ * frames captured into graphs since fsb_lm_create. */
+int fsb_lm_set_decode_tile(fsb_lm* h, int tile);
+int fsb_lm_decode_tile(fsb_lm* h);
+long long fsb_lm_graph_captures(fsb_lm* h);
+
 /* Prefix KV reuse (SURVEY §8(f).2; the reference re-prefills the whole growing conversation for every chunk,
  * inference.py:611-721). The slow KV cache of a slot stays valid for the positions a prefill wrote until they are
  * overwritten, so a prompt that shares its first p rows with what a slot already holds only needs rows [p, T):

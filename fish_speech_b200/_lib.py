@@ -74,6 +74,7 @@ def lib() -> C.CDLL:
     L.fsb_lm_destroy.argtypes = [vp]
     L.fsb_lm_destroy.restype = None
     L.fsb_lm_prefill.argtypes = [vp, vp, vp, vp, i32, vp, vp, i32, i32, C.POINTER(Sampling), vp]
+    L.fsb_lm_prefill_deferred.argtypes = [vp, vp, vp, vp, i32, vp, vp, i32, C.POINTER(C.c_int32), vp]
     L.fsb_lm_decode.argtypes = [vp, i32, i32, C.POINTER(Sampling), i32, vp]
     L.fsb_lm_set_decode_tile.argtypes = [vp, i32]
     L.fsb_lm_decode_tile.argtypes = [vp]

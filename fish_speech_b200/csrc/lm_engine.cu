@@ -83,6 +83,7 @@ struct DecodeGraph {
     cudaGraphExec_t exec = nullptr;
     int batch = -1, tile = 0, lcap = -1, kernels = 0;
     bool slot_control = false;
+    bool first_frame = false;  // fused admission: the splice node and the first-frame sampler
     const float* noise = nullptr;
     fsb_sampling sampling{};
     unsigned long long used = 0;  // last use, for least-recently-used eviction
@@ -129,6 +130,14 @@ struct fsb_lm {
     int *cur_tok = nullptr, *out_tokens = nullptr, *n_out = nullptr, *pos = nullptr, *finished = nullptr;
     int *ras_window = nullptr, *iota = nullptr, *fpos = nullptr;
     int* kv_miss = nullptr;  // per slot: 0, or 1 + the position at which decode attention first met an unmapped page
+    // fused admission (fsb_lm_prefill_deferred): per slot, the staged last prompt row, its sums of squares and position,
+    // and whether its first frame is still to run; the host mirrors the flags (cleared once a frame serving them is
+    // enqueued)
+    bf16* stage_x = nullptr;
+    float* stage_ssq = nullptr;
+    int *stage_pos = nullptr, *pending = nullptr;
+    std::vector<char> pending_host;
+    int n_pending = 0;
     unsigned long long* step = nullptr;
     // debug / test hooks
     float *slow_logits = nullptr, *fast_logits = nullptr;
@@ -481,7 +490,7 @@ SampleArgs frame_sample_args(const fsb_lm* h, int p, const StepPartials& parts, 
 
 // Head + sampling + fast passes + bookkeeping for `rows` sequences whose last residual-stream rows (un-normed)
 // are in slow.xres[0..rows) with their sums of squares in slow.ssq, on the plans `fp`. inference.py:114-181.
-int run_frame_tail(fsb_lm* h, const FramePlans& fp, int rows, const int* row_slot, bool use_ras,
+int run_frame_tail(fsb_lm* h, const FramePlans& fp, int rows, const int* row_slot, bool use_ras, bool first_frame,
                    const int* set_pos_rows, const int* row_pos_src, const fsb_sampling& sp, cudaStream_t st) {
     const fsb_lm_config& c = h->cfg;
     const int C = c.num_codebooks;
@@ -490,7 +499,8 @@ int run_frame_tail(fsb_lm* h, const FramePlans& fp, int rows, const int* row_slo
     Stack& f = h->fast;
     // ---- slow head over the selectable rows (the final norm is applied on load) ----
     FSB_TRY(step_gemm_launch(*fp.head, rows, st));
-    FSB_TRY(launch_sample(frame_sample_args(h, 0, step_plan_partials(*fp.head), rows, row_slot, use_ras, sp), st));
+    const SampleArgs head_sample = frame_sample_args(h, 0, step_plan_partials(*fp.head), rows, row_slot, use_ras, sp);
+    FSB_TRY(first_frame ? launch_sample_first_frame(head_sample, st) : launch_sample(head_sample, st));
 
     // ---- fast pass 0 input: hidden = norm(x) (norm_fastlayer_input) [-> fast_project_in]  (llama.py:459-461, 819-828)
     RowsArgs hr{};
@@ -542,13 +552,100 @@ int run_frame_tail(fsb_lm* h, const FramePlans& fp, int rows, const int* row_slo
     return 0;
 }
 
-// One frame over rows [0, batch) on the plans of row tile `tile` (batch <= tile).
-int decode_one_frame(fsb_lm* h, int batch, int tile, const fsb_sampling& sp, cudaStream_t st) {
+FirstFrameArgs first_frame_args(fsb_lm* h, int rows) {
+    FirstFrameArgs a{};
+    a.x = h->slow.xres;
+    a.ssq = h->slow.ssq;
+    a.stage_x = h->stage_x;
+    a.stage_ssq = h->stage_ssq;
+    a.stage_pos = h->stage_pos;
+    a.pending = h->pending;
+    a.pos = h->pos;
+    a.state = h->slot_state;
+    a.rows = rows;
+    a.D = h->slow.D;
+    return a;
+}
+
+// One frame over rows [0, batch) on the plans of row tile `tile` (batch <= tile). first_frame (fused admission): the
+// rows of slots whose first frame a deferred prefill left pending take their staged last prompt row between the slow
+// stack and the head, and sample it by the prefill's rule.
+int decode_one_frame(fsb_lm* h, int batch, int tile, const fsb_sampling& sp, bool first_frame, cudaStream_t st) {
     Stack& s = h->slow;
     const FramePlans fp = frame_plans(h, tile);
     FSB_TRY(launch_embed(embed_args(h, h->cur_tok, s.xres, s.ssq, batch), st));
     FSB_TRY(run_stack_decode(h, s, *fp.slow, batch, h->iota, h->pos, false, st));
-    return run_frame_tail(h, fp, batch, nullptr, true, nullptr, nullptr, sp, st);
+    if (first_frame) FSB_TRY(launch_first_frame_splice(first_frame_args(h, batch), st));
+    return run_frame_tail(h, fp, batch, nullptr, true, first_frame, nullptr, nullptr, sp, st);
+}
+
+// `nframes` frames over rows [0, batch) on row tile `tile`, eagerly or as replays of a captured frame.
+int decode_frames(fsb_lm* h, int batch, int tile, int nframes, const fsb_sampling& spr, bool first_frame,
+                         int use_graph, cudaStream_t st) {
+    const fsb_sampling* sp = &spr;
+    if (!use_graph) {
+        for (int i = 0; i < nframes; ++i) FSB_TRY(decode_one_frame(h, batch, tile, *sp, first_frame, st));
+        return 0;
+    }
+    DecodeGraph* hit = nullptr;
+    for (DecodeGraph& g : h->graphs)
+        if (g.batch == batch && g.tile == tile && g.lcap == h->ctx_lcap && g.slot_control == h->slot_control &&
+            g.first_frame == first_frame && g.noise == h->noise_u && memcmp(&g.sampling, sp, sizeof(fsb_sampling)) == 0)
+            hit = &g;
+    if (hit == nullptr) {
+        if (static_cast<int>(h->graphs.size()) >= kGraphCache) {  // make room: drop the least recently used frame
+            auto lru = std::min_element(h->graphs.begin(), h->graphs.end(),
+                                        [](const DecodeGraph& a, const DecodeGraph& b) { return a.used < b.used; });
+            cudaGraphExecDestroy(lru->exec);
+            h->graphs.erase(lru);
+        }
+        // capture on a private stream so the caller's stream mode does not matter
+        cudaStream_t cs;
+        FSB_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+        cudaGraph_t g = nullptr;
+        cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
+        int rc = 1;
+        const int launches_before = g_launch_count;
+        if (e == cudaSuccess) {
+            rc = decode_one_frame(h, batch, tile, *sp, first_frame, cs);
+            e = cudaStreamEndCapture(cs, &g);
+        }
+        const int kernels = g_launch_count - launches_before;
+        g_launch_count = launches_before;  // captured, not launched
+        if (e != cudaSuccess || rc != 0 || g == nullptr) {
+            if (rc == 0) set_error("decode: graph capture failed: %s", cudaGetErrorString(e));
+            cudaStreamDestroy(cs);
+            if (g) cudaGraphDestroy(g);
+            return 1;
+        }
+        cudaGraphExec_t ge = nullptr;
+        e = cudaGraphInstantiate(&ge, g, 0);
+        cudaGraphDestroy(g);
+        cudaStreamDestroy(cs);
+        if (e != cudaSuccess) {
+            set_error("decode: cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
+            return 1;
+        }
+        ++h->graph_captures;
+        DecodeGraph d;
+        d.exec = ge;
+        d.batch = batch;
+        d.tile = tile;
+        d.lcap = h->ctx_lcap;
+        d.kernels = kernels;
+        d.slot_control = h->slot_control;
+        d.first_frame = first_frame;
+        d.noise = h->noise_u;
+        d.sampling = *sp;
+        h->graphs.push_back(d);
+        hit = &h->graphs.back();
+    }
+    hit->used = ++h->graph_uses;
+    for (int i = 0; i < nframes; ++i) {
+        FSB_CUDA(cudaGraphLaunch(hit->exec, st));
+        g_launch_count += hit->kernels;
+    }
+    return 0;
 }
 
 size_t step_ws_bound(int n_out, int ctas, int rt) {
@@ -705,6 +802,11 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &h->slot_top_k, cfg->max_batch, "slot_top_k"));
     TRYC(dalloc(h, &h->slot_seed, cfg->max_batch, "slot_seed"));
     TRYC(dalloc(h, &h->kv_miss, cfg->max_batch, "kv_miss"));
+    TRYC(dalloc(h, &h->stage_x, static_cast<size_t>(cfg->max_batch) * s.D));
+    TRYC(dalloc(h, &h->stage_ssq, static_cast<size_t>(cfg->max_batch) * kSsqStride));
+    TRYC(dalloc(h, &h->stage_pos, cfg->max_batch));
+    TRYC(dalloc(h, &h->pending, cfg->max_batch, "first_frame_pending"));
+    h->pending_host.assign(cfg->max_batch, 0);
     TRYC(dalloc(h, &h->iota, RT));
     TRYC(dalloc(h, &h->fpos, static_cast<size_t>(C) * RT));
     TRYC(dalloc(h, &h->step, 1, "step"));
@@ -820,6 +922,9 @@ int fsb_lm_reset(fsb_lm* h, void* stream) {
     FSB_CUDA(cudaMemsetAsync(h->ras_window, 0, static_cast<size_t>(c.max_batch) * 10 * 4, st));
     FSB_CUDA(cudaMemsetAsync(h->pos, 0, h->rt * 4, st));
     FSB_CUDA(cudaMemsetAsync(h->step, 0, 8, st));
+    FSB_CUDA(cudaMemsetAsync(h->pending, 0, c.max_batch * 4, st));
+    std::fill(h->pending_host.begin(), h->pending_host.end(), 0);
+    h->n_pending = 0;
     return 0;
 }
 
@@ -847,7 +952,44 @@ int fsb_lm_prefill(fsb_lm* h, const int32_t* d_tokens, const int32_t* d_row_slot
     g.rows = nseq; g.D = s.D; g.eps = c.norm_eps;
     FSB_TRY(launch_rows(g, st));
     // the reference resets the RAS window per generate() call and prefill uses no RAS
-    return run_frame_tail(h, frame_plans(h, h->rt), nseq, d_slots, false, d_last_rows, d_row_pos, *sp, st);
+    return run_frame_tail(h, frame_plans(h, h->rt), nseq, d_slots, false, false, d_last_rows, d_row_pos, *sp, st);
+}
+
+int fsb_lm_prefill_deferred(fsb_lm* h, const int32_t* d_tokens, const int32_t* d_row_slot, const int32_t* d_row_pos,
+                            int rows, const int32_t* d_last_rows, const int32_t* d_slots, int nseq,
+                            const int32_t* h_slots, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(h != nullptr, "prefill_deferred: null handle");
+    const fsb_lm_config& c = h->cfg;
+    FSB_CHECK(h->slot_control, "prefill_deferred: a deferred first frame needs slot control (fsb_lm_set_slot_control)");
+    FSB_CHECK(rows >= 1 && rows <= std::max(c.max_rows, 128), "prefill: rows=%d exceeds max_rows=%d", rows, c.max_rows);
+    FSB_CHECK(nseq >= 1 && nseq <= c.max_batch, "prefill: nseq=%d out of range", nseq);
+    FSB_CHECK(h_slots != nullptr, "prefill_deferred: null host slot list");
+    for (int i = 0; i < nseq; ++i)
+        FSB_CHECK(h_slots[i] >= 0 && h_slots[i] < c.max_batch, "prefill_deferred: slot %d outside [0, %d)", h_slots[i],
+                  c.max_batch);
+    Stack& s = h->slow;
+    FSB_TRY(prefill_embed(h, d_tokens, rows, st));
+    FSB_TRY(run_stack_prefill(h, rows, d_row_slot, d_row_pos, st));
+    // the gather of fsb_lm_prefill's tail, into the same rows; the decode residual stream is free between frames
+    RowsArgs g{};
+    g.x = h->xres_p;
+    g.y = s.xres;
+    g.ssq = s.ssq;
+    g.gather = d_last_rows;
+    g.gather_stride = 1;
+    g.rows = nseq; g.D = s.D; g.eps = c.norm_eps;
+    FSB_TRY(launch_rows(g, st));
+    FirstFrameArgs a = first_frame_args(h, nseq);
+    a.slots = d_slots;
+    a.last_rows = d_last_rows;
+    a.row_pos = d_row_pos;
+    FSB_TRY(launch_first_frame_stage(a, st));
+    for (int i = 0; i < nseq; ++i) {
+        if (!h->pending_host[h_slots[i]]) ++h->n_pending;
+        h->pending_host[h_slots[i]] = 1;
+    }
+    return 0;
 }
 
 int fsb_lm_set_slot_control(fsb_lm* h, int enable) {
@@ -878,13 +1020,21 @@ static int slot_state_args(fsb_lm* h, int slot, const void* d_blob, const char* 
 int fsb_lm_slot_save(fsb_lm* h, int slot, void* d_blob, void* stream) {
     SlotStateArgs a{};
     FSB_TRY(slot_state_args(h, slot, d_blob, "slot_save", &a));
+    FSB_CHECK(!h->pending_host[slot], "slot_save: slot %d has a deferred first frame that no decode frame has served yet",
+              slot);
     return launch_slot_save(a, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int fsb_lm_slot_restore(fsb_lm* h, int slot, const void* d_blob, void* stream) {
     SlotStateArgs a{};
     FSB_TRY(slot_state_args(h, slot, d_blob, "slot_restore", &a));
-    return launch_slot_restore(a, reinterpret_cast<cudaStream_t>(stream));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (h->pending_host[slot]) {  // a request vacated before its first frame: the restored one replaces it
+        FSB_CUDA(cudaMemsetAsync(h->pending + slot, 0, sizeof(int), st));
+        h->pending_host[slot] = 0;
+        --h->n_pending;
+    }
+    return launch_slot_restore(a, st);
 }
 
 int fsb_lm_set_sampler_noise(fsb_lm* h, const float* d_u, int draws_per_frame, int ld) {
@@ -907,68 +1057,18 @@ int fsb_lm_decode(fsb_lm* h, int batch, int nframes, const fsb_sampling* sp, int
     const fsb_sampling sp_none{1.f, 1.f, 1, 0};
     if (sp == nullptr || h->slot_control) sp = &sp_none;  // per-slot parameters: one graph for every mix of requests
     h->last_tile = tile;
-    if (!use_graph) {
-        for (int i = 0; i < nframes; ++i) FSB_TRY(decode_one_frame(h, batch, tile, *sp, st));
-        return 0;
+    if (h->n_pending > 0 && nframes >= 1) {
+        // fused admission: the first frame also serves the first frames that deferred prefills left pending
+        FSB_CHECK(h->slot_control, "decode: slots with a deferred first frame need slot control");
+        for (int s = batch; s < h->cfg.max_batch; ++s)
+            FSB_CHECK(!h->pending_host[s], "decode: slot %d waits for its first frame outside the batch of %d rows", s,
+                      batch);
+        FSB_TRY(decode_frames(h, batch, tile, 1, *sp, true, use_graph, st));
+        std::fill(h->pending_host.begin(), h->pending_host.end(), 0);
+        h->n_pending = 0;
+        --nframes;
     }
-    DecodeGraph* hit = nullptr;
-    for (DecodeGraph& g : h->graphs)
-        if (g.batch == batch && g.tile == tile && g.lcap == h->ctx_lcap && g.slot_control == h->slot_control &&
-            g.noise == h->noise_u && memcmp(&g.sampling, sp, sizeof(fsb_sampling)) == 0)
-            hit = &g;
-    if (hit == nullptr) {
-        if (static_cast<int>(h->graphs.size()) >= kGraphCache) {  // make room: drop the least recently used frame
-            auto lru = std::min_element(h->graphs.begin(), h->graphs.end(),
-                                        [](const DecodeGraph& a, const DecodeGraph& b) { return a.used < b.used; });
-            cudaGraphExecDestroy(lru->exec);
-            h->graphs.erase(lru);
-        }
-        // capture on a private stream so the caller's stream mode does not matter
-        cudaStream_t cs;
-        FSB_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        cudaGraph_t g = nullptr;
-        cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-        int rc = 1;
-        const int launches_before = g_launch_count;
-        if (e == cudaSuccess) {
-            rc = decode_one_frame(h, batch, tile, *sp, cs);
-            e = cudaStreamEndCapture(cs, &g);
-        }
-        const int kernels = g_launch_count - launches_before;
-        g_launch_count = launches_before;  // captured, not launched
-        if (e != cudaSuccess || rc != 0 || g == nullptr) {
-            if (rc == 0) set_error("decode: graph capture failed: %s", cudaGetErrorString(e));
-            cudaStreamDestroy(cs);
-            if (g) cudaGraphDestroy(g);
-            return 1;
-        }
-        cudaGraphExec_t ge = nullptr;
-        e = cudaGraphInstantiate(&ge, g, 0);
-        cudaGraphDestroy(g);
-        cudaStreamDestroy(cs);
-        if (e != cudaSuccess) {
-            set_error("decode: cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
-            return 1;
-        }
-        ++h->graph_captures;
-        DecodeGraph d;
-        d.exec = ge;
-        d.batch = batch;
-        d.tile = tile;
-        d.lcap = h->ctx_lcap;
-        d.kernels = kernels;
-        d.slot_control = h->slot_control;
-        d.noise = h->noise_u;
-        d.sampling = *sp;
-        h->graphs.push_back(d);
-        hit = &h->graphs.back();
-    }
-    hit->used = ++h->graph_uses;
-    for (int i = 0; i < nframes; ++i) {
-        FSB_CUDA(cudaGraphLaunch(hit->exec, st));
-        g_launch_count += hit->kernels;
-    }
-    return 0;
+    return decode_frames(h, batch, tile, nframes, *sp, false, use_graph, st);
 }
 
 int fsb_lm_set_decode_tile(fsb_lm* h, int tile) {

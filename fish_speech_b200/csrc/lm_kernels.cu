@@ -1022,9 +1022,13 @@ __device__ __forceinline__ ArgMax block_argmax(ArgMax x, ArgMax* red) {
     return red[32];
 }
 
-__global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
-    pdl_launch_dependents();
-    pdl_wait();
+// One row of the sampler. FIRST_FRAME (fused admission, slot control only): a row whose slot has produced no frame yet
+// samples by the prefill's rule, no RAS substitution and no RAS-window update (inference.py:336-352 samples the first
+// frame without previous_tokens); every other row by a.use_ras / a.ras_update as in sample_kernel. The arguments are
+// taken by value and each rule is read where it is used, so that sample_kernel compiles to the very instructions it had
+// before this template existed.
+template <bool FIRST_FRAME>
+__device__ __forceinline__ void sample_row(SampleArgs a) {
     __shared__ float lg[kSampleMaxN];
     __shared__ ArgMax red[33];
     __shared__ float fred[33];
@@ -1043,6 +1047,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     const float top_p = per_slot ? ctl.top_p[slot] : a.top_p;
     const int top_k = per_slot ? ctl.top_k[slot] : a.top_k;
     const unsigned long long seed = per_slot ? ctl.seed[slot] : a.seed;
+#define FSB_ROW_RULE(flag) (FIRST_FRAME ? ((flag) && ctl.n_out[slot] != 0) : (flag))
     for (int e0 = threadIdx.x; e0 < n; e0 += 4 * kSampleThreads) {
         int feat[4];
         bool ok[4];
@@ -1065,7 +1070,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
 
     // top_k <= 1 keeps rank 0 only, as the reference's mask does (ranks >= top_k removed, then rank 0 restored): the
     // greedy argmax, and no RAS re-draw, whose top-k cut is the same
-    const bool two = a.slow && a.use_ras && top_k > 1;
+    const bool two = a.slow && FSB_ROW_RULE(a.use_ras) && top_k > 1;
     if (top_k <= 1) {
         ArgMax x{-INFINITY, 0x7fffffff};
         for (int e = threadIdx.x; e < n; e += kSampleThreads) x = better(x, ArgMax{lg[e], e});
@@ -1168,7 +1173,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         if (a.slow) {
             int e = s_choice[0];
             int tok = e < a.n_sem ? a.sem_begin + e : a.im_end_id;
-            if (a.use_ras) {
+            if (FSB_ROW_RULE(a.use_ras)) {
                 const int eh = s_choice[1];
                 const int tok_h = eh < a.n_sem ? a.sem_begin + eh : a.im_end_id;
                 bool in_win = false;
@@ -1180,7 +1185,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
             c0 = c0 < 0 ? 0 : (c0 > a.codebook_size - 1 ? a.codebook_size - 1 : c0);
             ct[0] = tok;
             ct[1] = c0;
-            if (a.ras_update) {
+            if (FSB_ROW_RULE(a.ras_update)) {
                 for (int k = 0; k < 9; ++k) a.ras_window[slot * 10 + k] = a.ras_window[slot * 10 + k + 1];
                 a.ras_window[slot * 10 + 9] = tok;
             }
@@ -1191,6 +1196,63 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         } else {
             ct[a.cb_index + 1] = s_choice[0];
         }
+    }
+#undef FSB_ROW_RULE
+}
+
+__global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    sample_row<false>(a);
+}
+
+__global__ void __launch_bounds__(kSampleThreads) sample_first_frame_kernel(SampleArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    sample_row<true>(a);
+}
+
+// ------------------------------------------------------------------------------------------------
+// fused admission: stage a deferred prefill's last rows per slot, splice them into the next decode frame
+// ------------------------------------------------------------------------------------------------
+constexpr int kFirstFrameThreads = 256;
+
+// 16-byte copy of one residual row (D % 8 == 0) and its sums of squares
+__device__ __forceinline__ void copy_resid_row(__nv_bfloat16* y, float* y_ssq, const __nv_bfloat16* x,
+                                               const float* x_ssq, int D) {
+    const uint4* src = reinterpret_cast<const uint4*>(x);
+    uint4* dst = reinterpret_cast<uint4*>(y);
+    for (int i = threadIdx.x; i < D / 8; i += kFirstFrameThreads) dst[i] = src[i];
+    if (threadIdx.x < kSsqRowStride) y_ssq[threadIdx.x] = x_ssq[threadIdx.x];
+}
+
+__global__ void __launch_bounds__(kFirstFrameThreads) first_frame_stage_kernel(FirstFrameArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int i = blockIdx.x;
+    const int slot = a.slots[i];
+    copy_resid_row(a.stage_x + static_cast<size_t>(slot) * a.D, a.stage_ssq + slot * kSsqRowStride,
+                   a.x + static_cast<size_t>(i) * a.D, a.ssq + i * kSsqRowStride, a.D);
+    if (threadIdx.x == 0) {
+        a.stage_pos[slot] = a.row_pos[a.last_rows[i]];
+        a.pending[slot] = 1;
+        a.pos[slot] = -1;
+    }
+}
+
+__global__ void __launch_bounds__(kFirstFrameThreads) first_frame_splice_kernel(FirstFrameArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int slot = blockIdx.x;  // decode row r is slot r
+    if (a.pending[slot] == 0) return;
+    const int s = a.state[slot];
+    if (s == 1 || s == 3)
+        copy_resid_row(a.x + static_cast<size_t>(slot) * a.D, a.ssq + slot * kSsqRowStride,
+                       a.stage_x + static_cast<size_t>(slot) * a.D, a.stage_ssq + slot * kSsqRowStride, a.D);
+    __syncthreads();  // every thread has read the flag before it is cleared
+    if (threadIdx.x == 0) {
+        if (s == 1 || s == 3) a.pos[slot] = a.stage_pos[slot];
+        a.pending[slot] = 0;
     }
 }
 
@@ -1495,6 +1557,28 @@ int launch_sample(const SampleArgs& a, cudaStream_t st) {
     if (a.rows <= 0) return 0;
     FSB_CHECK(a.n > 0 && a.n <= kSampleMaxN, "sample: n=%d out of range", a.n);
     FSB_LAUNCH(sample_kernel, dim3(a.rows), dim3(kSampleThreads), 0, st, a);
+    return 0;
+}
+
+int launch_sample_first_frame(const SampleArgs& a, cudaStream_t st) {
+    if (a.rows <= 0) return 0;
+    FSB_CHECK(a.n > 0 && a.n <= kSampleMaxN, "sample: n=%d out of range", a.n);
+    FSB_CHECK(a.ctl.state != nullptr && a.slow, "sample: the first-frame rule needs slot control and the slow head");
+    FSB_LAUNCH(sample_first_frame_kernel, dim3(a.rows), dim3(kSampleThreads), 0, st, a);
+    return 0;
+}
+
+int launch_first_frame_stage(const FirstFrameArgs& a, cudaStream_t st) {
+    if (a.rows <= 0) return 0;
+    FSB_CHECK(a.D % 8 == 0 && a.D <= kSsqTile * kSsqRowStride, "first_frame_stage: D=%d unsupported", a.D);
+    FSB_LAUNCH(first_frame_stage_kernel, dim3(a.rows), dim3(kFirstFrameThreads), 0, st, a);
+    return 0;
+}
+
+int launch_first_frame_splice(const FirstFrameArgs& a, cudaStream_t st) {
+    if (a.rows <= 0) return 0;
+    FSB_CHECK(a.D % 8 == 0 && a.D <= kSsqTile * kSsqRowStride, "first_frame_splice: D=%d unsupported", a.D);
+    FSB_LAUNCH(first_frame_splice_kernel, dim3(a.rows), dim3(kFirstFrameThreads), 0, st, a);
     return 0;
 }
 

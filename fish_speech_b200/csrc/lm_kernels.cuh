@@ -250,6 +250,35 @@ struct SampleArgs {
     SlotCtl ctl;
 };
 int launch_sample(const SampleArgs& a, cudaStream_t st);
+// The slow sampler of a decode frame that also serves admitted requests' first frames (fused admission): a row whose
+// slot has produced no frame yet (n_out[slot] == 0) samples by the prefill's rule -- no RAS substitution, no
+// RAS-window update --, every other row as launch_sample does with a.use_ras / a.ras_update. Slot control only.
+int launch_sample_first_frame(const SampleArgs& a, cudaStream_t st);
+
+// Fused admission: a prefill that defers its requests' first frames leaves each sequence's last residual row here, per
+// slot, and the next decode frame splices it into its own residual stream right before the head GEMM.
+struct FirstFrameArgs {
+    __nv_bfloat16* x;          // decode residual stream [RT][D] (stage: rows [0, rows) = the gathered last rows)
+    float* ssq;                // its sums of squares [RT][kSsqRowStride]
+    __nv_bfloat16* stage_x;    // [max_batch][D] staged last rows, by slot
+    float* stage_ssq;          // [max_batch][kSsqRowStride]
+    int* stage_pos;            // [max_batch] position of the staged row
+    int* pending;              // [max_batch] 1: the slot's first frame is still to run
+    int* pos;                  // decode positions [RT]
+    const int* slots;          // stage: slot of row i
+    const int* last_rows;      // stage: prefill row of sequence i (its position is row_pos[last_rows[i]])
+    const int* row_pos;        // stage: positions of the prefill rows
+    const int* state;          // splice: slot states (a slot vacated while pending is not spliced)
+    int rows, D;
+};
+// Stage: rows [0, rows) of x / ssq -> their slots' staging rows, with the position of the prefill's last row; the
+// slot is marked pending and parked at position -1, so that the frame serving it neither appends K/V for the row nor
+// attends for it in the slow stack.
+int launch_first_frame_stage(const FirstFrameArgs& a, cudaStream_t st);
+// Splice, after the slow stack's last finalize and before the head GEMM: for each of the frame's `rows` rows whose slot
+// is pending and live, its staged row and sums of squares replace the frame's row, and its position becomes the staged
+// one (frame_end then advances it as the prefill's own frame would); the pending flag is cleared either way.
+int launch_first_frame_splice(const FirstFrameArgs& a, cudaStream_t st);
 
 // bookkeeping at the end of a frame for each row's slot:
 //   out_tokens[slot][c][n_out[slot]] = cur_tok[slot][c]; n_out[slot]++;

@@ -629,9 +629,14 @@ class LmEngine:
 
     def prefill(self, prompts: Sequence[torch.Tensor], slots: Sequence[int], sp: Optional[_lib.Sampling],
                 start_pos: Optional[Sequence[int]] = None, do_sample: bool = True,
-                kv_end: Optional[Sequence[int]] = None) -> None:
+                kv_end: Optional[Sequence[int]] = None, defer_first_frame: bool = False) -> None:
         """prompts[k]: integer tensor [C+1, T_k] (row 0 token ids, rows 1..C codes) for slot slots[k]. `kv_end[k]`:
-        reserve KV pages up to that position (prompt + frames to come) instead of the prompt alone."""
+        reserve KV pages up to that position (prompt + frames to come) instead of the prompt alone.
+        `defer_first_frame` (with do_sample, under slot control): the first frames are not run here; the next `decode`
+        runs them as rows of its first frame, next to the running requests, with the same tokens
+        (include/fishb200.h fsb_lm_prefill_deferred)."""
+        if defer_first_frame and not self.slot_control:
+            raise ValueError("defer_first_frame needs slot control (set_slot_control)")
         C1 = self.cfg.num_codebooks + 1
         start_pos = list(start_pos) if start_pos is not None else [0] * len(prompts)
         for p, s0 in zip(prompts, start_pos):
@@ -687,10 +692,16 @@ class LmEngine:
                 d_pos = torch.cat(rpos).to(dev)
                 d_last = torch.tensor(last, dtype=torch.int32, device=dev)
                 d_gsl = torch.tensor(gsl, dtype=torch.int32, device=dev)
-                _lib.check(self.lib.fsb_lm_prefill(
-                    self.h, d_tok.data_ptr(), d_slot.data_ptr(), d_pos.data_ptr(), rows, d_last.data_ptr(),
-                    d_gsl.data_ptr(), len(grp), int(do_sample and final), C.byref(sp) if sp is not None else None,
-                    _stream()))
+                if defer_first_frame and do_sample and final:
+                    h_gsl = (C.c_int32 * len(gsl))(*gsl)
+                    _lib.check(self.lib.fsb_lm_prefill_deferred(
+                        self.h, d_tok.data_ptr(), d_slot.data_ptr(), d_pos.data_ptr(), rows, d_last.data_ptr(),
+                        d_gsl.data_ptr(), len(grp), h_gsl, _stream()))
+                else:
+                    _lib.check(self.lib.fsb_lm_prefill(
+                        self.h, d_tok.data_ptr(), d_slot.data_ptr(), d_pos.data_ptr(), rows, d_last.data_ptr(),
+                        d_gsl.data_ptr(), len(grp), int(do_sample and final), C.byref(sp) if sp is not None else None,
+                        _stream()))
                 # index tensors must outlive the asynchronous kernels that read them
                 self._inflight = (d_tok, d_slot, d_pos, d_last, d_gsl)
 
@@ -706,13 +717,14 @@ class LmEngine:
         return int(diff[0]) if len(diff) else n
 
     def prefill_reusing(self, prompts: Sequence[torch.Tensor], slots: Sequence[int], sp: Optional[_lib.Sampling],
-                        do_sample: bool = True, kv_end: Optional[Sequence[int]] = None) -> list[int]:
+                        do_sample: bool = True, kv_end: Optional[Sequence[int]] = None,
+                        defer_first_frame: bool = False) -> list[int]:
         """`prefill` of full prompts that skips every row whose K/V the cache already holds: the longest prefix
         a prompt shares with what its own slot was last prefilled with, or with another slot that is not being
         re-prefilled in this call (its whole pages are mapped by reference; a partly shared last page is copied).
         The reference re-prefills the whole growing conversation for every chunk of `generate_long`
         (inference.py:611-721); prefill is row-independent, so the reused K/V is bit-identical to what a full
-        prefill would write. Returns the reused length per prompt."""
+        prefill would write. `defer_first_frame` as for `prefill`. Returns the reused length per prompt."""
         host = [p.detach().to("cpu", torch.int32) for p in prompts]
         busy = set(int(s) for s in slots)
         ends = [p.shape[1] if kv_end is None else max(p.shape[1], min(int(e), self.kv_len))
@@ -729,7 +741,8 @@ class LmEngine:
         self._reserve([(int(s), e, b) for s, e, b in zip(slots, ends, reused)])
         for p, b in zip(prompts, reused):
             pieces.append(p[:, b:])
-        self.prefill(pieces, slots, sp, start_pos=reused, do_sample=do_sample, kv_end=ends)
+        defer = dict(defer_first_frame=True) if defer_first_frame else {}
+        self.prefill(pieces, slots, sp, start_pos=reused, do_sample=do_sample, kv_end=ends, **defer)
         for p, s in zip(host, slots):
             self._slot_tokens[int(s)] = p
         self.rows_reused += sum(reused)

@@ -513,7 +513,9 @@ def serve_requests(model, input_queue: "queue.Queue", max_slots: int, frames_per
     dry. FSB_SERVE_KV_GROW=1 (with FSB_SERVE_KV_GB) lets requests take KV pages as they decode instead of reserving
     prompt + budget at admission (ContinuousBatcher kv_growth). FSB_SERVE_COMPACT=1 decodes only the rows up to the
     highest live slot and moves requests below slot 32 whenever they all fit there, so that an engine of more than 32
-    slots runs its 32-row frame off-peak (ContinuousBatcher compact_rows). A request dict may carry `cancel` (a threading.Event): once it is set the request in flight is taken out
+    slots runs its 32-row frame off-peak (ContinuousBatcher compact_rows). FSB_SERVE_FUSED_ADMIT=1 runs each admitted
+    request's first frame inside the next decode frame instead of a frame of its own (ContinuousBatcher
+    fused_admission), with the same tokens. A request dict may carry `cancel` (a threading.Event): once it is set the request in flight is taken out
     of the scheduler, the plan ends and nothing more is put on its response queue."""
     from ...scheduler import Cancelled, ContinuousBatcher, SlotRequest, StreamClock
 
@@ -521,8 +523,9 @@ def serve_requests(model, input_queue: "queue.Queue", max_slots: int, frames_per
         max_live = max(max_slots, int(os.environ.get("FSB_SERVE_LIVE", "0") or 0))
         grow = serve_kv_grow(os.environ.get("FSB_SERVE_KV_GROW"), os.environ.get("FSB_SERVE_KV_GB"))
         compact = serve_compact(os.environ.get("FSB_SERVE_COMPACT"))
+        fused = serve_fused_admit(os.environ.get("FSB_SERVE_FUSED_ADMIT"))
         batcher = ContinuousBatcher(model, max_slots=max_slots, frames_per_poll=frames_per_poll, max_live=max_live,
-                                    kv_growth=grow, compact_rows=compact)
+                                    kv_growth=grow, compact_rows=compact, fused_admission=fused)
     paced = getattr(batcher, "max_live", 0) > getattr(batcher, "max_slots", 0)
     live = 0  # plans not yet exhausted
     waiting_queues: dict = {}  # id(plan) -> response queue of every plan that has a generate call in flight
@@ -708,6 +711,17 @@ def serve_compact(value: Optional[str]) -> bool:
     return True
 
 
+def serve_fused_admit(value: Optional[str]) -> bool:
+    """FSB_SERVE_FUSED_ADMIT: 1 = an admitted request's first frame runs as a row of the next decode frame, beside the
+    running requests, instead of a frame over the new rows alone (ContinuousBatcher fused_admission); unset, empty or
+    0 = off. A ValueError naming FSB_SERVE_FUSED_ADMIT for any other value."""
+    if value is None or value.strip() in ("", "0"):
+        return False
+    if value.strip() != "1":
+        raise ValueError(f"FSB_SERVE_FUSED_ADMIT={value!r} must be 0 or 1")
+    return True
+
+
 def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool = False):
     """inference.py:736-799: the model lives in ONE daemon worker thread fed by a queue; `None` shuts
     it down; errors are returned as WrappedGenerateResponse(status="error", response=exc).
@@ -725,9 +739,13 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
     FSB_SERVE_KV_GROW=1 (needs FSB_SERVE_KV_GB; else a ValueError naming both) maps a request's prompt and first frames
     at admission and further pages as it decodes; a request that cannot get its next page safely waits parked.
     FSB_SERVE_COMPACT=1 (0 or unset = off; else a ValueError naming it) keeps the live requests in the lowest slots and
-    decodes only the rows they occupy: an engine of 33..64 slots runs its faster 32-row frame while load fits in 32."""
+    decodes only the rows they occupy: an engine of 33..64 slots runs its faster 32-row frame while load fits in 32.
+    FSB_SERVE_FUSED_ADMIT=1 (0 or unset = off; else a ValueError naming it) runs an admitted request's first frame in
+    the next decode frame, beside the running requests, instead of a frame that streams the head and fast weights for
+    the new rows alone; the tokens are the same."""
     serve_kv_grow(os.environ.get("FSB_SERVE_KV_GROW"), os.environ.get("FSB_SERVE_KV_GB"))
     serve_compact(os.environ.get("FSB_SERVE_COMPACT"))
+    serve_fused_admit(os.environ.get("FSB_SERVE_FUSED_ADMIT"))
     input_queue = queue.Queue()
     init_event = threading.Event()
     init_error: list = []

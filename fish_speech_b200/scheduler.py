@@ -17,6 +17,10 @@ Compact rows (`ContinuousBatcher(compact_rows=True)`): a frame decodes rows [0, 
 every slot, and when the live requests fit in 32 rows the ones above them move down between two polls (the same park /
 resume, no K/V copied), so that an engine of more than 32 slots runs its 32-row step GEMMs whenever load allows;
 `compact_moves` is the whole policy.
+
+Fused admission (`ContinuousBatcher(fused_admission=True)`): an admitted request is prefilled without its first frame,
+which then runs as one more row of the poll's first decode frame (LmEngine.prefill defer_first_frame), with the same
+tokens; until that frame has run, the request is neither moved nor parked.
 """
 from __future__ import annotations
 
@@ -170,11 +174,12 @@ def kv_safe(avail: int, claims) -> bool:
 class ContinuousBatcher:
     def __init__(self, model, max_slots: int = 32, frames_per_poll: int = 8, min_free_to_admit: int = 1,
                  max_live: Optional[int] = None, clock: Callable[[], float] = time.monotonic, kv_growth: bool = False,
-                 compact_rows: bool = False):
+                 compact_rows: bool = False, fused_admission: bool = False):
         """`frames_per_poll`: decode frames between two looks at the device-side slot states (a finished slot
         idles for at most that many frames). `min_free_to_admit`: admissions wait until that many slots are
         free (or nothing is running) — every admission is one extra prefill pass + first frame that streams
-        all weights for the new rows only, so grouping them trades admission latency for throughput.
+        all weights for the new rows only, so grouping them trades admission latency for throughput. With
+        `fused_admission` the first frame rides in the running frame and only the prefill pass is extra.
         `max_live`: the most requests admitted at a time, running plus parked; the default, `max_slots`, means
         nothing is ever parked. `clock`: the time source of the pacing policy (seconds).
         `kv_growth`: on an engine whose page pool cannot hold every request at its full budget, a request maps its
@@ -185,7 +190,11 @@ class ContinuousBatcher:
         boundary, when the running requests fit in 32 rows, those in slots >= 32 move to the lowest free slots below 32
         (compact_moves; LmEngine.park_slot / resume_slot: a small state blob and a page-table row, no K/V copied). An
         engine of more than 32 slots then runs its 32-row step GEMMs, with the same bits. Off: every frame decodes
-        all `max_slots` rows and a request never changes slot unless it is parked."""
+        all `max_slots` rows and a request never changes slot unless it is parked.
+        `fused_admission`: an admitted request's prefill leaves its first frame (head, sampler, fast passes) to the
+        poll's first decode frame, where it runs as one more row beside the running requests, instead of a frame of
+        its own that streams the head and fast weights for the new rows alone; the tokens are the same, and the
+        request makes `frames_per_poll` frames in its first poll instead of one more. Off: as before."""
         from .models.text2semantic.inference import _ensure_engine
 
         if not 1 <= max_slots <= MAX_DECODE_BATCH:
@@ -199,6 +208,8 @@ class ContinuousBatcher:
             raise ValueError(f"max_live must be >= max_slots ({max_slots}), got {max_live}")
         self.clock = clock
         self.compact_rows = bool(compact_rows)
+        self.fused_admission = bool(fused_admission)
+        self._pending: set[int] = set()  # fused_admission: slots whose first frame the next decode frame runs
         self.moves = 0  # compact_rows: requests moved to a lower slot
         self.parked: list[SlotRequest] = []  # admitted, between two polls without a slot (SlotRequest._parked)
         self.frames_per_poll = int(frames_per_poll)
@@ -289,6 +300,7 @@ class ContinuousBatcher:
 
     def _park(self, req: SlotRequest):
         s = req.slot
+        assert s not in self._pending, f"slot {s} is parked before its first frame"
         req._parked = self.eng.park_slot(s, self._len.pop(s))
         del self.active[s]
         req.slot = -1
@@ -323,7 +335,8 @@ class ContinuousBatcher:
 
     def _compact(self):
         for frm, to in compact_moves(list(self.active), self._free_slots()):
-            self._move(self.active[frm], to)
+            if frm not in self._pending:  # a request waiting for its first frame stays in its slot
+                self._move(self.active[frm], to)
 
     def _schedule(self):
         """One scheduling decision (schedule_live) carried out: park, resume, admit, fill. With kv_growth, requests
@@ -416,7 +429,9 @@ class ContinuousBatcher:
         One page-table upload for all grants (LmEngine.grow_kv)."""
         ends, short = dict(self._grants), []
         claims = self._kv[1]
-        for req in sorted((r for r in self.active.values() if r.slot not in ends), key=lambda r: claims[r][0]):
+        # a request admitted with its first frame pending holds its first poll's pages from admission: nothing to grant
+        for req in sorted((r for r in self.active.values() if r.slot not in ends and r.slot not in self._pending),
+                          key=lambda r: claims[r][0]):
             end = self._grant(req)
             if end is None:
                 short.append(req)
@@ -463,6 +478,7 @@ class ContinuousBatcher:
         for r in reqs:
             del self.active[r.slot]
             del self._len[r.slot]
+            self._pending.discard(r.slot)  # a first frame still pending is dropped with the slot's state
             if hasattr(self.eng, "retire_slot"):
                 self.eng.retire_slot(r.slot)  # its pages stay a reusable prefix until the pool needs them
 
@@ -535,6 +551,9 @@ class ContinuousBatcher:
         # (with kv_growth: the prompt and the first poll's frames)
         kw = dict(kv_end=[int(r.prompt.size(1)) + (min(self.frames_per_poll, r._limit) if self.kv_growth else r._limit)
                           for r in batch]) if pool is not None else {}
+        if self.fused_admission:  # the first frames run in the next decode frame (_len above stays an upper bound)
+            kw["defer_first_frame"] = True
+            self._pending.update(slots)
         if any(r.reuse_prefix for r in batch) and hasattr(self.eng, "prefill_reusing"):
             self.eng.prefill_reusing([r.prompt for r in batch], slots, None, do_sample=True, **kw)
         else:
@@ -610,6 +629,7 @@ class ContinuousBatcher:
         # compact_rows: only rows up to the highest live slot, on the 32-row tile when that is at most 32 rows
         rows = 1 + max(self.active) if self.compact_rows else self.max_slots
         self.eng.decode(rows, k, None, use_graph=True)
+        self._pending.clear()
         self.frames_run += k
         self.slot_frames += k * len(self.active)
         return self._retire()

@@ -134,9 +134,23 @@ int fsb_lm_prefill(fsb_lm* h, const int32_t* d_tokens, const int32_t* d_row_slot
                    const int32_t* d_slots, int nseq, int do_sample, const fsb_sampling* s,
                    void* stream);
 
+/* Fused admission: fsb_lm_prefill with do_sample set, except that the sequences' first frames are not run here. Each
+ * sequence's last prompt row (its residual row and sums of squares) and position are staged for its slot d_slots[k]
+ * (h_slots[k] on the host: the same list), the slot is marked pending and parked at position -1. The next
+ * fsb_lm_decode runs its first frame with a splice after the slow stack that puts each pending slot's staged row into
+ * its decode row, and samples a row whose slot has produced no frame yet by the prefill's rule (no RAS); every request
+ * gets the tokens fsb_lm_prefill with do_sample would have given it, one fewer pass over the head and fast weights per
+ * admission. Needs slot control. A split prompt (longer than max_rows) defers with the call of its last rows; earlier
+ * pieces go through fsb_lm_prefill with do_sample = 0. While a slot is pending, fsb_lm_slot_save refuses it and
+ * fsb_lm_slot_restore into it drops the pending first frame; fsb_lm_decode needs every pending slot in [0, batch). */
+int fsb_lm_prefill_deferred(fsb_lm* h, const int32_t* d_tokens, const int32_t* d_row_slot, const int32_t* d_row_pos,
+                            int rows, const int32_t* d_last_rows, const int32_t* d_slots, int nseq,
+                            const int32_t* h_slots, void* stream);
+
 /* decode_n_tokens (inference.py:184-238): `nframes` more frames for slots [0, batch). One frame =
  * slow step + constrained sampling (+RAS) + num_codebooks fast steps; captured as a CUDA graph when
- * use_graph != 0. The per-frame <|im_end|> test is kept on the device (finished flags). */
+ * use_graph != 0. The per-frame <|im_end|> test is kept on the device (finished flags). After
+ * fsb_lm_prefill_deferred, the first frame is the fused one (its own graph). */
 int fsb_lm_decode(fsb_lm* h, int batch, int nframes, const fsb_sampling* s, int use_graph,
                   void* stream);
 
@@ -144,8 +158,8 @@ int fsb_lm_decode(fsb_lm* h, int batch, int nframes, const fsb_sampling* s, int 
  * and 32-row plans with the same stream-K schedule over the first 32 rows of the same buffers (fsb_lm_create fails if
  * the schedules differ). fsb_lm_decode runs a frame of batch <= 32 rows on the 32-row plans and a larger one on the
  * 64-row plans; every output element is the same sum of the same MMAs at either tile, so only the time differs.
- * Decode graphs are kept per (batch, tile, context bound, slot control, noise, sampling), up to 16 per engine, so
- * changing the row count or the tile between calls replays a captured frame once it has been seen.
+ * Decode graphs are kept per (batch, tile, context bound, slot control, fused first frame, noise, sampling), up to 16
+ * per engine, so changing the row count or the tile between calls replays a captured frame once it has been seen.
  * fsb_lm_set_decode_tile (test hook): 0 = by the row count (default), 32 or 64 = that tile for every frame (64 needs
  * an engine of more than 32 slots; a decode of more rows than a forced 32-row tile holds fails).
  * fsb_lm_decode_tile: the tile of the last fsb_lm_decode call (0 before the first). fsb_lm_graph_captures: decode

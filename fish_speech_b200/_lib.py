@@ -127,6 +127,7 @@ def lib() -> C.CDLL:
     L.fsb_lm_test_layer_gemms.argtypes = [vp, i32, i32, i32, i32, vp]
     L.fsb_lm_test_layer_attn.argtypes = [vp, i32, i32, i32, i32, vp]
     L.fsb_lm_test_prefill_stage.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]
+    L.fsb_lm_test_frame_stage.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, i32, C.POINTER(Sampling), vp]
     L.fsb_pcm_to_mono.argtypes = [vp, vp, i32, ll, vp, vp]
     L.fsb_resample.argtypes = [vp, vp, i32, ll, vp, vp]
     L.fsb_audio_out.argtypes = [vp, vp, i32, ll, vp, vp]

@@ -488,70 +488,6 @@ SampleArgs frame_sample_args(const fsb_lm* h, int p, const StepPartials& parts, 
     return a;
 }
 
-// Head + sampling + fast passes + bookkeeping for `rows` sequences whose last residual-stream rows (un-normed)
-// are in slow.xres[0..rows) with their sums of squares in slow.ssq, on the plans `fp`. inference.py:114-181.
-int run_frame_tail(fsb_lm* h, const FramePlans& fp, int rows, const int* row_slot, bool use_ras, bool first_frame,
-                   const int* set_pos_rows, const int* row_pos_src, const fsb_sampling& sp, cudaStream_t st) {
-    const fsb_lm_config& c = h->cfg;
-    const int C = c.num_codebooks;
-    const int* slots = row_slot ? row_slot : h->iota;
-    Stack& s = h->slow;
-    Stack& f = h->fast;
-    // ---- slow head over the selectable rows (the final norm is applied on load) ----
-    FSB_TRY(step_gemm_launch(*fp.head, rows, st));
-    const SampleArgs head_sample = frame_sample_args(h, 0, step_plan_partials(*fp.head), rows, row_slot, use_ras, sp);
-    FSB_TRY(first_frame ? launch_sample_first_frame(head_sample, st) : launch_sample(head_sample, st));
-
-    // ---- fast pass 0 input: hidden = norm(x) (norm_fastlayer_input) [-> fast_project_in]  (llama.py:459-461, 819-828)
-    RowsArgs hr{};
-    hr.x = s.xres;
-    hr.ssq_in = s.ssq;
-    hr.norm_w = c.norm_fastlayer_input ? h->norm_w : nullptr;
-    hr.rows = rows; hr.D = s.D; hr.eps = c.norm_eps;
-    if (h->has_proj) {
-        hr.y = h->hid_d;
-        FSB_TRY(launch_rows(hr, st));
-        FSB_TRY(step_gemm_launch(*fp.proj, rows, st));  // fast_project_in
-        FSB_TRY(step_finalize_launch(*fp.proj_out, rows, st));
-    } else {
-        hr.y = f.xres;
-        hr.ssq = f.ssq;
-        FSB_TRY(launch_rows(hr, st));
-    }
-    for (int p = 0; p < C; ++p) {
-        if (p > 0) {
-            // input = fast_embeddings[code_{p-1}] ; codes live in cur_tok[slot][p]
-            RowsArgs er{};
-            er.x = h->fast_emb;
-            er.y = f.xres;
-            er.ssq = f.ssq;
-            er.gather = h->cur_tok + p;
-            er.gather_map = row_slot;
-            er.gather_stride = C + 1;
-            er.rows = rows; er.D = f.D; er.eps = c.norm_eps;
-            FSB_TRY(launch_rows(er, st));
-        }
-        FSB_TRY(run_stack_decode(h, f, *fp.fast, rows, slots, h->fpos + p * h->rt, p == 0, st));
-        if (p == 0) continue;
-        FSB_TRY(step_gemm_launch(*fp.fast_out, rows, st));
-        FSB_TRY(launch_sample(frame_sample_args(h, p, step_plan_partials(*fp.fast_out), rows, row_slot, false, sp),
-                              st));
-    }
-    FrameEndArgs fe{};
-    fe.ctl = slot_ctl(h);
-    fe.cur_tok = h->cur_tok;
-    fe.out_tokens = h->out_tokens;
-    fe.n_out = h->n_out;
-    fe.pos = h->pos;
-    fe.row_slot = row_slot;
-    fe.set_pos_rows = set_pos_rows;
-    fe.row_pos_src = row_pos_src;
-    fe.step = h->step;
-    fe.rows = rows; fe.ncols = C + 1; fe.T_cap = c.max_frames;
-    FSB_TRY(launch_frame_end(fe, st));
-    return 0;
-}
-
 FirstFrameArgs first_frame_args(fsb_lm* h, int rows) {
     FirstFrameArgs a{};
     a.x = h->slow.xres;
@@ -567,15 +503,121 @@ FirstFrameArgs first_frame_args(fsb_lm* h, int rows) {
     return a;
 }
 
+// The launches of a decode frame around its two stacks, in launch order (fsb_lm_test_frame_stage runs any one of them):
+// embed, [slow stack], first-frame splice, slow head, fast pass 0 input, then per fast pass p: fast embed (p >= 1),
+// [fast stack], fast head (p >= 1); frame end.
+enum FrameStage { kFrEmbed = 0, kFrSplice, kFrHead, kFrFastIn, kFrFastEmbed, kFrFastHead, kFrEnd, kFrStages };
+
+// What the frame-tail stages of one call share: the frame's rows and the arguments that differ between a decode
+// frame and the prefill's tail.
+struct FrameRows {
+    int rows;
+    const int* row_slot;      // row i is slot row_slot[i] (NULL: slot i)
+    bool use_ras, first_frame;
+    const int* set_pos_rows;  // the prefill's tail: pos[slot] from row_pos_src[set_pos_rows[i]] (NULL: decode)
+    const int* row_pos_src;
+};
+
+// One stage of a frame on the plans `fp` (fast pass p for kFrFastEmbed / kFrFastHead): one place for decode_one_frame,
+// run_frame_tail and fsb_lm_test_frame_stage, so that the test hook launches exactly what a frame launches.
+int frame_stage(fsb_lm* h, const FramePlans& fp, int stage, int p, const FrameRows& fr, const fsb_sampling& sp,
+                cudaStream_t st) {
+    const fsb_lm_config& c = h->cfg;
+    const int C = c.num_codebooks;
+    const int rows = fr.rows;
+    const int* row_slot = fr.row_slot;
+    Stack& s = h->slow;
+    Stack& f = h->fast;
+    switch (stage) {
+        case kFrEmbed:  // decode row r is slot r
+            return launch_embed(embed_args(h, h->cur_tok, s.xres, s.ssq, rows), st);
+        case kFrSplice:
+            return launch_first_frame_splice(first_frame_args(h, rows), st);
+        case kFrHead: {
+            // slow head over the selectable rows (the final norm is applied on load)
+            FSB_TRY(step_gemm_launch(*fp.head, rows, st));
+            const SampleArgs head_sample =
+                frame_sample_args(h, 0, step_plan_partials(*fp.head), rows, row_slot, fr.use_ras, sp);
+            return fr.first_frame ? launch_sample_first_frame(head_sample, st) : launch_sample(head_sample, st);
+        }
+        case kFrFastIn: {
+            // fast pass 0 input: hidden = norm(x) (norm_fastlayer_input) [-> fast_project_in]
+            // (llama.py:459-461, 819-828)
+            RowsArgs hr{};
+            hr.x = s.xres;
+            hr.ssq_in = s.ssq;
+            hr.norm_w = c.norm_fastlayer_input ? h->norm_w : nullptr;
+            hr.rows = rows; hr.D = s.D; hr.eps = c.norm_eps;
+            if (h->has_proj) {
+                hr.y = h->hid_d;
+                FSB_TRY(launch_rows(hr, st));
+                FSB_TRY(step_gemm_launch(*fp.proj, rows, st));  // fast_project_in
+                return step_finalize_launch(*fp.proj_out, rows, st);
+            }
+            hr.y = f.xres;
+            hr.ssq = f.ssq;
+            return launch_rows(hr, st);
+        }
+        case kFrFastEmbed: {
+            // input = fast_embeddings[code_{p-1}] ; codes live in cur_tok[slot][p]
+            RowsArgs er{};
+            er.x = h->fast_emb;
+            er.y = f.xres;
+            er.ssq = f.ssq;
+            er.gather = h->cur_tok + p;
+            er.gather_map = row_slot;
+            er.gather_stride = C + 1;
+            er.rows = rows; er.D = f.D; er.eps = c.norm_eps;
+            return launch_rows(er, st);
+        }
+        case kFrFastHead:
+            FSB_TRY(step_gemm_launch(*fp.fast_out, rows, st));
+            return launch_sample(frame_sample_args(h, p, step_plan_partials(*fp.fast_out), rows, row_slot, false, sp),
+                                 st);
+        case kFrEnd: {
+            FrameEndArgs fe{};
+            fe.ctl = slot_ctl(h);
+            fe.cur_tok = h->cur_tok;
+            fe.out_tokens = h->out_tokens;
+            fe.n_out = h->n_out;
+            fe.pos = h->pos;
+            fe.row_slot = row_slot;
+            fe.set_pos_rows = fr.set_pos_rows;
+            fe.row_pos_src = fr.row_pos_src;
+            fe.step = h->step;
+            fe.rows = rows; fe.ncols = C + 1; fe.T_cap = c.max_frames;
+            return launch_frame_end(fe, st);
+        }
+    }
+    set_error("frame: no stage %d", stage);
+    return 1;
+}
+
+// Head + sampling + fast passes + bookkeeping for `rows` sequences whose last residual-stream rows (un-normed)
+// are in slow.xres[0..rows) with their sums of squares in slow.ssq, on the plans `fp`. inference.py:114-181.
+int run_frame_tail(fsb_lm* h, const FramePlans& fp, int rows, const int* row_slot, bool use_ras, bool first_frame,
+                   const int* set_pos_rows, const int* row_pos_src, const fsb_sampling& sp, cudaStream_t st) {
+    const FrameRows fr{rows, row_slot, use_ras, first_frame, set_pos_rows, row_pos_src};
+    const int* slots = row_slot ? row_slot : h->iota;
+    FSB_TRY(frame_stage(h, fp, kFrHead, 0, fr, sp, st));
+    FSB_TRY(frame_stage(h, fp, kFrFastIn, 0, fr, sp, st));
+    for (int p = 0; p < h->cfg.num_codebooks; ++p) {
+        if (p > 0) FSB_TRY(frame_stage(h, fp, kFrFastEmbed, p, fr, sp, st));
+        FSB_TRY(run_stack_decode(h, h->fast, *fp.fast, rows, slots, h->fpos + p * h->rt, p == 0, st));
+        if (p > 0) FSB_TRY(frame_stage(h, fp, kFrFastHead, p, fr, sp, st));
+    }
+    return frame_stage(h, fp, kFrEnd, 0, fr, sp, st);
+}
+
 // One frame over rows [0, batch) on the plans of row tile `tile` (batch <= tile). first_frame (fused admission): the
 // rows of slots whose first frame a deferred prefill left pending take their staged last prompt row between the slow
 // stack and the head, and sample it by the prefill's rule.
 int decode_one_frame(fsb_lm* h, int batch, int tile, const fsb_sampling& sp, bool first_frame, cudaStream_t st) {
-    Stack& s = h->slow;
     const FramePlans fp = frame_plans(h, tile);
-    FSB_TRY(launch_embed(embed_args(h, h->cur_tok, s.xres, s.ssq, batch), st));
-    FSB_TRY(run_stack_decode(h, s, *fp.slow, batch, h->iota, h->pos, false, st));
-    if (first_frame) FSB_TRY(launch_first_frame_splice(first_frame_args(h, batch), st));
+    const FrameRows fr{batch, nullptr, true, first_frame, nullptr, nullptr};
+    FSB_TRY(frame_stage(h, fp, kFrEmbed, 0, fr, sp, st));
+    FSB_TRY(run_stack_decode(h, h->slow, *fp.slow, batch, h->iota, h->pos, false, st));
+    if (first_frame) FSB_TRY(frame_stage(h, fp, kFrSplice, 0, fr, sp, st));
     return run_frame_tail(h, fp, batch, nullptr, true, first_frame, nullptr, nullptr, sp, st);
 }
 
@@ -761,7 +803,7 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &s.ssq, static_cast<size_t>(RT) * kSsqStride, "ssq_slow"));
     TRYC(dalloc(h, &f.xres, static_cast<size_t>(RT) * f.D, "x_fast"));
     TRYC(dalloc(h, &f.ssq, static_cast<size_t>(RT) * kSsqStride, "ssq_fast"));
-    TRYC(dalloc(h, &h->hid_d, static_cast<size_t>(RT) * Dm));
+    TRYC(dalloc(h, &h->hid_d, static_cast<size_t>(RT) * Dm, "fast_hidden"));
     TRYC(dalloc(h, &h->q_d, static_cast<size_t>(RT) * Qm, "q"));
     if (cfg->attn_split > 0)
         TRYC(dalloc(h, &h->span_ws,
@@ -802,9 +844,9 @@ int fsb_lm_create(const fsb_lm_config* cfg, const fsb_lm_weights* w, fsb_lm** ou
     TRYC(dalloc(h, &h->slot_top_k, cfg->max_batch, "slot_top_k"));
     TRYC(dalloc(h, &h->slot_seed, cfg->max_batch, "slot_seed"));
     TRYC(dalloc(h, &h->kv_miss, cfg->max_batch, "kv_miss"));
-    TRYC(dalloc(h, &h->stage_x, static_cast<size_t>(cfg->max_batch) * s.D));
-    TRYC(dalloc(h, &h->stage_ssq, static_cast<size_t>(cfg->max_batch) * kSsqStride));
-    TRYC(dalloc(h, &h->stage_pos, cfg->max_batch));
+    TRYC(dalloc(h, &h->stage_x, static_cast<size_t>(cfg->max_batch) * s.D, "first_frame_x"));
+    TRYC(dalloc(h, &h->stage_ssq, static_cast<size_t>(cfg->max_batch) * kSsqStride, "first_frame_ssq"));
+    TRYC(dalloc(h, &h->stage_pos, cfg->max_batch, "first_frame_pos"));
     TRYC(dalloc(h, &h->pending, cfg->max_batch, "first_frame_pending"));
     h->pending_host.assign(cfg->max_batch, 0);
     TRYC(dalloc(h, &h->iota, RT));
@@ -1189,6 +1231,36 @@ int fsb_lm_test_prefill_stage(fsb_lm* h, int layer, int stage, int rows, const i
     FSB_CHECK((stage != kPfQkv && stage != kPfAttn) || (d_row_seq != nullptr && d_row_pos != nullptr),
               "test_prefill_stage: stage %d needs the rows' sequences and positions", stage);
     return prefill_stage(h, layer, stage, rows, d_row_seq, d_row_pos, st);
+}
+
+int fsb_lm_test_frame_stage(fsb_lm* h, int stage, int tile, int rows, int p, const int32_t* d_row_slot,
+                            const int32_t* d_set_pos_rows, const int32_t* d_row_pos_src, int first_frame,
+                            const fsb_sampling* sp, void* stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    FSB_CHECK(h != nullptr, "test_frame_stage: null handle");
+    const fsb_lm_config& c = h->cfg;
+    FSB_CHECK(stage >= kFrEmbed && stage < kFrStages, "test_frame_stage: stage=%d outside [0, %d)", stage, kFrStages);
+    FSB_CHECK(tile == h->rt || (tile == kStepRows && h->rt == kStepRowsMax),
+              "test_frame_stage: tile=%d is not a row tile of this engine (%d%s)", tile, h->rt,
+              h->rt == kStepRowsMax ? " or 32" : "");
+    FSB_CHECK(rows >= 1 && rows <= std::min(tile, c.max_batch), "test_frame_stage: rows=%d outside [1, %d]", rows,
+              std::min(tile, c.max_batch));
+    const bool fast = stage == kFrFastEmbed || stage == kFrFastHead;
+    FSB_CHECK(!fast || (p >= 1 && p < c.num_codebooks), "test_frame_stage: p=%d outside [1, %d)", p,
+              c.num_codebooks);
+    FSB_CHECK((stage != kFrEmbed && stage != kFrSplice) || d_row_slot == nullptr,
+              "test_frame_stage: stage %d runs row r as slot r (no row_slot)", stage);
+    FSB_CHECK((d_set_pos_rows == nullptr) == (d_row_pos_src == nullptr),
+              "test_frame_stage: set_pos_rows and row_pos_src go together");
+    FSB_CHECK(!first_frame || (stage == kFrHead && d_set_pos_rows == nullptr),
+              "test_frame_stage: first_frame is a decode frame's slow head only");
+    FSB_CHECK(sp != nullptr || h->slot_control || (stage != kFrHead && stage != kFrFastHead),
+              "test_frame_stage: sampling parameters required");
+    const fsb_sampling sp_none{1.f, 1.f, 1, 0};
+    // a decode frame's arguments, or the prefill tail's (no RAS) when the positions come from the prefill's rows
+    const FrameRows fr{rows, d_row_slot, d_set_pos_rows == nullptr, first_frame != 0, d_set_pos_rows, d_row_pos_src};
+    return frame_stage(h, frame_plans(h, tile), stage, fast ? p : 0, fr, (sp && !h->slot_control) ? *sp : sp_none,
+                       st);
 }
 
 int fsb_lm_test_sample(fsb_lm* h, int fast, int cb_index, int rows, const int32_t* d_row_slot, const float* d_logits,

@@ -441,6 +441,13 @@ class LmEngine:
             "attn_prefill": ((R, c.n_head * c.head_dim), "<u2"),
             "h_prefill": ((R, c.intermediate_size), "<u2"),
             "ws_prefill": ((nbytes.value // 4,), "<f4"),
+            # frame tail (include/fishb200.h fsb_lm_test_frame_stage): the fast_project_in operand, rows at stride dim;
+            # fused admission's staged last prompt rows, by slot
+            "fast_hidden": ((rt * max(c.dim, c.fast_dim),), "<u2"),
+            "first_frame_x": ((self.max_batch, c.dim), "<u2"),
+            "first_frame_ssq": ((self.max_batch, 32), "<f4"),
+            "first_frame_pos": ((self.max_batch,), "<i4"),
+            "first_frame_pending": ((self.max_batch,), "<i4"),
         }
         shape, ts = shapes[name]
         with torch.cuda.device(self.device):
@@ -513,6 +520,27 @@ class LmEngine:
             _lib.check(self.lib.fsb_lm_test_prefill_stage(
                 self.h, int(layer), self.PREFILL_STAGES.index(stage), int(rows), *(
                     None if t is None else t.data_ptr() for t in (tok, seq, pos)), _stream()))
+            torch.cuda.current_stream().synchronize()
+
+    FRAME_STAGES = ("embed", "splice", "head", "fast_in", "fast_embed", "fast_head", "end")
+
+    def test_frame_stage(self, stage: str, rows: int, tile: Optional[int] = None, p: int = 0,
+                         row_slot: Optional[torch.Tensor] = None, set_pos_rows: Optional[torch.Tensor] = None,
+                         row_pos_src: Optional[torch.Tensor] = None, first_frame: bool = False,
+                         sp: Optional[_lib.Sampling] = None):
+        """Test hook (include/fishb200.h fsb_lm_test_frame_stage): one launch group of a decode frame around its stacks
+        over `rows` rows on the plans of row tile `tile` (default: the engine's), on the buffers as they are; fast pass
+        `p` for fast_embed / fast_head. row_slot / set_pos_rows / row_pos_src int32 on the device or None. Returns after
+        the stage has finished."""
+        def dev(t):
+            return None if t is None else t.to(device=self.device, dtype=torch.int32).contiguous()
+
+        rs, spr, rps = dev(row_slot), dev(set_pos_rows), dev(row_pos_src)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.fsb_lm_test_frame_stage(
+                self.h, self.FRAME_STAGES.index(stage), int(tile or self.row_tile), int(rows), int(p),
+                *(None if t is None else t.data_ptr() for t in (rs, spr, rps)), int(bool(first_frame)),
+                None if sp is None else C.byref(sp), _stream()))
             torch.cuda.current_stream().synchronize()
 
     # ---- paged slow KV cache (KvPagePool) --------------------------------------------------------------------------

@@ -245,7 +245,11 @@ int fsb_lm_reset(fsb_lm* h, void* stream);
  *   [R][n_head][head_dim], "attn_prefill" bf16 [R][n_head*head_dim], "h_prefill" bf16 [R][intermediate] and
  *   "ws_prefill" f32, flat: the fp32 result of the prefill GEMM run last, [rows][n_out] at a row stride of n_out
  *   ((n_head + 2 n_kv_head) * head_dim for qkv, dim for wo and w2, ceil(intermediate / 64) * 128 for w1|w3, whose
- *   columns are in the interleaved row order of the fused matrix) */
+ *   columns are in the interleaved row order of the fused matrix);
+ *   the frame-tail buffers (for fsb_lm_test_frame_stage): "fast_hidden" bf16 [RT * max(dim, fast_dim)] (the
+ *   fast_project_in operand, rows at stride dim), and fused admission's staged rows "first_frame_x" bf16
+ *   [max_batch][dim], "first_frame_ssq" f32 [max_batch][32], "first_frame_pos" int32 [max_batch] and
+ *   "first_frame_pending" int32 [max_batch] */
 int fsb_lm_buffer(fsb_lm* h, const char* name, void** d_ptr, size_t* bytes);
 
 /* Measurement hook for bench.py: launch every weight-streaming step GEMM of one decode frame `reps` times
@@ -502,6 +506,33 @@ int fsb_lm_test_layer_attn(fsb_lm* h, int fast, int layer, int rows, int kv_only
  * d_row_seq / d_row_pos int32 [rows] (stages 1 and 2). rows in [1, max(max_rows, 128)]. */
 int fsb_lm_test_prefill_stage(fsb_lm* h, int layer, int stage, int rows, const int32_t* d_tokens,
                               const int32_t* d_row_seq, const int32_t* d_row_pos, void* stream);
+
+/* Runs one launch group of a decode frame around its two stacks exactly as fsb_lm_decode (and, for the stages after
+ * the slow stack, fsb_lm_prefill's tail) does: the same function, the plans of row tile `tile` (the engine's RT, or 32
+ * on an RT = 64 engine), on the fsb_lm_buffer arrays as the caller left them. Row i is slot d_row_slot[i] (NULL: slot i;
+ * distinct slots in [0, max_batch), not checked). rows in [1, min(tile, max_batch)].
+ *   stage 0 (embed): "cur_tok"[r] -> "x_slow"[r] and "ssq_slow"[r] (row r is slot r; no d_row_slot)
+ *   stage 1 (first-frame splice): for each row r whose "first_frame_pending"[r] is set: if "slot_state"[r] is 1 or 3,
+ *           "first_frame_x" / "first_frame_ssq"[r] -> "x_slow" / "ssq_slow"[r] and "first_frame_pos"[r] -> "pos"[r];
+ *           the flag is cleared in every case (no d_row_slot)
+ *   stage 2 (slow head): the head GEMM of "x_slow" normalised on load with "norm" and "ssq_slow", then the slow
+ *           sampler -> "cur_tok"[slot][0] (and [1..C] at <|im_end|>), "ras_window", "finished", "slot_state",
+ *           "slow_logits" (debug engines); first_frame != 0: the first-frame sampler of fused admission
+ *   stage 3 (fast input): norm("x_slow") with "norm" if the model has norm_fastlayer_input (else a copy); with
+ *           fast_project_in -> "fast_hidden" (bf16 [RT][dim] at row stride dim), then its GEMM + bias (no residual)
+ *           -> "x_fast", "ssq_fast"; without it -> "x_fast", "ssq_fast" directly
+ *   stage 4 (fast embed, pass p in [1, C)): fast_embeddings["cur_tok"[slot][p]] -> "x_fast", "ssq_fast"
+ *   stage 5 (fast head, pass p in [1, C)): the fast_output GEMM of "x_fast" normalised on load with "fast_norm" and
+ *           "ssq_fast", then the codebook sampler -> "cur_tok"[slot][p + 1], "fast_logits"[p - 1] (debug engines)
+ *   stage 6 (frame end): for each live slot (any slot without slot control) "cur_tok"[slot] -> "out_tokens" at frame
+ *           "n_out"[slot] (not stored at or past max_frames), "n_out" + 1, "pos" + 1 unless the slot freezes at its
+ *           limit or <|im_end|> ("slot_state" = 2); then "step" + 1.
+ * d_set_pos_rows / d_row_pos_src (int32, both or neither): the prefill tail's arguments -- the head samples without
+ * RAS and the frame end sets pos[slot] = d_row_pos_src[d_set_pos_rows[i]] (+ 1 unless frozen); without them the stages
+ * take a decode frame's. The sampling stages read `s` (ignored with slot control, may be NULL then). */
+int fsb_lm_test_frame_stage(fsb_lm* h, int stage, int tile, int rows, int p, const int32_t* d_row_slot,
+                            const int32_t* d_set_pos_rows, const int32_t* d_row_pos_src, int first_frame,
+                            const fsb_sampling* s, void* stream);
 
 /* Runs the sampler (csrc/lm_kernels.cu sample_kernel) on its own for `rows` batch rows, with the arguments a decode
  * frame gives it: the slow head's (fast = 0, cb_index = 0; use_ras != 0 as in a decode frame, 0 as in the prefill's) or

@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import torch
 
-from tests.prefill_ref import rbf
+from tests.kernel_ref import rbf
 
 
 def embed_emul(tokens, emb, cb_emb, C, cs, sem_begin, sem_end, scale):

@@ -1,12 +1,99 @@
-"""Shared helpers for the LM parity tests (oracle config -> product model)."""
+"""Shared helpers for the LM tests: oracle config -> product model, the kernel tests' configurations and sweep tables,
+and the plumbing of their GPU modules."""
 from __future__ import annotations
 
 import ast
 
 import numpy as np
+import pytest
 import torch
 
 from oracle import lm_oracle as O
+
+
+def _lib():
+    from fish_speech_b200 import _lib
+
+    return _lib
+
+
+def _bits(t: torch.Tensor) -> torch.Tensor:
+    return t.view(torch.int16) if t.element_size() == 2 else t.view(torch.int32)
+
+
+def _gen(seed: int) -> torch.Generator:
+    return torch.Generator(device="cuda").manual_seed(seed)
+
+
+def _randn(shape, seed, scale=1.0) -> torch.Tensor:
+    return (torch.randn(shape, generator=_gen(seed), device="cuda") * scale).bfloat16()
+
+
+def _sms() -> int:
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the decode step GEMM's sweep (test_step_gemm_gpu, test_decode64_gpu)
+# ---------------------------------------------------------------------------------------------------------------------
+STAGES = (2, 3, 4, 8)  # 8 does not fit two CTAs per SM: step_plan_init shrinks it
+
+SHAPES = [
+    pytest.param(6144, 2560, id="s2pro-qkv"),
+    pytest.param(2560, 4096, id="s2pro-wo"),
+    pytest.param(19456, 2560, id="s2pro-w13"),
+    pytest.param(2560, 9728, id="s2pro-w2"),
+    pytest.param(4097, 2560, id="s2pro-head"),
+    pytest.param(4096, 2560, id="s2pro-fast-out"),
+    pytest.param(384, 256, id="tiny-qkv"),
+    pytest.param(96, 256, id="tiny-fast-out"),
+    pytest.param(97, 256, id="tiny-head"),
+    pytest.param(1, 1000, id="one-row-K1000"),  # partial last k-block (40 of 64) and a one-feature tile
+    pytest.param(200, 528, id="K528"),  # w2 with an intermediate size that is not a multiple of 64
+]
+
+
+def _ctas():
+    return (1, 2, 3, 7, 132, 2 * _sms(), 10 ** 6)  # 10^6: clamped to what one wave holds
+
+
+def layer_configs():
+    """name -> config of the decode layer GEMM tests."""
+    return {
+        # wo bias in both stacks; intermediate sizes that are not multiples of 64 (w1|w3 padded, w2 with K % 64 != 0)
+        "tiny": O.tiny_config(attention_o_bias=True, fast_attention_o_bias=True, intermediate_size=528,
+                              fast_intermediate_size=400),
+        # S2-Pro layer shapes with two layers per stack and a reduced vocabulary (test_lm_gpu.py builds it so too)
+        "s2pro": O.LMConfig(n_layer=2, n_fast_layer=2, vocab_size=8192, max_seq_len=256, semantic_begin_id=4000,
+                            semantic_end_id=8095, im_end_id=3999),
+    }
+
+
+def attn_configs():
+    """name -> (config, slots): every (head_dim, group) instance of the attention kernels in one stack or the other.
+    (Dh, G) per stack in the comments; both row tiles; qk-norm and qkv bias on and off."""
+    s2 = dict(vocab_size=8192, semantic_begin_id=4000, semantic_end_id=8095, im_end_id=3999, max_seq_len=32768)
+    return {
+        # slow (64, 8) norm; fast (128, 2) norm + bias
+        "tiny-a": (O.tiny_config(max_seq_len=1024, n_head=8, n_local_heads=1, head_dim=64, fast_n_head=2,
+                                 fast_n_local_heads=1, fast_head_dim=128, fast_attention_qk_norm=True,
+                                 fast_attention_qkv_bias=True), 32),
+        # slow (128, 1) bias; fast (64, 2) plain, behind fast_project_in (fast_dim != dim)
+        "tiny-b": (O.tiny_config(max_seq_len=1024, n_head=2, n_local_heads=2, head_dim=128, attention_qk_norm=False,
+                                 attention_qkv_bias=True, fast_dim=128, fast_n_head=4, fast_n_local_heads=2,
+                                 fast_head_dim=64), 64),
+        # slow (64, 1) norm + bias; fast (128, 8) norm
+        "tiny-c": (O.tiny_config(max_seq_len=1024, n_head=2, n_local_heads=2, head_dim=64, attention_qkv_bias=True,
+                                 fast_n_head=8, fast_n_local_heads=1, fast_head_dim=128, fast_attention_qk_norm=True),
+                   32),
+        # slow (128, 2) plain; fast (64, 4) bias
+        "tiny-d": (O.tiny_config(max_seq_len=1024, n_head=4, n_local_heads=2, head_dim=128, attention_qk_norm=False,
+                                 fast_attention_qkv_bias=True), 64),
+        # S2-Pro layers: slow (128, 4) norm, fast (128, 4) plain; 32 768 positions per slot
+        "s2pro": (O.LMConfig(n_layer=2, n_fast_layer=2, **s2), 64),
+        # slow (128, 8) norm: the smallest score buffer per position
+        "s2pro-g8": (O.LMConfig(n_layer=2, n_fast_layer=1, n_local_heads=4, **s2), 32),
+    }
 
 
 def model_args(cfg: O.LMConfig):

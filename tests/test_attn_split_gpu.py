@@ -4,7 +4,8 @@ spans of T positions at absolute positions, one CTA each, merged in ascending or
 
 What must hold, and what each test checks through the handle's own launch sequence (fsb_lm_test_layer_attn) or end to
 end:
-  * long rows against float64: the reference, the brackets and the wrong references of tests/test_decode_attn_gpu.py.
+  * long rows against float64: the reference, the brackets and the wrong references of tests/test_decode_attn_gpu.py
+    (the case harness of tests/decode_attn_case.py).
     The tolerance is that module's bound for the unsplit kernel, unchanged: it counts ceil(L / 8) + 9 fp32
     accumulations of the weighted values and ceil(L / 32) + 8 of the sum of exponentials, and the split does fewer of
     each per span (ceil(T / 8) + 8, ceil(T / 32) + 5) plus one product with exp(m_s - M) (expf's 2 ulp, already in
@@ -25,8 +26,9 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.lm_util import make_prompt, model_args
-from tests.test_decode_attn_gpu import PAGE, TEETH, Geom, State, _bits, _check_case, _configs, _lib, _report_teeth
+from tests.decode_attn_case import TEETH, Geom, State, _check_case, _report_teeth
+from tests.kernel_ref import PAGE
+from tests.lm_util import _bits, _lib, attn_configs, make_prompt, model_args
 
 pytestmark = pytest.mark.gpu
 
@@ -35,7 +37,8 @@ _ENG: dict = {}
 
 def _split_configs():
     """name -> (config, slots, T). test_decode_attn_gpu's geometries and the default tiny one, slow (64, 4)."""
-    out = {name: (cfg, slots, 2048 if cfg.max_seq_len > 16384 else 128) for name, (cfg, slots) in _configs().items()}
+    out = {name: (cfg, slots, 2048 if cfg.max_seq_len > 16384 else 128)
+           for name, (cfg, slots) in attn_configs().items()}
     out["tiny-e"] = (O.tiny_config(max_seq_len=1024), 32, 128)
     return out
 

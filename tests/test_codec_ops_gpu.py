@@ -79,12 +79,12 @@ import torch
 import torch.nn.functional as F
 
 from oracle import codec_oracle as CO
-from tests.test_step_gemm_gpu import _bracket_bf16, _check_rounded, bf16_key, rbf
+from tests.kernel_ref import C_CONV, bf16_key, bracket_bf16, check_bracket, rbf
+from tests.lm_util import _bits, _gen, _lib, _randn
 
 pytestmark = pytest.mark.gpu
 
 U = 2.0 ** -24
-C_CONV = 2.0 ** -18  # conv GEMM accumulation, relative to |W| |X| (module docstring)
 SECOND_ORDER = 1 + 2.0 ** -10
 G_ERF = 2.0 ** -20  # GELU allowance, relative to 0.5 |x| (module docstring)
 SIN_ACC = 2.0 ** -23  # sinf: 2 ulp of a value below 1
@@ -101,12 +101,6 @@ TEETH = {"cb-semantic": 0.9, "ln-eps": 0.9, "dw-shift": 0.9, "dw-window": 0.9, "
          "win": 0.9}
 
 
-def _lib():
-    from fish_speech_b200 import _lib
-
-    return _lib
-
-
 def _L():
     return _lib().lib()
 
@@ -117,18 +111,6 @@ def _check(rc):
 
 def _st():
     return torch.cuda.current_stream().cuda_stream
-
-
-def _gen(seed):
-    return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def _randn(shape, seed, scale=1.0):
-    return (torch.randn(shape, generator=_gen(seed), device="cuda") * scale).bfloat16()
-
-
-def _bits(t):
-    return t.view(torch.int16) if t.element_size() == 2 else t.view(torch.int32)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -283,9 +265,9 @@ def test_codebook_sum(name, request):
         t64 = (cb @ Wo.T + bo)[ci[:, s]]
         tabs64.append(t64)
         E = E + (cfg.codebook_dim + 1) * U * tab_abs[ci[:, s]] + S * U * t64.abs()
-    _check_rounded(out.float(), *_bracket_bf16(v, E), rbf(v), f"{name}: codebook_sum")
+    check_bracket(out.float(), *bracket_bf16(v, E), f"{name}: codebook_sum", rbf(v))
     teeth = Teeth()
-    teeth.add("cb-semantic", out.float(), *_bracket_bf16(v - tabs64[0], E))
+    teeth.add("cb-semantic", out.float(), *bracket_bf16(v - tabs64[0], E))
     teeth.report(f"{name} codebook_sum")
 
 
@@ -376,16 +358,16 @@ def test_dwconv_ln(C, T, request):
     torch.cuda.synchronize()
     v, E, var = _dwconv_ln_ref(w, prefix, x)
     got = y.float()
-    _check_rounded(got, *_bracket_bf16(v, E), rbf(v), f"dwconv_ln C={C} T={T}")
+    check_bracket(got, *bracket_bf16(v, E), f"dwconv_ln C={C} T={T}", rbf(v))
     assert tiny_var.any() and offset.any() and (var[tiny_var] < 1e-5).all()
     teeth = Teeth()
     v5 = _dwconv_ln_ref(w, prefix, x, eps=1e-5)[0]
-    teeth.add("ln-eps", got, *_bracket_bf16(v5, E), mask=tiny_var)
+    teeth.add("ln-eps", got, *bracket_bf16(v5, E), mask=tiny_var)
     if T > 1:
         vs = _dwconv_ln_ref(w, prefix, x, shift=1)[0]
         rows = torch.zeros(B, T, dtype=torch.bool, device="cuda")
         rows[:, 1:] = True
-        teeth.add("dw-shift", got, *_bracket_bf16(vs, E), mask=rows & ~tiny_var & ~offset)
+        teeth.add("dw-shift", got, *bracket_bf16(vs, E), mask=rows & ~tiny_var & ~offset)
     teeth.report(f"dwconv_ln C={C} T={T}")
 
 
@@ -402,14 +384,14 @@ def test_dwconv_ln_window(full):
     torch.cuda.synchronize()
     v, E, _ = _dwconv_ln_ref(full.w, prefix, x)
     got = y.float()
-    _check_rounded(got, *_bracket_bf16(v[:, H:], E[:, H:]), rbf(v[:, H:]), "dwconv_ln_window")
+    check_bracket(got, *bracket_bf16(v[:, H:], E[:, H:]), "dwconv_ln_window", rbf(v[:, H:]))
     x0 = x.clone()
     x0[:, :H] = 0
     v0 = _dwconv_ln_ref(full.w, prefix, x0)[0]
     teeth = Teeth()
     first = torch.zeros(B, n, dtype=torch.bool, device="cuda")
     first[:, : H] = True
-    teeth.add("dw-window", got, *_bracket_bf16(v0[:, H:], E[:, H:]), mask=first)
+    teeth.add("dw-window", got, *bracket_bf16(v0[:, H:], E[:, H:]), mask=first)
     teeth.report("dwconv_ln_window")
 
 
@@ -457,14 +439,14 @@ def test_first_conv(name, T, alphas, request):
         return v, (K + 1) * U * A
 
     v, E = ref()
-    _check_rounded(raw.float(), *_bracket_bf16(v, E), rbf(v), f"first_conv {name} T={T} raw")
+    check_bracket(raw.float(), *bracket_bf16(v, E), f"first_conv {name} T={T} raw", rbf(v))
     y, Ey = _snake_ref(v, E, a64, lambda z: SIN_ACC)
     ref_y = _cl(CO.snake(_cl(v), a64[None, :, None]))
     assert torch.allclose(ref_y, y, rtol=0, atol=1e-12)
-    _check_rounded(act.float(), *_bracket_bf16(y, Ey), rbf(y), f"first_conv {name} T={T} act")
+    check_bracket(act.float(), *bracket_bf16(y, Ey), f"first_conv {name} T={T} act", rbf(y))
     teeth = Teeth()
     vs, _ = ref(shift=1)
-    teeth.add("fc-shift", raw.float(), *_bracket_bf16(vs, E))
+    teeth.add("fc-shift", raw.float(), *bracket_bf16(vs, E))
     teeth.report(f"first_conv {name} T={T}")
 
 
@@ -552,10 +534,10 @@ def test_snake(name, request):
     assert torch.allclose(CO.snake(v.T, a64[:, None]).T, ys, rtol=0, atol=1e-12)
     got = y.reshape(-1)[:n].float()
     ys, Ey = ys.reshape(-1)[:n], Ey.reshape(-1)[:n]
-    _check_rounded(got, *_bracket_bf16(ys, Ey), rbf(ys), f"snake {name}")
+    check_bracket(got, *bracket_bf16(ys, Ey), f"snake {name}", rbf(ys))
     teeth = Teeth()
     yw, _ = _snake_ref(v, torch.zeros_like(v), a64.roll(1), lambda z: SIN_ACC)
-    teeth.add("snake-alpha", got, *_bracket_bf16(yw.reshape(-1)[:n], Ey))
+    teeth.add("snake-alpha", got, *bracket_bf16(yw.reshape(-1)[:n], Ey))
     teeth.report(f"snake {name}")
 
 
@@ -674,7 +656,7 @@ def _leak_teeth(teeth, got, vfn, x64, E, rows):
     """Batch 1 computed with batch 0's tail as its history: the first `rows` outputs of batch 1."""
     cat = torch.cat([x64[0], x64[1]], -1)[None]
     vw = vfn(cat)[..., -vfn(x64[1:]).shape[-1]:]  # batch 1's outputs, [1, C, T_out]
-    lo, hi = _bracket_bf16(_cl(vw)[0], E[1])
+    lo, hi = bracket_bf16(_cl(vw)[0], E[1])
     m = torch.zeros_like(lo, dtype=torch.bool)
     m[:rows] = True
     teeth.add("leak", got[1], lo, hi, mask=m)
@@ -695,10 +677,10 @@ def test_conv_gemm_convnext_linears(name, request):
     W1 = g.w[f"{prefix}.pwconv1.weight"].bfloat16().double().cuda()
     b1 = g.w[f"{prefix}.pwconv1.bias"].double().cuda()
     v, E = _epi(F.linear(x.double(), W1), F.linear(x.double().abs(), W1.abs()), bias=b1, gelu=True)
-    _check_rounded(h.float(), *_bracket_bf16(v, E), rbf(v), f"{name} pw1")
+    check_bracket(h.float(), *bracket_bf16(v, E), f"{name} pw1", rbf(v))
     teeth = Teeth()
     vt = F.gelu(F.linear(x.double(), W1, b1), approximate="tanh")
-    teeth.add("gelu-tanh", h.float(), *_bracket_bf16(vt, E))
+    teeth.add("gelu-tanh", h.float(), *bracket_bf16(vt, E))
     # pw2, in place on the residual stream
     W2 = g.w[f"{prefix}.pwconv2.weight"].bfloat16().double().cuda()
     b2 = g.w[f"{prefix}.pwconv2.bias"].double().cuda()
@@ -710,7 +692,7 @@ def test_conv_gemm_convnext_linears(name, request):
     torch.cuda.synchronize()
     v, E = _epi(F.linear(hh.double(), W2), F.linear(hh.double().abs(), W2.abs()), bias=b2, gamma=gam,
                 resid=r0.double())
-    _check_rounded(r.float(), *_bracket_bf16(v, E), rbf(v), f"{name} pw2")
+    check_bracket(r.float(), *bracket_bf16(v, E), f"{name} pw2", rbf(v))
     teeth.report(f"{name} convnext linears")
 
 
@@ -748,10 +730,10 @@ def test_conv_gemm_encoder_strided(name, bi, request):
     v, E = _epi(_cl(CO.causal_conv(_d(W, None), "c", x64, stride=s)),
                 _cl(CO.causal_conv(_d(W.abs(), None), "c", x64.abs(), stride=s)), bias=b)
     assert torch.allclose(v, vraw, rtol=1e-12, atol=1e-9)
-    _check_rounded(out0.float(), *_bracket_bf16(v, E), rbf(v), f"{name} enc{bi} raw")
+    check_bracket(out0.float(), *bracket_bf16(v, E), f"{name} enc{bi} raw", rbf(v))
     if nxt is not None:
         y, Ey = _snake_ref(v, E, _alpha(g, nxt_p), allow_sin)
-        _check_rounded(out1.float(), *_bracket_bf16(y, Ey), rbf(y), f"{name} enc{bi} snake")
+        check_bracket(out1.float(), *bracket_bf16(y, Ey), f"{name} enc{bi} snake", rbf(y))
     teeth = Teeth()
     _leak_teeth(teeth, out0.float(), vfn, x64, E, 1)
     teeth.report(f"{name} enc{bi}")
@@ -780,17 +762,17 @@ def test_conv_gemm_decoder_transposed(name, bi, request):
     v, E = _epi(_cl(CO.causal_conv_transpose(_d(W, None), "c", x64, s)),
                 _cl(CO.causal_conv_transpose(_d(W.abs(), None), "c", x64.abs(), s)), bias=b)  # [B, T*s, cout]
     g0, g1 = out0.view(B, T * s, cout).float(), out1.view(B, T * s, cout).float()
-    _check_rounded(g0, *_bracket_bf16(v, E), rbf(v), f"{name} dec{bi} convT raw")
+    check_bracket(g0, *bracket_bf16(v, E), f"{name} dec{bi} convT raw", rbf(v))
     alpha = _alpha(g, f"{p}.2.block.0")
     y, Ey = _snake_ref(v, E, alpha, allow_sin)
     assert torch.allclose(_cl(CO.snake(_cl(v), alpha[None, :, None])), y, rtol=0, atol=1e-9)
-    _check_rounded(g1, *_bracket_bf16(y, Ey), rbf(y), f"{name} dec{bi} convT snake")
+    check_bracket(g1, *bracket_bf16(y, Ey), f"{name} dec{bi} convT snake", rbf(y))
     teeth = Teeth()
     # alphas in (co, p) order: GEMM channel j = p * cout + co would get alpha[j // s]
     wrong = alpha.repeat_interleave(s).view(s, cout)  # [p, co]
     vv = v.view(B, T, s, cout)
     yw, _ = _snake_ref(vv, E.view(B, T, s, cout), wrong, allow_sin)
-    lo, hi = _bracket_bf16(yw.view(B, T * s, cout), Ey)
+    lo, hi = bracket_bf16(yw.view(B, T * s, cout), Ey)
     changed = (wrong != alpha[None, :]).expand(B, T, s, cout).reshape(B, T * s, cout)
     teeth.add("snake-co-p", g1, lo, hi, mask=changed)
     _leak_teeth(teeth, g0, vfn, x64, E, s)
@@ -820,7 +802,7 @@ def test_conv_gemm_window(full):
                 _cl(CO.causal_conv(_d(W.abs(), None), "c", x64.abs(), dilation=dil))[:, H:], bias=b)
     alpha = _alpha(g, f"{prefix}.block.2")
     y, Ey = _snake_ref(v, E, alpha, allow_sin)
-    _check_rounded(out1.float(), *_bracket_bf16(y, Ey), rbf(y), "window conv7")
+    check_bracket(out1.float(), *bracket_bf16(y, Ey), "window conv7", rbf(y))
     teeth = Teeth()
     x0 = x64.clone()
     x0[..., :H] = 0
@@ -828,7 +810,7 @@ def test_conv_gemm_window(full):
     y0, _ = _snake_ref(v0, E, alpha, allow_sin)
     m = torch.zeros(nb, n, C, dtype=torch.bool, device="cuda")
     m[:, :H] = True
-    teeth.add("win", out1.float(), *_bracket_bf16(y0, Ey), mask=m)
+    teeth.add("win", out1.float(), *bracket_bf16(y0, Ey), mask=m)
     teeth.report("window conv7")
 
 

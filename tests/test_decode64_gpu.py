@@ -15,19 +15,13 @@ import pytest
 import torch
 
 from oracle import lm_oracle as O
-from tests.lm_util import build_model, make_prompt
-from tests.test_step_gemm_gpu import (SHAPES, STAGES, _configs, _ctas, _gen, _randn, _sms, acc_bound, fp64_gemm,
-                                      norm_operand, tile_ssq)
+from tests.kernel_ref import acc_bound, fp64_gemm, norm_operand, tile_ssq
+from tests.lm_util import (SHAPES, STAGES, _bits, _ctas, _gen, _lib, _randn, _sms, build_model, layer_configs,
+                           make_prompt)
 
 pytestmark = pytest.mark.gpu
 
 ROWS64 = (1, 33, 47, 64)
-
-
-def _lib():
-    from fish_speech_b200 import _lib
-
-    return _lib
 
 
 def step_gemm_tile(w, x, row_tile, rows, num_ctas, stages, norm_w=None, ssq=None, eps=1e-6):
@@ -44,10 +38,6 @@ def step_gemm_tile(w, x, row_tile, rows, num_ctas, stages, norm_w=None, ssq=None
     return out[:rows], dict(ctas=info[0], stages=info[1], parts=info[2], units=info[3], items=info[4])
 
 
-def _bits(t: torch.Tensor) -> torch.Tensor:
-    return t.contiguous().view(torch.int32)
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # one GEMM at RT = 64 against float64, over the shapes and schedules of test_step_gemm_matches_fp64
 # ---------------------------------------------------------------------------------------------------------------------
@@ -55,7 +45,7 @@ def _bits(t: torch.Tensor) -> torch.Tensor:
 def test_step_gemm64_matches_fp64(n_out, K):
     w = _randn((n_out, K), seed=n_out * 7 + K)
     x = _randn((64, K), seed=n_out * 7 + K + 3)
-    ref, absprod = fp64_gemm(w, x)
+    ref, absprod = fp64_gemm(x, w)
     tiles, kblocks = math.ceil(n_out / 128), math.ceil(K / 64)
     infos = []
     for ci, ctas in enumerate(_ctas()):
@@ -88,7 +78,7 @@ def test_step_gemm64_keeps_two_ctas_per_sm_at_the_engine_schedule():
             x = _randn((rt, K), seed=K)
             ssq = torch.zeros(rt, 32, device="cuda") if norm else None
             if norm:
-                ssq[:, : math.ceil(K / 128)] = tile_ssq(x)
+                ssq[:, : math.ceil(K / 128)] = tile_ssq(x).float()
             infos.append(step_gemm_tile(w, x, rt, rt, 2 * _sms(), 4, nw, ssq)[1])
         assert infos[0] == infos[1], infos
         assert infos[1]["ctas"] == 2 * _sms() and infos[1]["stages"] == 4, infos[1]
@@ -109,7 +99,7 @@ def test_step_gemm64_halves_equal_the_32_row_tile_bitwise(n_out, K, norm):
     nt = math.ceil(K / 128)
     ssq = torch.full((64, 32), float("nan"), device="cuda")
     if norm:
-        ssq[:, :nt] = tile_ssq(x)
+        ssq[:, :nt] = tile_ssq(x).float()
     s = ssq if norm else None
     full, _ = step_gemm_tile(w, x, 64, 64, *sched, nw, s, eps)
     assert torch.isfinite(full).all()
@@ -138,7 +128,7 @@ def test_step_gemm64_normalise_on_load_identity():
     x = (_randn((64, K), seed=K + 11) * scale).bfloat16()
     nw = (1 + 0.1 * torch.randn(K, generator=_gen(K + 12), device="cuda")).bfloat16()
     ssq = torch.full((64, 32), float("nan"), device="cuda")
-    ssq[:, :nt] = tile_ssq(x)
+    ssq[:, :nt] = tile_ssq(x).float()
     eye = torch.eye(K, device="cuda").bfloat16()
     for ctas, stages in ((7, 3), (2 * _sms(), 4)):
         out, info = step_gemm_tile(eye, x, 64, 64, ctas, stages, nw, ssq, eps)
@@ -164,7 +154,7 @@ def layer_models():
                 for e in m[1:]:
                     e.engine.close()
             built.clear()
-            cfg = _configs()[name]
+            cfg = layer_configs()[name]
             w = O.make_weights(cfg, seed=97)
             built[name] = (cfg, build_model(cfg, w, max_batch=64, debug=False, max_rows=128),
                            build_model(cfg, w, max_batch=32, debug=False, max_rows=128))

@@ -5,7 +5,7 @@ import torch
 
 from oracle import lm_oracle as O
 from tests import frame_ref as F
-from tests.prefill_ref import embed_ref, rbf
+from tests.kernel_ref import embed_ref, rbf
 
 
 def _cfg(**over):

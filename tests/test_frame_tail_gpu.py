@@ -3,7 +3,7 @@ against float64 references and exact models: the decode embed, the first-frame s
 pass 0 input (norm_fastlayer_input, fast_project_in), the fast embed and head of passes p >= 1, and the frame end. Each
 test writes its stage's inputs itself (teacher forcing), so an error in one stage cannot reach the next; the fast
 stack's layers are covered by test_step_gemm_gpu.py and test_decode_attn_gpu.py. The helpers live in tests/frame_ref.py
-(rehearsed on the CPU by test_frame_tail_cpu.py), tests/prefill_ref.py and test_step_gemm_gpu.py.
+(rehearsed on the CPU by test_frame_tail_cpu.py) and tests/kernel_ref.py.
 
 Heads. logits = rbf(W X'), X' = norm(x) normalised on load (the final `norm` for the slow head, `fast_norm` for the
 codebook heads) with the sums of squares the test wrote. norm_operand brackets X' over rsqrtf's 2 ulp; the step GEMM's
@@ -27,8 +27,9 @@ import pytest
 import torch
 
 from tests import frame_ref as F
-from tests.prefill_ref import embed_ref, rbf
-from tests.test_step_gemm_gpu import C_AMB, _bracket_bf16, norm_operand, tile_ssq
+from tests.kernel_ref import (C_AMB, bracket_bf16, check_bracket, check_ssq, check_tally, embed_ref, norm_operand,
+                              normed_gemm, rbf, tile_ssq)
+from tests.lm_util import _bits, _gen
 
 pytestmark = pytest.mark.gpu
 
@@ -82,10 +83,6 @@ def _free_engines():
     _ENG.clear()
 
 
-def _gen(seed):
-    return torch.Generator(device="cuda").manual_seed(seed)
-
-
 def _rows(eng):
     return (1, 13, 32) + ((33, 64) if eng.max_batch == 64 else ())
 
@@ -101,10 +98,6 @@ def _tile(eng, rows):
     return 32 if rows <= 32 else 64
 
 
-def _bits(t):
-    return t.view(torch.int16) if t.element_size() == 2 else t.view(torch.int32)
-
-
 def _same(a, b):
     return torch.equal(_bits(a.contiguous()), _bits(b.contiguous()))
 
@@ -117,41 +110,14 @@ def _resid_rows(eng, D, rows, seed):
     x = (torch.randn(RT, D, generator=_gen(seed), device="cuda") * scale).bfloat16()
     x[rows:] = float("nan")
     ssq = torch.full((RT, 32), float("nan"), device="cuda")
-    ssq[:rows, : math.ceil(D / 128)] = tile_ssq(x[:rows])
+    ssq[:rows, : math.ceil(D / 128)] = tile_ssq(x[:rows]).float()
     return x, ssq
-
-
-def _check_ssq(ssq, x, what):
-    """The sums of squares a kernel left for its rows x: within 2^-16 of float64, NaN in the tiles past the row's."""
-    nt = math.ceil(x.shape[1] / 128)
-    want = tile_ssq(x).double()
-    rel = ((ssq[:, :nt].double() - want).abs() / want.clamp(min=1e-30)).max()
-    assert rel <= 2.0 ** -16, f"{what}: sums of squares off by {float(rel):.3g} (relative)"
-    assert torch.isnan(ssq[:, nt:]).all(), f"{what}: sums of squares written past the row's {nt} tiles"
-
-
-def _inside(got, lo, hi, mid, what, tally):
-    """got inside [lo, hi] (bit-identical where lo == hi); counts the elements that differ from mid into tally, whose
-    share _check_share bounds over a whole test (a single row of 96 logits cannot show a share below 1 %)."""
-    inside = (got >= lo) & (got <= hi)
-    assert inside.all(), (f"{what}: off at {(~inside).nonzero()[0].tolist()} ({int((~inside).sum())} of "
-                          f"{got.numel()}): got {float(got[~inside][0])} want {float(mid[~inside][0])}")
-    tally[0] += int((got != mid).sum())
-    tally[1] += got.numel()
-
-
-def _check_share(tally, what):
-    assert tally[0] == 0 or tally[0] < 0.01 * tally[1], f"{what}: {tally[0]} of {tally[1]} elements differ from float64"
 
 
 def _head_bracket(x, ssq, norm_w, W, eps):
     """(lo, hi, mid) of rbf(W X') with X' = norm(x) normalised on load (module docstring)."""
-    mid, lo, hi = norm_operand(x, ssq, norm_w, eps, x.shape[1])
-    W64 = W.double()
-    v = mid.double() @ W64.T
-    E = C_AMB * (torch.maximum(lo.abs(), hi.abs()).double() @ W64.abs().T) + (hi - lo).double() @ W64.abs().T
-    b_lo, b_hi = _bracket_bf16(v, E)
-    return b_lo, b_hi, rbf(v)
+    v, E = normed_gemm(x, ssq, norm_w, eps, W)
+    return *bracket_bf16(v, E), rbf(v)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -198,7 +164,7 @@ def test_decode_embed(name):
         assert not bad.any(), f"{what}: {int(bad.sum())} elements differ from the emulation, first {bad.nonzero()[0]}"
         lo, hi, mid, x64 = embed_ref(tok[:rows], emb, cb, C, cfg.codebook_size, cfg.semantic_begin_id,
                                      cfg.semantic_end_id, cfg.scale_codebook_embeddings)
-        _inside(x, lo, hi, mid, what, tally)
+        check_bracket(x, lo, hi, what, mid, tally=tally)
         # the bracket's float64 centre is oracle.embed on the clamped ids (the clamps keep each row's semantic flag)
         clamped = tok[:rows].long().clone()
         clamped[:, 0] = clamped[:, 0].clamp(0, cfg.vocab_size - 1)
@@ -207,10 +173,10 @@ def test_decode_embed(name):
                              for k in ("embeddings.weight", "codebook_embeddings.weight")})
         ref = O.embed(st, clamped[:, :, None])[:, 0]
         assert torch.allclose(ref, x64, rtol=0, atol=1e-12), f"{what}: embed_ref's centre is not oracle.embed"
-        _check_ssq(sb[:rows], xb[:rows], what)
+        check_ssq(sb[:rows], xb[:rows], what, nan_past=True)
         assert (xb[rows:].float() == SENTINEL).all() and torch.isnan(sb[rows:]).all(), f"{what}: rows past rows written"
         assert torch.equal(ct, tok), f"{what}: cur_tok written"
-    _check_share(tally, f"{name} embed")
+    check_tally(tally, f"{name} embed")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -245,7 +211,7 @@ def test_slow_head(name):
                 lg.fill_(float("nan"))
                 eng.test_frame_stage("head", rows, tile=tile, row_slot=rs, sp=_sp(eng))
                 got = lg[slots]
-                _inside(got, lo, hi, mid, f"{what} tile={tile}", tally)
+                check_bracket(got, lo, hi, f"{what} tile={tile}", mid, tally=tally)
                 others = torch.ones(eng.max_batch, dtype=torch.bool, device="cuda")
                 others[slots] = False
                 assert torch.isnan(lg[others]).all(), f"{what}: logits of slots outside the rows written"
@@ -261,7 +227,7 @@ def test_slow_head(name):
                     first = got.clone()
                 else:
                     assert _same(got, first), f"{what}: the 32- and 64-row tiles differ"
-    _check_share(tally, f"{name} slow head")
+    check_tally(tally, f"{name} slow head")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -289,7 +255,7 @@ def test_fast_input(name):
         h = (hid[: rows * D].view(rows, D) if proj else xf[:rows]).float()
         if norm:
             mid, lo, hi = norm_operand(x[:rows], ssq[:rows], w["norm.weight"], cfg.norm_eps, D)
-            _inside(h, lo, hi, mid, f"{what}: normed hidden", tally)
+            check_bracket(h, lo, hi, f"{what}: normed hidden", mid, tally=tally)
         else:
             assert _same(h.bfloat16(), x[:rows]), f"{what}: the plain copy is not bit-exact"
         if proj:
@@ -298,11 +264,11 @@ def test_fast_input(name):
             hb = hid[: rows * D].view(rows, D)
             # rbf(y + b) with no residual: the finalize's rounding of y + b may go either way within C_AMB |W||h|
             v = hb.double() @ Wp.double().T + b.double()[None, :]
-            y_lo, y_hi = _bracket_bf16(v, C_AMB * (hb.double().abs() @ Wp.double().abs().T))
-            _inside(xf[:rows].float(), y_lo, y_hi, rbf(v), f"{what}: fast_project_in", tally)
-        _check_ssq(sf[:rows], xf[:rows], what)
+            y_lo, y_hi = bracket_bf16(v, C_AMB * (hb.double().abs() @ Wp.double().abs().T))
+            check_bracket(xf[:rows].float(), y_lo, y_hi, f"{what}: fast_project_in", rbf(v), tally=tally)
+        check_ssq(sf[:rows], xf[:rows], what, nan_past=True)
         assert (xf[rows:].float() == SENTINEL).all() and torch.isnan(sf[rows:]).all(), f"{what}: rows past rows written"
-    _check_share(tally, f"{name} fast input")
+    check_tally(tally, f"{name} fast input")
 
 
 def test_fast_input_covers_every_variant():
@@ -342,7 +308,7 @@ def test_fast_embed(name):
                 eng.test_frame_stage("fast_embed", rows, tile=_tile(eng, rows), p=p, row_slot=rs)
                 want = fe[tok[slots, p].long()]
                 assert _same(xf[:rows], want), f"{what}: x_fast is not fast_embeddings[cur_tok[slot][p]]"
-                _check_ssq(sf[:rows], xf[:rows], what)
+                check_ssq(sf[:rows], xf[:rows], what, nan_past=True)
                 assert (xf[rows:].float() == SENTINEL).all() and torch.isnan(sf[rows:]).all(), \
                     f"{what}: rows past rows written"
                 assert torch.equal(ct, tok), f"{what}: cur_tok written"
@@ -370,14 +336,14 @@ def test_fast_head(name):
                 lg.fill_(float("nan"))
                 eng.test_frame_stage("fast_head", rows, tile=_tile(eng, rows), p=p, row_slot=rs, sp=_sp(eng))
                 got = lg[p - 1, slots]
-                _inside(got, lo, hi, mid, what, tally)
+                check_bracket(got, lo, hi, what, mid, tally=tally)
                 written = torch.zeros(C, B, dtype=torch.bool, device="cuda")
                 written[p - 1, slots] = True
                 assert torch.isnan(lg[~written]).all(), f"{what}: logits written outside [p - 1][slots]"
                 want = tok.clone()
                 want[slots, p + 1] = got.argmax(1).int()
                 assert torch.equal(ct, want), f"{what}: cur_tok is not the old one with [slot][p + 1] = argmax"
-    _check_share(tally, f"{name} fast head")
+    check_tally(tally, f"{name} fast head")
 
 
 # ---------------------------------------------------------------------------------------------------------------------

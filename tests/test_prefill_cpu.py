@@ -1,5 +1,5 @@
-"""The float64 references and fp32 emulations of tests/prefill_ref.py on the CPU: shapes, orderings and the bounds'
-logic, without a GPU (tests/test_prefill_gpu.py runs them against the kernels)."""
+"""The prefill float64 references and fp32 emulations of tests/kernel_ref.py on the CPU: shapes, orderings and the
+bounds' logic, without a GPU (tests/test_prefill_gpu.py runs them against the kernels)."""
 from __future__ import annotations
 
 import math
@@ -7,8 +7,8 @@ import math
 import torch
 
 from oracle import lm_oracle as O
-from tests import prefill_ref as R
-from tests.prefill_ref import rbf
+from tests import kernel_ref as R
+from tests.kernel_ref import rbf
 
 
 def test_gate_row_matches_interleave_w13():

@@ -3,7 +3,7 @@ float64 references built from the same bf16 operands. Each stage reads inputs th
 so an error in one stage cannot reach the next: embed + attention_norm_0, the qkv GEMM + qkv_prep_row_kernel (bias,
 per-head qk-norm, RoPE, K/V append through the page table), attn_tile_kernel over the page table, wo + residual + norm,
 w1|w3 + SwiGLU, w2 + residual + the next layer's norm. The hand-off to decode (rows_kernel, frame_end_kernel) is checked
-after a whole fsb_lm_prefill. The helpers live in tests/prefill_ref.py (rehearsed on the CPU by test_prefill_cpu.py).
+after a whole fsb_lm_prefill. The helpers live in tests/kernel_ref.py (rehearsed on the CPU by test_prefill_cpu.py).
 
 Rows. One pass holds sequences of 1, 63, 64, 65, 200 and 333 rows in scrambled slots, starting at positions 0, 100
 (mid-page), 128 (page edge) and, with S2-Pro's 32 768 positions, 16 400; several sequences share each 64-row tile.
@@ -68,8 +68,9 @@ import random
 import pytest
 import torch
 
-from tests import prefill_ref as R
-from tests.prefill_ref import PAGE, rbf
+from tests import kernel_ref as R
+from tests.kernel_ref import PAGE, rbf
+from tests.lm_util import _bits, _lib, _randn, _sms, attn_configs
 
 pytestmark = pytest.mark.gpu
 
@@ -85,27 +86,10 @@ TEETH = {"drop": 0.9, "double": 0.9, "leak": 0.6, "rope+1": 0.9, "next-head": 0.
 LENS = (1, 63, 64, 65, 200, 333)
 
 
-def _lib():
-    from fish_speech_b200 import _lib
-
-    return _lib
-
-
-def _sms() -> int:
-    L = _lib()
-    n = ctypes.c_int()
-    L.check(L.lib().fsb_device_info(ctypes.byref(n), None, None))
-    return n.value
-
-
 def wide_from(n_out: int) -> int:
     """Fewest rows that launch_rows_of gives the 256-row plan (lm_engine.cu): >= 512 rows and two waves of tiles."""
     tiles = math.ceil(n_out / 128)
     return max(512, 256 * (math.ceil(2 * _sms() / tiles) - 1) + 1)
-
-
-def _bits(t):
-    return t.view(torch.int16) if t.element_size() == 2 else t.view(torch.int32)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -113,10 +97,9 @@ def _bits(t):
 # ---------------------------------------------------------------------------------------------------------------------
 def _configs():
     from oracle import lm_oracle as O
-    from tests.test_decode_attn_gpu import _configs as decode_configs
 
     out = {}
-    for name, (cfg, slots) in decode_configs().items():
+    for name, (cfg, slots) in attn_configs().items():
         if name == "tiny-b":
             cfg = dataclasses.replace(cfg, attention_o_bias=True)
         out[name] = (cfg, slots)
@@ -244,11 +227,6 @@ def _main_pass(eng, g, seed, with_unmapped=True):
     if with_unmapped:
         seqs.insert(3, (slots[-1], 120, 10, 1))
     return Pass(eng, g, seqs, seed)
-
-
-def _randn(shape, seed, scale=1.0):
-    gen = torch.Generator(device="cuda").manual_seed(seed)
-    return (torch.randn(shape, generator=gen, device="cuda") * scale).bfloat16()
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -26,33 +26,13 @@ import math
 import pytest
 import torch
 
+from tests.kernel_ref import (C_AMB, acc_bound, bracket_bf16, check_bracket, check_ssq, fp64_gemm, norm_operand,
+                              normed_gemm, rbf, swiglu_from, tile_ssq)
+from tests.lm_util import SHAPES, STAGES, _ctas, _gen, _lib, _randn, _sms, build_model, layer_configs
+
 pytestmark = pytest.mark.gpu
 
-C_AMB = 2.0 ** -19
 ROWS = (1, 5, 31, 32)
-STAGES = (2, 3, 4, 8)  # 8 does not fit two CTAs per SM: step_plan_init shrinks it
-
-
-def _sms() -> int:
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _ctas():
-    return (1, 2, 3, 7, 132, 2 * _sms(), 10 ** 6)  # 10^6: clamped to what one wave holds
-
-
-def _lib():
-    from fish_speech_b200 import _lib
-
-    return _lib
-
-
-def _gen(seed: int) -> torch.Generator:
-    return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def _randn(shape, seed, scale=1.0) -> torch.Tensor:
-    return (torch.randn(shape, generator=_gen(seed), device="cuda") * scale).bfloat16()
 
 
 def step_gemm(w, x, rows, num_ctas, stages, norm_w=None, ssq=None, eps=1e-6):
@@ -69,50 +49,14 @@ def step_gemm(w, x, rows, num_ctas, stages, norm_w=None, ssq=None, eps=1e-6):
     return out[:rows], dict(ctas=info[0], stages=info[1], parts=info[2], units=info[3], items=info[4])
 
 
-def fp64_gemm(w, x):
-    """(W X^T)^T and (|W| |X|^T)^T in float64: [rows, n_out] each."""
-    w64, x64 = w.double(), x.double()
-    return x64 @ w64.T, x64.abs() @ w64.abs().T
-
-
-def acc_bound(absprod, K, parts):
-    return (K / 16 + parts + 1) * 2.0 ** -23 * absprod  # (ACC) in the module docstring
-
-
-def rbf(t: torch.Tensor) -> torch.Tensor:
-    """Round to bf16 the way the kernels do: to fp32 first (a no-op for fp32 input), then to bf16."""
-    return t.float().bfloat16().float()
-
-
-def bf16_key(t: torch.Tensor) -> torch.Tensor:
-    """Integers ordered like the bf16 values of t, one apart for neighbouring values (ulp distance)."""
-    b = t.bfloat16().view(torch.int16).int()
-    return torch.where(b < 0, -(b & 0x7FFF), b)
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # 3a: one GEMM against float64 over the engine's shapes and the whole range of schedules
 # ---------------------------------------------------------------------------------------------------------------------
-SHAPES = [
-    pytest.param(6144, 2560, id="s2pro-qkv"),
-    pytest.param(2560, 4096, id="s2pro-wo"),
-    pytest.param(19456, 2560, id="s2pro-w13"),
-    pytest.param(2560, 9728, id="s2pro-w2"),
-    pytest.param(4097, 2560, id="s2pro-head"),
-    pytest.param(4096, 2560, id="s2pro-fast-out"),
-    pytest.param(384, 256, id="tiny-qkv"),
-    pytest.param(96, 256, id="tiny-fast-out"),
-    pytest.param(97, 256, id="tiny-head"),
-    pytest.param(1, 1000, id="one-row-K1000"),  # partial last k-block (40 of 64) and a one-feature tile
-    pytest.param(200, 528, id="K528"),  # w2 with an intermediate size that is not a multiple of 64
-]
-
-
 @pytest.mark.parametrize("n_out,K", SHAPES)
 def test_step_gemm_matches_fp64(n_out, K):
     w = _randn((n_out, K), seed=n_out * 7 + K)
     x = _randn((32, K), seed=n_out * 7 + K + 1)
-    ref, absprod = fp64_gemm(w, x)
+    ref, absprod = fp64_gemm(x, w)
     tiles, kblocks = math.ceil(n_out / 128), math.ceil(K / 64)
     infos = []
     full = None
@@ -154,7 +98,7 @@ def test_step_gemm_error_at_engine_schedules():
     for n_out, K in ((6144, 2560), (2560, 4096), (19456, 2560), (2560, 9728), (384, 256)):
         w = _randn((n_out, K), seed=K, scale=0.02)
         x = _randn((32, K), seed=K + 1)
-        ref, absprod = fp64_gemm(w, x)
+        ref, absprod = fp64_gemm(x, w)
         out, info = step_gemm(w, x, 32, 2 * _sms(), 4)
         ratio = float(((out.double() - ref).abs() / absprod).max())
         assert ratio <= C_AMB / 4, f"{n_out}x{K} {info}: max error 2^{math.log2(ratio):.2f} * sum|w x|"
@@ -175,34 +119,6 @@ def test_step_gemm_rejects_bad_arguments():
 # ---------------------------------------------------------------------------------------------------------------------
 # 3b: normalise-on-load
 # ---------------------------------------------------------------------------------------------------------------------
-def tile_ssq(x: torch.Tensor) -> torch.Tensor:
-    """Per-128-feature-tile sums of squares [rows, ceil(D/128)] in fp32 (what the residual-add finalize leaves)."""
-    rows, D = x.shape
-    nt = math.ceil(D / 128)
-    xp = torch.zeros(rows, nt * 128, dtype=torch.float64, device=x.device)
-    xp[:, :D] = x.double() ** 2
-    return xp.view(rows, nt, 128).sum(-1).float()
-
-
-def norm_operand(x, ssq, norm_w, eps, K):
-    """X' = rbf(rbf(x * r) * w) in the kernel's order (tile sums added in tile order in fp32, / K, + eps, rsqrt) for
-    r and for r * (1 -+ 2^-21): rsqrtf may be off by 2 ulp (2^-22 relative). Returns (mid, lo, hi), fp32 [rows, K];
-    lo / hi bracket every X' a 2-ulp rsqrtf can give."""
-    nt = math.ceil(K / 128)
-    tot = torch.zeros(ssq.shape[0], dtype=torch.float32, device=ssq.device)
-    for t in range(nt):
-        tot = tot + ssq[:, t]
-    v = tot / torch.tensor(float(K), dtype=torch.float32) + torch.tensor(eps, dtype=torch.float32)
-    r = (1.0 / torch.sqrt(v.double())).float()
-
-    def apply(rr):
-        return rbf(rbf(x.float() * rr[:, None]) * norm_w.float()[None, :])
-
-    mid = apply(r)
-    a, b = apply((r.double() * (1 - 2.0 ** -21)).float()), apply((r.double() * (1 + 2.0 ** -21)).float())
-    return mid, torch.minimum(a, b), torch.maximum(a, b)
-
-
 @pytest.mark.parametrize("K", [2560, 1000])  # 20 tiles; 8 tiles, the last one partial, and a partial last k-block
 def test_step_gemm_normalise_on_load(K):
     eps = 1e-6
@@ -211,7 +127,7 @@ def test_step_gemm_normalise_on_load(K):
     scale = torch.tensor([2.0 ** (j % 7 - 3) for j in range(32)], device="cuda")[:, None]
     x = (_randn((32, K), seed=K) * scale).bfloat16()
     norm_w = (1 + 0.1 * torch.randn(K, generator=_gen(K + 1), device="cuda")).bfloat16()
-    ssq_live = tile_ssq(x)
+    ssq_live = tile_ssq(x).float()
     schedules = [(1, 2), (7, 3), (2 * _sms(), 4), (10 ** 6, 8)]
     # identity weights: out = X' itself, so every element of the normalised operand is checked, not only their sums
     eye = torch.eye(K, device="cuda").bfloat16()
@@ -231,9 +147,9 @@ def test_step_gemm_normalise_on_load(K):
                               f"{(~inside).nonzero()[0].tolist()} ({int((~inside).sum())} elements)")
 
         out, info = step_gemm(w, x, rows, ctas, stages, norm_w, ssq, eps)
-        ref, absprod = fp64_gemm(w, mid)
+        ref, absprod = fp64_gemm(mid, w)
         slack = (hi - lo).double() @ w.double().abs().T  # zero wherever the rounding of X' is unambiguous
-        bound = acc_bound(fp64_gemm(w, torch.maximum(lo.abs(), hi.abs()))[1], K, info["parts"]) + slack
+        bound = acc_bound(fp64_gemm(torch.maximum(lo.abs(), hi.abs()), w)[1], K, info["parts"]) + slack
         bad = ~((out.double() - ref).abs() <= bound)
         assert not bad.any(), f"ctas={ctas} stages={stages} rows={rows} {info}: {int(bad.sum())} elements off"
 
@@ -250,7 +166,7 @@ def test_step_gemm_bits_reproducible_and_row_independent(n_out, K, norm):
     nt = math.ceil(K / 128)
     ssq = torch.full((32, 32), float("nan"), device="cuda")
     if norm:
-        ssq[:, :nt] = tile_ssq(x)
+        ssq[:, :nt] = tile_ssq(x).float()
     sched = (2 * _sms(), 4)
     base, _ = step_gemm(w, x, 32, *sched, nw, ssq if norm else None, eps)
     again, _ = step_gemm(w, x, 32, *sched, nw, ssq if norm else None, eps)
@@ -274,31 +190,17 @@ def test_step_gemm_bits_reproducible_and_row_independent(n_out, K, norm):
 # ---------------------------------------------------------------------------------------------------------------------
 # 3d: one decode layer through the engine's own plans
 # ---------------------------------------------------------------------------------------------------------------------
-def _configs():
-    from oracle import lm_oracle as O
-
-    return {
-        # wo bias in both stacks; intermediate sizes that are not multiples of 64 (w1|w3 padded, w2 with K % 64 != 0)
-        "tiny": O.tiny_config(attention_o_bias=True, fast_attention_o_bias=True, intermediate_size=528,
-                              fast_intermediate_size=400),
-        # S2-Pro layer shapes with two layers per stack and a reduced vocabulary (test_lm_gpu.py builds it so too)
-        "s2pro": O.LMConfig(n_layer=2, n_fast_layer=2, vocab_size=8192, max_seq_len=256, semantic_begin_id=4000,
-                            semantic_end_id=8095, im_end_id=3999),
-    }
-
-
 _MODELS: dict = {}
 
 
 def _model(name):
     if name not in _MODELS:
         from oracle import lm_oracle as O
-        from tests.lm_util import build_model
 
         for _, _, m in _MODELS.values():  # one at a time on the device
             m.engine.close()
         _MODELS.clear()
-        cfg = _configs()[name]
+        cfg = layer_configs()[name]
         w = O.make_weights(cfg, seed=97)
         _MODELS[name] = (cfg, w, build_model(cfg, w, max_batch=32, debug=False, max_rows=128))
     return _MODELS[name]
@@ -312,42 +214,13 @@ def _free_models():
     _MODELS.clear()
 
 
-def _bracket_bf16(v, E):
-    """The bf16 values between which the kernel's rbf(fp32 accumulation) of the float64 value v lies when the
-    accumulation is off by at most E (rounding to fp32, then to bf16, is monotone)."""
-    return rbf(v - E), rbf(v + E)
-
-
-def _check_rounded(got, lo, hi, mid, what):
-    """got inside [lo, hi] everywhere (bit-identical to mid where lo == hi), and different from mid in < 1 % of it."""
-    inside = (got >= lo) & (got <= hi)
-    assert inside.all(), (f"{what}: off at {(~inside).nonzero()[0].tolist()} ({int((~inside).sum())} of "
-                          f"{got.numel()}): got {float(got[~inside][0])} want {float(mid[~inside][0])}")
-    diff = got != mid
-    assert diff.double().mean() < 0.01, f"{what}: {int(diff.sum())} of {got.numel()} elements differ from float64"
-
-
 def _check_resid(x_new, x_old, y, b, absprod, what):
     """x_new = rbf(x_old + rbf(y + b)) with y the float64 GEMM; the rounding of y + b may go either way within
     C_AMB * absprod of a bf16 rounding boundary."""
     v = y + (b.double()[None, :] if b is not None else 0.0)
-    y_lo, y_hi = _bracket_bf16(v, C_AMB * absprod)
+    y_lo, y_hi = bracket_bf16(v, C_AMB * absprod)
     x_old = x_old.float()
-    _check_rounded(x_new.float(), rbf(x_old + y_lo), rbf(x_old + y_hi), rbf(x_old + rbf(v)), f"{what}: x")
-
-
-def _check_ssq(ssq, x, what):
-    want = tile_ssq(x).double()
-    got = ssq[:, : want.shape[1]].double()
-    rel = ((got - want).abs() / want).max()
-    assert rel <= 2.0 ** -16, f"{what}: sums of squares off by {float(rel):.3g} (relative)"
-
-
-def _silu(g, exp_scale=1.0):
-    """rbf(g / (1 + expf(-g))) with the add and the division in fp32 as the kernel does; exp_scale = 1 -+ 2^-22
-    brackets an expf that is off by up to 2 fp32 ulp."""
-    ef = (torch.exp(-g.double()) * exp_scale).float()
-    return rbf(g / (1.0 + ef))
+    check_bracket(x_new.float(), rbf(x_old + y_lo), rbf(x_old + y_hi), f"{what}: x", rbf(x_old + rbf(v)))
 
 
 def _check_swiglu(h, x, ssq, w, prefix, eps, what):
@@ -355,22 +228,11 @@ def _check_swiglu(h, x, ssq, w, prefix, eps, what):
     matrix), X' = ffn_norm(x) normalised on load with the sums of squares the residual-add finalize left. Ambiguity
     sources: the accumulation (C_AMB), the rounding of X' (rsqrtf) and expf."""
     nw = w[f"{prefix}.ffn_norm.weight"].cuda()
-    mid, lo, hi = norm_operand(x, ssq, nw, eps, x.shape[1])
-    xmax = torch.maximum(lo.abs(), hi.abs())
-    br, ref = [], []
-    for name in ("w1", "w3"):
-        W = w[f"{prefix}.feed_forward.{name}.weight"].cuda()
-        v, _ = fp64_gemm(W, mid)
-        E = C_AMB * fp64_gemm(W, xmax)[1] + (hi - lo).double() @ W.double().abs().T
-        br.append(_bracket_bf16(v, E))
-        ref.append(rbf(v))
-    (g_lo, g_hi), (u_lo, u_hi) = br
+    g, u = (normed_gemm(x, ssq, nw, eps, w[f"{prefix}.feed_forward.{name}.weight"].cuda()) for name in ("w1", "w3"))
     # h is monotone in u, and in g wherever a bracket of g holds more than two bf16 values (|g| small, silu rising):
     # the extremes over the corners bracket it
-    corners = torch.stack([rbf(_silu(g, f) * u) for g in (g_lo, g_hi) for f in (1 - 2.0 ** -22, 1 + 2.0 ** -22)
-                           for u in (u_lo, u_hi)])
-    _check_rounded(h.float(), corners.min(0).values, corners.max(0).values, rbf(_silu(ref[0]) * ref[1]),
-                   f"{what}: h")
+    lo, hi, mid = swiglu_from(*bracket_bf16(*g), rbf(g[0]), *bracket_bf16(*u), rbf(u[0]))
+    check_bracket(h.float(), lo, hi, f"{what}: h", mid)
 
 
 LAYER_CASES = [pytest.param(name, fast, last, id=f"{name}-{'fast' if fast else 'slow'}-{'last' if last else 'first'}")
@@ -427,9 +289,9 @@ def test_decode_layer_gemms(name, fast, last):
 
         # upto = 1: x1 = rbf(x0 + rbf(wo attn + bo)) and its sums of squares
         x1, s1, h1 = run(1)
-        y, absprod = fp64_gemm(wo, attn[:rows])
+        y, absprod = fp64_gemm(attn[:rows], wo)
         _check_resid(x1[:rows], x0[:rows], y, bo, absprod, f"{what} wo")
-        _check_ssq(s1[:rows], x1[:rows], f"{what} wo")
+        check_ssq(s1[:rows], x1[:rows], f"{what} wo")
         dead_regions_untouched(x1, s1, h1, False)
 
         # upto = 2: the same x, then h = SwiGLU of the w1|w3 GEMM normalised on load with those sums of squares
@@ -443,7 +305,7 @@ def test_decode_layer_gemms(name, fast, last):
         # upto = 3: x3 = rbf(x1 + rbf(w2 h)) (w2 has no bias) and its sums of squares, finished by the next consumer
         x3, s3, h3 = run(3)
         assert torch.equal(h3.view(torch.int16), h2.view(torch.int16)), f"{what}: h differs between runs"
-        y, absprod = fp64_gemm(w2, hl)
+        y, absprod = fp64_gemm(hl, w2)
         _check_resid(x3[:rows], x1[:rows], y, None, absprod, f"{what} w2")
-        _check_ssq(s3[:rows], x3[:rows], f"{what} w2")
+        check_ssq(s3[:rows], x3[:rows], f"{what} w2")
         dead_regions_untouched(x3, s3, h3, True)

@@ -70,6 +70,37 @@ def kv_pages_for(n_positions: int) -> int:
     return -(-int(n_positions) // KV_PAGE)
 
 
+PREFIX_BLOCK = 16  # token rows per link of a cached prefix's hash chain (= LmEngine.MIN_REUSE)
+
+
+def _chain_keys(rows: np.ndarray) -> list:
+    """Chained hashes of the whole PREFIX_BLOCK-row blocks of token rows [n, C+1]: key j names rows [0, 16 (j + 1))."""
+    keys, h = [], 0
+    for a in range(0, rows.shape[0] - PREFIX_BLOCK + 1, PREFIX_BLOCK):
+        h = hash((h, rows[a:a + PREFIX_BLOCK].tobytes()))
+        keys.append(h)
+    return keys
+
+
+def _common_rows(a: np.ndarray, b: np.ndarray) -> int:
+    """Length of the common prefix of two token-row arrays [n, C+1]."""
+    n = min(len(a), len(b))
+    diff = np.flatnonzero((a[:n] != b[:n]).any(axis=1))
+    return int(diff[0]) if len(diff) else n
+
+
+@dataclass(eq=False)
+class CachedRow:
+    """A prompt prefix kept in the page pool after its request left its slot (KvPagePool.insert): a page-table row
+    outside every slot, like a parked request's, that holds references to the pages of positions [0, n)."""
+
+    row: np.ndarray  # pages of positions [0, n); -1 past them
+    rows: np.ndarray  # token rows [n, C+1] (int32) whose K/V those positions hold, as prefill wrote it
+    n: int
+    keys: list  # _chain_keys(rows)
+    stamp: int = 0  # last insert or reuse (KvPagePool.tick)
+
+
 class KvPagePool:
     """Host side of the paged slow KV cache: which pool page holds each 64-position block of each slot.
 
@@ -81,10 +112,16 @@ class KvPagePool:
     also be detached: taken out of the table with its page references, for a request that is parked between two frames
     and continues later in whichever slot is idle then.
 
+    With `prefix_cache`, a prompt prefix also outlives its slot: `insert` keeps the pages of a retiring slot's prompt
+    as a cached row (CachedRow), `lookup` finds the longest cached prefix of a prompt, and a reservation short of pages
+    drops cached rows least recently used first, after the retired slots. Cached rows hold only pages nobody else
+    needs: `available()` counts the pages only they map as available.
+
     Device effects are callbacks, so that the rules can run without a GPU: `copy_page(src, dst, n)` copies positions
     [0, n) of a page, stream-ordered before the writes that follow."""
 
-    def __init__(self, slots: int, pages_per_slot: int, n_pages: int, copy_page=None, on_reclaim=None):
+    def __init__(self, slots: int, pages_per_slot: int, n_pages: int, copy_page=None, on_reclaim=None,
+                 prefix_cache: bool = False):
         if n_pages < 1:
             raise ValueError(f"kv_pages must be >= 1, got {n_pages}")
         self.slots, self.pages_per_slot, self.n_pages = slots, pages_per_slot, n_pages
@@ -97,13 +134,20 @@ class KvPagePool:
         self.on_reclaim = on_reclaim or (lambda slot: None)
         self.dirty = True
         self.peak = 0
+        self.prefix_cache = bool(prefix_cache)
+        self.cached: dict[CachedRow, None] = {}  # least recently used first
+        self._index: dict[int, set] = {}  # chain key -> cached rows whose keys include it
+        self.held: set = set()  # cached rows that are donors of the admission being reserved: dropped last
+        self.tick = 0
+        self.hits = 0  # admissions that mapped a cached prefix
+        self.evictions = 0  # cached rows dropped because a reservation was short of pages
 
     # ---- queries ------------------------------------------------------------------------------------------------
     def in_use(self) -> int:
         return self.n_pages - len(self.free)
 
     def available(self) -> int:
-        """Pages a reservation can get: free ones plus those that only retired slots map."""
+        """Pages a reservation can get: free ones plus those that only retired slots and cached rows map."""
         live = [s for s in range(self.slots) if s not in self.retired]
         pages = np.concatenate([self.table[live].ravel(), *self.detached])
         return self.n_pages - len(np.unique(pages[pages >= 0]))
@@ -184,10 +228,12 @@ class KvPagePool:
                 self.ref[p] -= 1
                 self.dirty = True
 
-    def share(self, dst: int, src: int, n_pages: int):
-        """Map the first `n_pages` pages of `src` into `dst` as well (a shared prompt prefix)."""
+    def share(self, dst: int, src, n_pages: int):
+        """Map the first `n_pages` pages of `src` into `dst` as well (a shared prompt prefix). `src`: a slot, or a
+        row outside the table (CachedRow.row)."""
+        src_row = src if isinstance(src, np.ndarray) else self.table[src]
         for j in range(n_pages):
-            p = int(self.table[src, j])
+            p = int(src_row[j])
             if p < 0 or p == self.table[dst, j]:
                 continue
             old = int(self.table[dst, j])
@@ -224,14 +270,19 @@ class KvPagePool:
             need = len(cow) + len(missing)
             if len(self.free) >= need:
                 break
-            if not self.retired:
+            if self.retired:
+                victim = next(iter(self.retired))
+                del self.retired[victim]
+                self.release(victim)
+                self.on_reclaim(victim)
+            elif self.cached:
+                # least recently used first; a donor of the admission being reserved only when nothing else is left
+                self.drop_cached(next((e for e in self.cached if e not in self.held), next(iter(self.cached))))
+                self.evictions += 1
+            else:
                 raise RuntimeError(
                     f"KV page pool exhausted: slot {slot} needs {need} more pages of {KV_PAGE} positions for {end} "
                     f"positions, {len(self.free)} of the pool's {self.n_pages} pages (kv_pages) are free")
-            victim = next(iter(self.retired))
-            del self.retired[victim]
-            self.release(victim)
-            self.on_reclaim(victim)
         for j in cow:
             old, new = int(row[j]), self._take()
             keep = min(max(0, start - j * KV_PAGE), KV_PAGE)
@@ -242,6 +293,90 @@ class KvPagePool:
         for j in missing:
             row[j] = self._take()
         self.peak = max(self.peak, self.in_use())
+
+    # ---- prefix cache: prompt prefixes kept after their slot moved on ---------------------------------------------
+    def touch(self, entry: CachedRow):
+        """`entry` was just inserted or reused: it becomes the most recently used."""
+        self.tick += 1
+        entry.stamp = self.tick
+        self.cached.pop(entry, None)
+        self.cached[entry] = None
+
+    def insert(self, slot: int, tokens: torch.Tensor):
+        """The retiring `slot` holds the K/V its prefill wrote for `tokens` [C+1, n] at positions [0, n): keep the
+        pages of those positions as a cached row, then release the slot's row, so that pages only its decode frames
+        wrote go back to the free list. A cached row that already covers the prefix is only touched; cached rows that
+        are a prefix of it are dropped. A prefix shorter than one hash block is not kept."""
+        rows = np.ascontiguousarray(tokens.numpy().T, dtype=np.int32)
+        n = rows.shape[0]
+        keys = _chain_keys(rows)
+        if keys and (self.table[slot, :kv_pages_for(n)] >= 0).all():
+            cover = next((e for e in self._index.get(keys[-1], ()) if e.n >= n and _common_rows(rows, e.rows) >= n),
+                         None)
+            if cover is not None:
+                self.touch(cover)
+            else:
+                for j, k in enumerate(keys):
+                    for e in list(self._index.get(k, ())):
+                        if len(e.keys) == j + 1 and e.n <= n and _common_rows(rows, e.rows) >= e.n:
+                            self.drop_cached(e)
+                row = np.full(self.pages_per_slot, -1, dtype=np.int32)
+                m = kv_pages_for(n)
+                row[:m] = self.table[slot, :m]
+                self.ref[row[:m]] += 1
+                entry = CachedRow(row, rows, n, keys)
+                for k in keys:
+                    self._index.setdefault(k, set()).add(entry)
+                self.touch(entry)
+        self.release(slot)
+
+    def lookup(self, rows: np.ndarray) -> tuple[int, Optional[CachedRow]]:
+        """(rows, cached row) of the longest prefix of token rows [T, C+1] that a cached row holds; (0, None) below
+        one hash block. The chain keys narrow the search to the cached rows that share the prompt's deepest matching
+        block; an exact compare confirms the one chosen."""
+        cands, depth = (), 0
+        for j, k in enumerate(_chain_keys(rows)):
+            c = self._index.get(k)
+            if not c:
+                break
+            cands, depth = c, j + 1
+        lo = depth * PREFIX_BLOCK
+        best, hit = 0, None
+        for e in cands:  # all of them share rows [0, lo) with the prompt; each diverges within the next block
+            n = lo + _common_rows(rows[lo:lo + PREFIX_BLOCK], e.rows[lo:lo + PREFIX_BLOCK])
+            if n > best:
+                best, hit = n, e
+        if hit is not None and _common_rows(rows[:lo], hit.rows[:lo]) < lo:  # a hash collision: compare everything
+            best, hit = 0, None
+            for e in self.cached:
+                n = _common_rows(rows, e.rows)
+                if n > best:
+                    best, hit = n, e
+        return best, hit
+
+    def drop_cached(self, entry: CachedRow):
+        """Forget a cached row: pages no slot, parked row or other cached row maps return to the free list."""
+        del self.cached[entry]
+        self.held.discard(entry)
+        for k in entry.keys:
+            s = self._index[k]
+            s.discard(entry)
+            if not s:
+                del self._index[k]
+        pages = entry.row[entry.row >= 0]
+        self.ref[pages] -= 1
+        self.free.extend(pages[self.ref[pages] == 0].tolist())
+
+    def drop_cache(self):
+        for e in list(self.cached):
+            self.drop_cached(e)
+
+    def cached_pages(self) -> int:
+        """Pages at least one cached row maps."""
+        if not self.cached:
+            return 0
+        pages = np.concatenate([e.row for e in self.cached])
+        return len(np.unique(pages[pages >= 0]))
 
 
 @dataclass(eq=False)
@@ -261,11 +396,14 @@ class LmEngine:
 
     def __init__(self, config, state_dict: dict, device, im_end_id: int, max_batch: int = 1,
                  kv_len: Optional[int] = None, max_rows: int = 2048, max_frames: Optional[int] = None,
-                 debug: bool = False, kv_pages: Optional[int] = None, attn_split: int = 0):
+                 debug: bool = False, kv_pages: Optional[int] = None, attn_split: int = 0, prefix_cache: bool = False):
         """`kv_len`: KV positions one sequence can hold. `kv_pages`: size of the slow KV cache's page pool (pages of
         64 positions); None = room for every slot at full capacity, so that no reservation can fail. `attn_split`:
         0 = off; else a multiple of 64: a decode row with a longer context has its attention split into spans of that
-        many positions over several CTAs (include/fishb200.h fsb_lm_config.attn_split)."""
+        many positions over several CTAs (include/fishb200.h fsb_lm_config.attn_split). `prefix_cache`: the prompt
+        pages of a request that `prefill_reusing` admitted stay in the pool after its slot moves on, as a prefix later
+        requests reuse until the pool needs the pages (KvPagePool.insert); off: a prefix lives as long as its slot
+        holds it."""
         if not torch.cuda.is_available():
             raise _lib.FsbError("fish_speech_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.lib = _lib.lib()
@@ -357,7 +495,7 @@ class LmEngine:
         self.rows_reused = 0
         self.rows_prefilled = 0
         self.kv_pool = KvPagePool(max_batch, pages_per_slot, K.kv_pages, copy_page=self._copy_page,
-                                  on_reclaim=self._forget_slot)
+                                  on_reclaim=self._forget_slot, prefix_cache=prefix_cache)
         self._wfrom: dict = {}  # slot -> lowest position the next decode frames write (copy-on-write bound)
         self._covered: dict = {}  # slot -> pages [0, n) its last reservation mapped (decode skips what is covered)
 
@@ -581,9 +719,35 @@ class LmEngine:
         self._reserve([(int(s), int(e), self._covered.get(int(s), 0) * KV_PAGE) for s, e in ends.items()
                        if kv_pages_for(e) > self._covered.get(int(s), 0)])
 
-    def retire_slot(self, slot: int):
-        """The slot's request is done: its pages stay mapped as a reusable prefix until the pool needs them."""
-        self.kv_pool.retire(int(slot))
+    def retire_slot(self, slot: int, cache: bool = True):
+        """The slot's request is done: its pages stay mapped as a reusable prefix until the pool needs them. With the
+        prefix cache, a slot that holds a prompt record (prefill_reusing) moves the pages of that prompt into the cache
+        instead and gives the rest back; `cache=False` (a request whose tokens are void) keeps it out of the cache."""
+        slot = int(slot)
+        tokens = self._slot_tokens.get(slot)
+        if cache and tokens is not None and self.kv_pool.prefix_cache:
+            self.kv_pool.insert(slot, tokens)
+            self._forget_slot(slot)
+        self.kv_pool.retire(slot)
+
+    @property
+    def prefix_cache(self) -> bool:
+        return self.kv_pool.prefix_cache
+
+    @property
+    def prefix_hits(self) -> int:
+        """Admissions that mapped a prefix from the prefix cache."""
+        return self.kv_pool.hits
+
+    @property
+    def prefix_evictions(self) -> int:
+        """Cached prefixes dropped because a reservation needed their pages."""
+        return self.kv_pool.evictions
+
+    @property
+    def pages_cached(self) -> int:
+        """Pool pages the prefix cache maps now."""
+        return self.kv_pool.cached_pages()
 
     def park_slot(self, slot: int, ctx_len: int = 0) -> ParkedSlot:
         """Take the request running in `slot` out of it, between two frames: its per-slot decode state goes into a
@@ -615,16 +779,18 @@ class LmEngine:
         self.kv_pool.drop(parked.row)
 
     def release_kv(self):
-        """Forget every slot's K/V: all pages return to the pool."""
+        """Forget every slot's K/V and the prefix cache: all pages return to the pool."""
         self._slot_tokens.clear()
         self._covered.clear()
+        self.kv_pool.drop_cache()
         for s in range(self.max_batch):
             self.kv_pool.release(s)
             self.kv_pool.retire(s)
         self._reserve([])
 
-    def _donor(self, prompt: torch.Tensor, slot: int, busy) -> tuple[int, int]:
-        """(rows, slot) of the longest prefix of `prompt` whose K/V a slot holds: its own, or one not in `busy`."""
+    def _donor(self, prompt: torch.Tensor, slot: int, busy) -> tuple[int, object]:
+        """(rows, donor) of the longest prefix of `prompt` whose K/V a slot holds -- its own, or one not in `busy` --
+        or the prefix cache does: the donor is a slot or a CachedRow."""
         best, donor = 0, slot
         for d, toks in self._slot_tokens.items():
             if d != slot and d in busy:
@@ -632,16 +798,22 @@ class LmEngine:
             n = self._common_prefix(prompt, toks)
             if n > best:
                 best, donor = n, d
+        if self.kv_pool.cached:
+            n, entry = self.kv_pool.lookup(np.ascontiguousarray(prompt.numpy().T, dtype=np.int32))
+            if n > best:
+                best, donor = n, entry
         best = min(best, prompt.shape[1] - 1)  # at least the last row is computed: its logits are sampled
         return (best, donor) if best >= self.MIN_REUSE else (0, slot)
 
     def kv_pages_needed(self, prompt: torch.Tensor, n_positions: int, slot: int, busy=(), reuse: bool = False) -> int:
         """Pages a request in `slot` adds to those live slots map: all of [0, n_positions), less the whole pages of a
-        prefix it shares with a live slot (prefill_reusing). `prompt`: the request's token rows on the host."""
+        prefix it shares with a live slot (prefill_reusing). A prefix from a retired slot or the prefix cache is not
+        subtracted: its pages count as available, and sharing them makes them live. `prompt`: the request's token rows
+        on the host."""
         need = kv_pages_for(min(int(n_positions), self.kv_len))
         if reuse:
             best, donor = self._donor(prompt, int(slot), set(busy) | {int(slot)})
-            if donor != slot and donor not in self.kv_pool.retired:
+            if isinstance(donor, int) and donor != slot and donor not in self.kv_pool.retired:
                 need -= best // KV_PAGE
         return need
 
@@ -650,7 +822,7 @@ class LmEngine:
 
     def reset(self):
         for s in range(self.max_batch):
-            self.kv_pool.retire(s)  # their K/V stays mapped for prefix reuse until the pool needs the pages
+            self.retire_slot(s)  # their K/V stays mapped (or cached) for prefix reuse until the pool needs the pages
         self._ctx_bound = 0
         with torch.cuda.device(self.device):
             _lib.check(self.lib.fsb_lm_reset(self.h, _stream()))
@@ -760,13 +932,22 @@ class LmEngine:
         for s, e in zip(slots, ends):
             self.kv_pool.hold(int(s), e, e)  # no slot of this call is reclaimed for another
         reused, pieces = [], []
+        pool = self.kv_pool
         for p, s in zip(host, slots):  # every prefix is mapped before any page is allocated: the pages the slots
             s = int(s)                 # held before (maybe shared among them) are released first
             best, donor = self._donor(p, s, busy)
-            if donor != s:
-                self.kv_pool.share(s, donor, kv_pages_for(best))
+            if isinstance(donor, CachedRow):
+                pool.share(s, donor.row, kv_pages_for(best))
+                pool.touch(donor)
+                pool.held.add(donor)
+                pool.hits += 1
+            elif donor != s:
+                pool.share(s, donor, kv_pages_for(best))
             reused.append(best)
-        self._reserve([(int(s), e, b) for s, e, b in zip(slots, ends, reused)])
+        try:
+            self._reserve([(int(s), e, b) for s, e, b in zip(slots, ends, reused)])
+        finally:
+            pool.held.clear()
         for p, b in zip(prompts, reused):
             pieces.append(p[:, b:])
         defer = dict(defer_first_frame=True) if defer_first_frame else {}

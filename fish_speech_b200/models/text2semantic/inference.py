@@ -46,7 +46,8 @@ def _as_float(v) -> float:
 def _ensure_engine(model: DualARTransformer, batch: int = 1):
     if model.engine is None or model.max_batch_size < batch:
         model.setup_caches(max_batch_size=max(batch, max(model.max_batch_size, 1)),
-                           max_seq_len=model.config.max_seq_len, dtype=model.dtype)
+                           max_seq_len=model.config.max_seq_len, dtype=model.dtype,
+                           prefix_cache=getattr(model, "prefix_cache", False))
         model._cache_setup_done = True
     return model.engine
 
@@ -722,6 +723,17 @@ def serve_fused_admit(value: Optional[str]) -> bool:
     return True
 
 
+def serve_prefix_cache(value: Optional[str]) -> bool:
+    """FSB_SERVE_PREFIX_CACHE: 1 = the prompt pages of a finished request stay in the KV page pool as a prefix later
+    requests reuse, until the pool needs them (setup_caches(prefix_cache=)); unset, empty or 0 = off. A ValueError
+    naming FSB_SERVE_PREFIX_CACHE for any other value."""
+    if value is None or value.strip() in ("", "0"):
+        return False
+    if value.strip() != "1":
+        raise ValueError(f"FSB_SERVE_PREFIX_CACHE={value!r} must be 0 or 1")
+    return True
+
+
 def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool = False):
     """inference.py:736-799: the model lives in ONE daemon worker thread fed by a queue; `None` shuts
     it down; errors are returned as WrappedGenerateResponse(status="error", response=exc).
@@ -742,10 +754,15 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
     decodes only the rows they occupy: an engine of 33..64 slots runs its faster 32-row frame while load fits in 32.
     FSB_SERVE_FUSED_ADMIT=1 (0 or unset = off; else a ValueError naming it) runs an admitted request's first frame in
     the next decode frame, beside the running requests, instead of a frame that streams the head and fast weights for
-    the new rows alone; the tokens are the same."""
+    the new rows alone; the tokens are the same.
+    FSB_SERVE_PREFIX_CACHE=1 (0 or unset = off; else a ValueError naming it), for the one-at-a-time loop and the slot
+    scheduler alike, keeps the prompt pages of a finished request in the KV page pool, so that the next request with
+    the same voice prefix prefills only the rows after it; the cache holds only pages no request needs and gives them
+    back when a reservation does. The tokens are the same."""
     serve_kv_grow(os.environ.get("FSB_SERVE_KV_GROW"), os.environ.get("FSB_SERVE_KV_GB"))
     serve_compact(os.environ.get("FSB_SERVE_COMPACT"))
     serve_fused_admit(os.environ.get("FSB_SERVE_FUSED_ADMIT"))
+    cache = serve_prefix_cache(os.environ.get("FSB_SERVE_PREFIX_CACHE"))
     input_queue = queue.Queue()
     init_event = threading.Event()
     init_error: list = []
@@ -764,11 +781,12 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
                     free = torch.cuda.mem_get_info(torch.device(device))[0] if cuda else float("inf")
                     pages = serve_kv_pool_pages(float(gb), model.config, free)
                     model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype, kv_pages=pages,
-                                       attn_split=split)
+                                       attn_split=split, prefix_cache=cache)
                 else:
                     if cuda:
                         check_serve_kv_fits(slots, kv, model.config, torch.cuda.mem_get_info(torch.device(device))[0])
-                    model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype, attn_split=split)
+                    model.setup_caches(max_batch_size=slots, max_seq_len=kv, dtype=model.dtype, attn_split=split,
+                                       prefix_cache=cache)
             except Exception as e:
                 init_error.append(e)
                 init_event.set()
@@ -776,7 +794,8 @@ def launch_thread_safe_queue(checkpoint_path, device, precision, compile: bool =
             init_event.set()
             serve_requests(model, input_queue, slots)
             return
-        model.setup_caches(max_batch_size=1, max_seq_len=model.config.max_seq_len, dtype=model.dtype)
+        model.setup_caches(max_batch_size=1, max_seq_len=model.config.max_seq_len, dtype=model.dtype,
+                           prefix_cache=cache)
         init_event.set()
         while True:
             item: Optional[GenerateRequest] = input_queue.get()

@@ -210,6 +210,7 @@ class DualARTransformer:
         self.max_seq_len = -1
         self.kv_pages: Optional[int] = None
         self.attn_split = 0
+        self.prefix_cache = False
         self._cache_setup_done = False
         self.debug = False
         self.max_rows = 2048
@@ -231,14 +232,16 @@ class DualARTransformer:
         return self
 
     def setup_caches(self, max_batch_size: int, max_seq_len: int, dtype: torch.dtype = torch.bfloat16,
-                     kv_pages: Optional[int] = None, attn_split: int = 0):
+                     kv_pages: Optional[int] = None, attn_split: int = 0, prefix_cache: bool = False):
         """llama.py:307-325 — (re)create the engine when more capacity is asked for. `kv_pages`: the slow KV
         cache's page pool (64 positions per page) when it should be smaller than every slot at full capacity.
         `attn_split`: 0 = off; else decode rows with a longer context split their attention into spans of that many
-        positions (LmEngine)."""
+        positions (LmEngine). `prefix_cache`: prompt prefixes stay in the page pool after their slot moves on, for
+        later requests to reuse (LmEngine)."""
         attn_split = int(attn_split or 0)
+        prefix_cache = bool(prefix_cache)
         if (self.max_seq_len >= max_seq_len and self.max_batch_size >= max_batch_size
-                and kv_pages == self.kv_pages and attn_split == self.attn_split):
+                and kv_pages == self.kv_pages and attn_split == self.attn_split and prefix_cache == self.prefix_cache):
             return
         max_seq_len = find_multiple(max_seq_len, 8)
         if self.engine is not None:
@@ -246,10 +249,11 @@ class DualARTransformer:
         im_end = self.tokenizer.get_token_id(IM_END_TOKEN)
         self.engine = LmEngine(self.config, self._state, self.device, im_end, max_batch=max_batch_size,
                                kv_len=max_seq_len, max_rows=self.max_rows, debug=self.debug, kv_pages=kv_pages,
-                               attn_split=attn_split)
+                               attn_split=attn_split, prefix_cache=prefix_cache)
         self.max_seq_len = max_seq_len
         self.kv_pages = kv_pages
         self.attn_split = attn_split
+        self.prefix_cache = prefix_cache
         self.max_batch_size = max_batch_size
 
     @staticmethod

@@ -469,8 +469,9 @@ class ContinuousBatcher:
             req.on_done(req)
         return True
 
-    def _vacate(self, reqs: list):
-        """The slots of `reqs` idle from the next frame on; their pages stay mapped as a reusable prefix."""
+    def _vacate(self, reqs: list, cache: bool = True):
+        """The slots of `reqs` idle from the next frame on; their pages stay mapped as a reusable prefix (with the
+        engine's prefix cache: their prompts' pages are cached, unless `cache` is False)."""
         idx = torch.tensor([r.slot for r in reqs], dtype=torch.long, device=self._state.device)
         self._state[idx] = 0
         self._pos[idx] = -1  # parked: the decode frames neither attend for this row nor touch its K/V (which a
@@ -479,8 +480,12 @@ class ContinuousBatcher:
             del self.active[r.slot]
             del self._len[r.slot]
             self._pending.discard(r.slot)  # a first frame still pending is dropped with the slot's state
-            if hasattr(self.eng, "retire_slot"):
+            if not hasattr(self.eng, "retire_slot"):
+                continue
+            if cache:
                 self.eng.retire_slot(r.slot)  # its pages stay a reusable prefix until the pool needs them
+            else:
+                self.eng.retire_slot(r.slot, cache=False)  # its tokens are void: its prompt is not cached
 
     def _admit(self, order: Optional[list] = None):
         """Admit the requests of `order` (from `waiting`; default: as they arrived), in that order, into free slots."""
@@ -604,7 +609,7 @@ class ContinuousBatcher:
             r.error = RuntimeError(f"slot {r.slot}: decode attention met an unmapped KV page at position "
                                    f"{int(miss[r.slot]) - 1}; the request's tokens are void")
         self._miss[torch.tensor([r.slot for r in bad], dtype=torch.long, device=self._miss.device)] = 0
-        self._vacate(bad)
+        self._vacate(bad, cache=False)
         for r in bad:
             r.done.set()
             if r.on_done is not None:
